@@ -2,7 +2,8 @@
 """
 bench.py — hours-of-audio/sec, Fbank-80 @ 16 kHz (25 ms / 10 ms, N = 512), batches of 10 s cuts.
 
-    python bench.py --gpus N --steps K --warmup W            # the B200 path (this repository)
+    python bench.py --gpus N --steps K --warmup W            # the H100 path (this repository)
+    python bench.py --steps K --warmup W --dump-outputs DIR  # + what the timed path computed, as DIR/<name>.npy
     python bench.py --impl reference --steps K --warmup W    # the reference's own CPU extractor on the host cores
 
 One "step" = `launches_per_step` passes of the hot path, each one fused kernel launch over a device-resident ragged batch
@@ -12,7 +13,8 @@ throttle reasons are sampled under sustained load).
   value    : whole-job hours-of-audio/s with inputs resident in HBM (CUDA events, max over ranks)
   e2e      : the same metric through the public API (`B200Fbank.extract_batch` on numpy arrays in pinned host memory ->
              numpy features; H2D + kernel + D2H inside the timed region), >= 1 s timed
-  roofline : algorithmic bytes of one launch / its mean duration (CUDA events) vs the measured HBM peak
+  roofline : algorithmic bytes of one launch / its mean duration (CUDA events) vs the HBM peak (MEASURED_PEAKS.json when
+             present, else the H100 SXM data-sheet 3.35 TB/s)
   extra    : secondary figures with their own CUDA-event timings (MFCC 13/23, N = 400, int16 staging e2e, the reference's
              torch op chain on the same GPU, the CutSet-level sharded store of BASELINE configs[4] at bench size)
   cpu_baseline / clocks / gpu_launches : see DESIGN.md "Measurement"
@@ -135,17 +137,18 @@ def bounded_cuts_per_worker(requested, cut_seconds_cpu, target_s=1.5):
 
 def cpu_what(kind):
     if kind == "reference":
-        return "lhotse.features.kaldi.extractors.Fbank.extract of the UNMODIFIED reference (oracle/_ref archive or /root/reference)"
+        return "lhotse.features.kaldi.extractors.Fbank.extract of the UNMODIFIED reference (oracle/_ref archive or LHOTSE_REFERENCE_ROOT)"
     return "oracle/kaldi_oracle.py: the reference's torch-CPU op chain (the reference package is not on this box)"
 
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi sampled DURING the timed region: SM clock, power, throttle reasons, and the card's name and power limit
+    (an absolute rate means little without them)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit")
 
     def __init__(self, gpu_index):
         self.rows, self.proc, self.gpu = [], None, gpu_index
@@ -173,7 +176,7 @@ class ClockSampler:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, smax, reasons, power = [], None, set(), []
+        sm, smax, reasons, power, gpu_name, plimit = [], None, set(), [], None, None
         for r in self.rows:
             try:
                 sm.append(float(r[1])); smax = float(r[2]); power.append(float(r[3]))
@@ -182,7 +185,12 @@ class ClockSampler:
                         reasons.add(name)
             except Exception:
                 pass
-        return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": smax,
+            try:  # a board may report either as "[N/A]": the clock samples above stand on their own
+                gpu_name = r[9]
+                plimit = float(r[10])
+            except Exception:
+                pass
+        return {"gpu": gpu_name, "power_limit_w": plimit, "sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": smax,
                 "power_w_max": max(power) if power else None, "samples": len(sm), "reasons": sorted(reasons)}
 
 
@@ -191,7 +199,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measurement"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -273,6 +281,26 @@ def _calibrate(torch, eng, x, lens, offs, target_ms):
     torch.cuda.synchronize()
     per = e0.elapsed_time(e1) / 8
     return max(1, int(target_ms / max(per, 1e-3) + 0.999))
+
+
+DUMP_ROWS = 8192  # rows of every dumped feature matrix: a fixed, seeded sample keeps a dump far below 64 MB
+DUMP_CUTS = 8     # cuts of the e2e result
+
+
+def dump_outputs(directory, torch, np, outs, last_bufs, feats):
+    """Writes what the timed paths computed in their last step as DIR/<name>.npy (float32), plus the sampled row / cut
+    indices (float64): `fbank_buf<k>` = rows of the device-resident output of input buffer k (every buffer the last timed
+    step wrote), `e2e_feats` = cuts of the last `extract_batch` result."""
+    os.makedirs(directory, exist_ok=True)
+    rows = outs[0].shape[0]
+    idx = np.sort(np.random.RandomState(0).choice(rows, size=min(rows, DUMP_ROWS), replace=False))
+    idx_dev = torch.from_numpy(idx).to(outs[0].device)
+    np.save(os.path.join(directory, "fbank_rows.npy"), idx.astype(np.float64))
+    for k in last_bufs:
+        np.save(os.path.join(directory, f"fbank_buf{k}.npy"), outs[k].index_select(0, idx_dev).cpu().numpy().astype(np.float32))
+    cuts = np.sort(np.random.RandomState(1).choice(feats.shape[0], size=min(feats.shape[0], DUMP_CUTS), replace=False))
+    np.save(os.path.join(directory, "e2e_cuts.npy"), cuts.astype(np.float64))
+    np.save(os.path.join(directory, "e2e_feats.npy"), np.ascontiguousarray(feats[cuts], dtype=np.float32))
 
 
 def run_b200(args):
@@ -368,6 +396,8 @@ def run_b200(args):
     e2e_value = world * (Be * nsamp / SR / 3600.0) * args.e2e_calls * args.e2e_steps / e2e_max
     d2h_bytes = int(feats.size) * 4 * args.e2e_calls
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:  # the launches of the last timed step wrote the buffers j % len(xs), j < NL
+        dump_outputs(args.dump_outputs, torch, np, outs, sorted({j % len(xs) for j in range(NL)}), feats)
 
     extra = {}
     if not args.no_extra:
@@ -377,15 +407,6 @@ def run_b200(args):
         peak, peak_src = measured_peak()
         kern_ms = statistics.mean(per_step_ms) / NL
         achieved = frames * BYTES_PER_FRAME / (kern_ms / 1000.0) / 1e9
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath):
-            try:
-                tj = json.load(open(tpath))
-                if tj.get("kernel") == eng.kernel and tj.get("frames"):
-                    traffic = tj["dram_bytes"] * frames / tj["frames"]
-            except Exception:
-                traffic = None
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": elapsed_max_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -393,14 +414,14 @@ def run_b200(args):
             "config": {"workload": f"Fbank-80 16kHz 25ms/10ms N=512 (L=400,S=160), {NL} launches x {B} x {args.cut_seconds:g}s cuts per GPU per step (BASELINE configs[1])",
                        "cuts_per_gpu_per_launch": B, "launches_per_step": NL, "frames_per_gpu_per_launch": frames, "kernel": eng.kernel,
                        "parallelism": f"dp{world} (cuts sharded per rank, no data-path collective)",
-                       "l2_policy": f"{len(xs)} distinct input buffers of {B * nsamp * 4 / 2**20:.0f} MiB (+ {frames * 320 / 2**20:.0f} MiB of output each) visited round-robin: every launch's input >> 126 MiB L2",
+                       "l2_policy": f"{len(xs)} distinct input buffers of {B * nsamp * 4 / 2**20:.0f} MiB (+ {frames * 320 / 2**20:.0f} MiB of output each) visited round-robin: every launch's input >> 50 MiB L2",
                        "host_numa_node": numa_node},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": Be * nsamp * 4 * args.e2e_calls,
                     "d2h_bytes_per_step": d2h_bytes, "cuts_per_step": Be * args.e2e_calls, "steps": args.e2e_steps, "timed_s": e2e_max,
                     "api": "B200Fbank.extract_batch(numpy (B, n) float32 in pinned memory) -> numpy (B, T, 80); C ABI b200feat_extract_host underneath"},
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src, "kernel_ms": kern_ms,
+                         "peak_source": peak_src, "kernel_ms": kern_ms,
                          "algorithmic_bytes_per_launch": frames * BYTES_PER_FRAME,
                          "read_only_frac": frames * 640 / (kern_ms / 1000.0) / 1e9 / peak},
             "cpu_baseline": cpu_baseline,
@@ -541,6 +562,8 @@ def main():
     ap.add_argument("--no-extra", action="store_true")
     ap.add_argument("--no-cutset", action="store_true")
     ap.add_argument("--cutset-hours", type=float, default=4.0, help="hours of audio per rank in the CutSet-level job of `extra`")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the timed paths computed in their last step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,9 +1,9 @@
 /*
- * b200feat — C ABI of the B200-native (sm_100a) batched Kaldi-style feature extractor.
+ * b200feat — C ABI of the H100-native (sm_90a) batched Kaldi-style feature extractor.
  *
  * This header is the drop-in boundary for the ONE hot path this repository replaces:
  * lhotse's `FeatureExtractor.extract / extract_batch` for the Kaldi-compatible extractors
- * (reference citations are relative to the lhotse tree, `/root/reference` in the build image):
+ * (reference citations are relative to the reference lhotse tree):
  *
  *   - lhotse/features/base.py:37-222          FeatureExtractor ABC (extract, extract_batch)
  *   - lhotse/features/kaldi/extractors.py:67  Fbank        (.extract :92, .extract_batch :117)
@@ -45,7 +45,7 @@ extern "C" {
 #define B200FEAT_EINVAL (-1)      /* bad argument / inconsistent plan */
 #define B200FEAT_EUNSUPPORTED (-2) /* plan not supported by any kernel */
 #define B200FEAT_ECUDA (-3)       /* CUDA runtime error (message has the cudaError string) */
-#define B200FEAT_ENODEVICE (-4)   /* no CUDA device / not an sm_100 part */
+#define B200FEAT_ENODEVICE (-4)   /* no CUDA device / not an sm_90 part */
 #define B200FEAT_ESHORT (-5)      /* a cut is too short to be framed (reference raises too) */
 
 /* feature kinds — which reference module the plan mirrors */
@@ -85,7 +85,7 @@ extern "C" {
 #define B200FEAT_KERNEL_AUTO 0
 #define B200FEAT_KERNEL_GENERIC 1 /* any L/S/N, mixed-radix Stockham in shared memory */
 #define B200FEAT_KERNEL_FAST 2    /* register-resident rFFT: N = 512 (radix 16x16, one frame per half-warp) or N = 256 (16x8, per quarter-warp) */
-#define B200FEAT_KERNEL_TC 3      /* tensor cores: the N = 512 real DFT as two tcgen05.mma (3xTF32) GEMM stages, 16 frames per tile; fbank / mfcc */
+#define B200FEAT_KERNEL_TC 3      /* tensor cores: the N = 512 real DFT as two wgmma (3xTF32) GEMM stages, 8 frames per tile; fbank / mfcc */
 
 typedef struct b200feat_plan_desc {
   int32_t struct_size;  /* sizeof(b200feat_plan_desc) — ABI guard */

@@ -1,4 +1,4 @@
-"""lhotse_b200 — B200-native (sm_100a) batched Kaldi-style feature extraction behind lhotse's
+"""lhotse_b200 — H100-native (sm_90a) batched Kaldi-style feature extraction behind lhotse's
 ``FeatureExtractor`` API.  See DESIGN.md for the hot-path scope and INTEGRATION.md for the binding."""
 from .plan import EPSILON, LOG_EPSILON, FeaturePlan, build_plan  # noqa: F401
 from .extractors import (  # noqa: F401

@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA library (sm_100a only).  `python -m lhotse_b200.build`."""
+"""In-tree build of the CUDA library (sm_90a only).  `python -m lhotse_b200.build`."""
 from __future__ import annotations
 
 import os
@@ -13,7 +13,7 @@ SOURCES = ["b200feat.cu"]
 HEADERS = ["common.cuh", "generic.cuh", "fast512.cuh", "tc512.cuh", "fast256.cuh", "fast2048.cuh", "fast1024.cuh", "fast400.cuh", os.path.join("..", "..", "include", "b200feat.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-mavx2", "-shared",
     "-Xptxas", "-v",

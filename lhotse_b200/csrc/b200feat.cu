@@ -1,4 +1,4 @@
-// b200feat — host side of the C ABI (include/b200feat.h) + kernel dispatch.  sm_100a only.
+// b200feat — host side of the C ABI (include/b200feat.h) + kernel dispatch.  sm_90a only.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
@@ -128,7 +128,7 @@ struct b200feat_handle {
   DevPlan plan;
   int device = 0;
   int kernel = B200FEAT_KERNEL_GENERIC;
-  int sm_count = 148;
+  int sm_count = 132;
   int frames_per_tile = 1;
   int generic_warps = 4;
   size_t generic_smem = 0;
@@ -177,9 +177,8 @@ int upload(b200feat_handle *h, const T *src, size_t count, const T **dst) {
 
 std::vector<int> factorize(int n) {
   std::vector<int> f;
-  // radix 4 / 2 passes.  (A register radix-16 pass — a quarter of the shared-memory round trips — was measured in round 2 and
-  // changed nothing: N = 2048 98 vs 90-99 h/s, N = 512 slower; at one warp per frame and 8 warps per SM the generic kernel is
-  // bound by its instruction count and occupancy, not by the passes.  profiles/r2_bench_other_configs.jsonl)
+  // radix 4 / 2 passes.  (A register radix-16 pass — a quarter of the shared-memory round trips — did not pay: at one warp
+  // per frame and 8 warps per SM the generic kernel is bound by its instruction count and occupancy, not by the passes.)
   while (n % 4 == 0) { f.push_back(4); n /= 4; }
   while (n % 2 == 0) { f.push_back(2); n /= 2; }
   for (int p = 3; n > 1; p += 2)
@@ -250,10 +249,10 @@ int b200feat_create(const b200feat_plan_desc *desc, const float *window, const f
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess)
     return fail(nullptr, B200FEAT_ECUDA, "cudaGetDeviceProperties failed");
-  if (prop.major != 10)
+  if (prop.major != 9 || prop.minor != 0)
     return fail(nullptr, B200FEAT_ENODEVICE,
                 std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) +
-                    "; this library carries sm_100a code only");
+                    "; this library carries sm_90a code only");
 
   b200feat_handle *h = new b200feat_handle();
   h->desc = *desc;

@@ -1,4 +1,4 @@
-// Shared device/host definitions for the b200feat kernels (sm_100a).
+// Shared device/host definitions for the b200feat kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -125,6 +125,12 @@ __device__ __forceinline__ float fast_lg2_normal(float x) {
   return r;
 }
 __device__ __forceinline__ float fast_log_normal(float x) { return fast_lg2_normal(x) * 0.69314718055994530942f; }
+
+// Pre-emphasis and window of two adjacent taps: ((d.x - preemph * dp) * w.x, (d.y - preemph * d.x) * w.y), every
+// operation rounded on its own (no contraction of the product into a neighbouring add)
+__device__ __forceinline__ float2 preemph_window2(float2 d, float dp, float preemph, float2 w) {
+  return make_float2(__fmul_rn(__fmaf_rn(dp, -preemph, d.x), w.x), __fmul_rn(__fmaf_rn(d.x, -preemph, d.y), w.y));
+}
 
 // one bin of the log-spectrogram: lhotse log(P + 1e-15) (layers.py:467) or Kaldi/torchaudio log(max(P, eps32))
 __device__ __forceinline__ float log_spec_value(const DevPlan &p, float x) {

@@ -9,9 +9,8 @@
 //   stage 3  fast2048.cuh's in-lane split with Q = 128: lane owns k in {lane + 32j, 128 - (lane + 32j)}, j = 0, 1
 //   power spectra of SLOTS consecutive frames as P[slot][bin] (513 bins), mel bank as balanced 12-tap work items.
 //
-// It replaced the round-1 kernel (one half-warp per 512-point sub-FFT plus a radix-2 combination across the halves: 1352 / 1375 /
-// 1487 h/s at 24 kHz / 22.05 kHz / 16 kHz-64 ms, spilling in its run-time-length variant) at 1616 / 1635 / 1859 h/s
-// (profiles/r2_bench_fast1024.jsonl).  The stage functions are __host__ __device__
+// It replaced a kernel that ran one half-warp per 512-point sub-FFT plus a radix-2 combination across the halves (spilling in
+// its run-time-length variant).  The stage functions are __host__ __device__
 // (scripts/micro/f2k_host_check.cu).  Replaces the same reference code as fast512.cuh (lhotse/features/kaldi/layers.py:151-186,
 // :32-42, :565-578, :708-724, framing :727-772).
 #pragma once
@@ -249,7 +248,7 @@ b200feat_fast1024_kernel(const DevPlan p, const Fast1024Tables ft, const DevBatc
           if (j >= L) d.x = 0.f;
           if (j + 1 >= L) d.y = 0.f;
           if (p.raw_energy) e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
-          const float2 y = __fmul2_rn(__ffma2_rn(make_float2(dp, d.x), make_float2(-p.preemph, -p.preemph), d), wv);
+          const float2 y = preemph_window2(d, dp, p.preemph, wv);
           if (!p.raw_energy) e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
           v[n1] = y;
         } else {

@@ -32,17 +32,8 @@
 #define F2K_PIECE 12                       // taps per mel work item: 3 x 128-bit, an odd count spreads the pieces of a wide filter
                                            // over the 16-byte bank groups (simulated wavefronts per 2 frames: 318 vs 716 whole-filter)
 
-// complex product with a table twiddle: F2K_PMUL 1 issues it as FMUL2 + FFMA2 (2 issue slots instead of 4, same FP32-pipe time)
-#ifndef F2K_PMUL
-#define F2K_PMUL 0
-#endif
-F512_HD float2 f2k_mul(float2 a, float2 b) {
-#if F2K_PMUL && defined(__CUDA_ARCH__)
-  return __ffma2_rn(f2pi(a), make_float2(b.y, b.y), __fmul2_rn(a, make_float2(b.x, b.x)));
-#else
-  return f2mul(a, b);
-#endif
-}
+// complex product with a table twiddle
+F512_HD float2 f2k_mul(float2 a, float2 b) { return f2mul(a, b); }
 
 // ---- stage 1: v0 = column `lane`, v1 = column `lane + 32` of z[64*n1 + c]; tw1[k1*16 + n2] = W256^(n2*k1)
 F512_HD void f2k_stage1(int lane, float2 (&v0)[16], float2 (&v1)[16], const float2 *tw1, float2 *xa) {
@@ -341,7 +332,7 @@ b200feat_fast2048_kernel(const DevPlan p, const Fast2048Tables ft, const DevBatc
             if (j >= L) d.x = 0.f;
             if (j + 1 >= L) d.y = 0.f;
             if (p.raw_energy) e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
-            const float2 y = __fmul2_rn(__ffma2_rn(make_float2(dp, d.x), make_float2(-p.preemph, -p.preemph), d), wv);
+            const float2 y = preemph_window2(d, dp, p.preemph, wv);
             if (!p.raw_energy) e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
             if (c) v1[n1] = y; else v0[n1] = y;
           }
@@ -484,10 +475,11 @@ struct Fast2048Host {
 
 // launch shapes {warps per CTA, frames per warp}, one CTA per SM (the data alone is 64 registers per lane); prepare() takes
 // the first shape whose shared memory fits next to the plan's mel tables.  B200FEAT_FAST2048_VARIANT forces one.
-// Measured on a B200 (h audio/s, 24 kHz / 50 ms and 44.1 kHz / 25 ms, profiles/r2_bench_fast2048.jsonl):
-//   {11, 2} 735 / 725    {10, 2} 691 / 680    {8, 2} 595 / 492    {14, 1} 690 / 553    (generic kernel: 90 / 87)
-// Tried and dropped (profiles/README.md): loading the next frame into the dead data registers during stage 3 (-1..3 %), an L1
-// prefetch of the warp's next tile before the mel stage (-6 %), FMUL2 + FFMA2 twiddle products (+1 %).
+// Measured on an H100 SXM with a 400 W power limit (h audio/s, 24 kHz / 50 ms and 44.1 kHz / 25 ms, scripts/bench_fast2048.py;
+// profiles/h100_launch_shapes.jsonl):
+//   {11, 2} 595 / 587    {10, 2} 562 / 556    {8, 2} 499 / 490    {14, 1} 581 / 588
+// Tried and dropped: loading the next frame into the dead data registers during stage 3, an L1 prefetch of the warp's next tile
+// before the mel stage.
 struct F2kVariant { int warps, slots; };
 #define F2K_NUM_VARIANTS 4
 static const F2kVariant kF2kVariants[F2K_NUM_VARIANTS] = {{11, 2}, {10, 2}, {8, 2}, {14, 1}};

@@ -203,7 +203,7 @@ b200feat_fast256_kernel(const DevPlan p, const Fast256Tables ft, const DevBatch 
           if (j0 >= L) d.x = 0.f;
           if (j0 + 1 >= L) d.y = 0.f;
           if (p.raw_energy) e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
-          const float2 y = __fmul2_rn(__ffma2_rn(make_float2(dp, d.x), make_float2(-p.preemph, -p.preemph), d), w);
+          const float2 y = preemph_window2(d, dp, p.preemph, w);
           if (!p.raw_energy) e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
           v[n1] = y;
         } else {

@@ -50,10 +50,10 @@ __device__ __forceinline__ void dft5(float2 &x0, float2 &x1, float2 &x2, float2 
   constexpr float C1 = 0.30901699437494742410f, C2 = -0.80901699437494742410f;   // cos(2pi/5), cos(4pi/5)
   constexpr float S1 = 0.95105651629515357212f, S2 = 0.58778525229247312917f;    // sin(2pi/5), sin(4pi/5)
   const float2 s1 = f2add(x1, x4), d1 = f2sub(x1, x4), s2 = f2add(x2, x3), d2 = f2sub(x2, x3);
-  const float2 a1 = __ffma2_rn(s2, make_float2(C2, C2), __ffma2_rn(s1, make_float2(C1, C1), x0));
-  const float2 a2 = __ffma2_rn(s2, make_float2(C1, C1), __ffma2_rn(s1, make_float2(C2, C2), x0));
-  const float2 b1 = __ffma2_rn(d2, make_float2(S2, S2), __fmul2_rn(d1, make_float2(S1, S1)));
-  const float2 b2 = __ffma2_rn(d2, make_float2(-S1, -S1), __fmul2_rn(d1, make_float2(S2, S2)));
+  const float2 a1 = make_float2(__fmaf_rn(s2.x, C2, __fmaf_rn(s1.x, C1, x0.x)), __fmaf_rn(s2.y, C2, __fmaf_rn(s1.y, C1, x0.y)));
+  const float2 a2 = make_float2(__fmaf_rn(s2.x, C1, __fmaf_rn(s1.x, C2, x0.x)), __fmaf_rn(s2.y, C1, __fmaf_rn(s1.y, C2, x0.y)));
+  const float2 b1 = make_float2(__fmaf_rn(d2.x, S2, __fmul_rn(d1.x, S1)), __fmaf_rn(d2.y, S2, __fmul_rn(d1.y, S1)));
+  const float2 b2 = make_float2(__fmaf_rn(d2.x, -S1, __fmul_rn(d1.x, S2)), __fmaf_rn(d2.y, -S1, __fmul_rn(d1.y, S2)));
   x0 = f2add(x0, f2add(s1, s2));
   x1 = f2add(a1, f2mi(b1));  // a1 - i*b1
   x4 = f2add(a1, f2pi(b1));  // a1 + i*b1
@@ -212,7 +212,7 @@ b200feat_fast400_kernel(const DevPlan p, const Fast400Tables ft, const DevBatch 
           const float2 d = f2add(x, make_float2(-mu, -mu));
           const float dp = xp - mu;
           if (p.raw_energy) e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
-          const float2 y = __fmul2_rn(__ffma2_rn(make_float2(dp, d.x), make_float2(-p.preemph, -p.preemph), d), w);
+          const float2 y = preemph_window2(d, dp, p.preemph, w);
           if (!p.raw_energy) e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
           v[bb] = y;
           m += 8;
@@ -226,7 +226,7 @@ b200feat_fast400_kernel(const DevPlan p, const Fast400Tables ft, const DevBatch 
           const float2 w = s_win[bb * 8 + l];
           const float2 d = f2add(x, make_float2(-mu, -mu));
           if (p.raw_energy) e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
-          const float2 y = __fmul2_rn(d, w);
+          const float2 y = make_float2(__fmul_rn(d.x, w.x), __fmul_rn(d.y, w.y));
           if (!p.raw_energy) e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
           v[bb] = y;
           m += 8;

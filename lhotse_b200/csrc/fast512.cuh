@@ -59,23 +59,18 @@ __device__ __forceinline__ unsigned f512_smem_u32(const void *p) { return (unsig
 // (F512_HD: the pure arithmetic helpers also compile for the host, where scripts/micro/f2k_host_check.cu runs the FFT
 // stages of fast2048.cuh lane by lane against a float64 DFT)
 #define F512_HD __host__ __device__ __forceinline__
-// Complex arithmetic on the (re, im) register pair with sm_100 packed-FP32 instructions.  SASS FADD2/FMUL2/FFMA2
-// take operand modifiers that swap the halves and flip one sign (`R.F32x2.LO_HI.NP`), so multiplying by -i / +i is
-// free inside the consuming add, and a complex multiply is FMUL2 + FFMA2 (2 issue slots instead of 4).  The FP32-pipe
-// time is unchanged (a packed op occupies it for two cycles); what halves is the number of issue slots.
-#ifndef F512_PACKED
-#define F512_PACKED 1
-#endif
+// Complex arithmetic on the (re, im) register pair.  On the device the complex adds are explicitly rounded
+// (__fadd_rn): the compiler never fuses a preceding product into them, so every stage rounds where the code says.
 F512_HD float2 f2add(float2 a, float2 b) {
-#if F512_PACKED && defined(__CUDA_ARCH__)
-  return __fadd2_rn(a, b);
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 #else
   return make_float2(a.x + b.x, a.y + b.y);
 #endif
 }
 F512_HD float2 f2sub(float2 a, float2 b) {
-#if F512_PACKED && defined(__CUDA_ARCH__)
-  return __fadd2_rn(a, make_float2(-b.x, -b.y));
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fadd_rn(a.x, -b.x), __fadd_rn(a.y, -b.y));
 #else
   return make_float2(a.x - b.x, a.y - b.y);
 #endif
@@ -83,18 +78,11 @@ F512_HD float2 f2sub(float2 a, float2 b) {
 F512_HD float2 f2mi(float2 a) { return make_float2(a.y, -a.x); }   // a * (-i)
 F512_HD float2 f2pi(float2 a) { return make_float2(-a.y, a.x); }   // a * (+i)
 F512_HD float2 f2conj(float2 a) { return make_float2(a.x, -a.y); }
-#ifndef F512_PACKED_MUL
-#define F512_PACKED_MUL 0
-#endif
 F512_HD float2 f2mul(float2 a, float2 b) {  // complex product a * b
-#if F512_PACKED_MUL && defined(__CUDA_ARCH__)
-  return __ffma2_rn(f2pi(a), make_float2(b.y, b.y), __fmul2_rn(a, make_float2(b.x, b.x)));
-#else
   return make_float2(fmaf(a.x, b.x, -a.y * b.y), fmaf(a.x, b.y, a.y * b.x));
-#endif
 }
 
-// forward 4-point DFT, in place, natural order: 8 complex adds (the two rotations by -/+ i ride on operand modifiers)
+// forward 4-point DFT, in place, natural order: 8 complex adds (the two rotations by -/+ i are swaps and sign flips folded into them)
 F512_HD void dft4(float2 &a0, float2 &a1, float2 &a2, float2 &a3) {
   const float2 s02 = f2add(a0, a2), d02 = f2sub(a0, a2);
   const float2 s13 = f2add(a1, a3), d13 = f2sub(a1, a3);
@@ -108,24 +96,22 @@ F512_HD void dft4(float2 &a0, float2 &a1, float2 &a2, float2 &a3) {
 #define F512_S1 0.38268343236508977f  // sin(pi/8)
 #define F512_R2 0.70710678118654752f  // sqrt(1/2)
 
-// Multiplications by the eighth roots of unity W8^1 = (1 - i)/sqrt2 and W8^3 = -(1 + i)/sqrt2: a*(1 -+ i) is ONE packed add
-// with a rotated operand (a + (-i)a resp. a + (+i)a, the rotation rides on the FADD2 operand modifiers) and the scale is
-// ONE packed multiply: 2 issue slots instead of the 4 (2 FMUL + 2 FFMA) of a general complex product.
-#ifndef F512_R2TRICK
-#define F512_R2TRICK 1
-#endif
+// Multiplications by the eighth roots of unity W8^1 = (1 - i)/sqrt2 and W8^3 = -(1 + i)/sqrt2: a*(1 -+ i) is one complex
+// add with a rotated operand (a + (-i)a resp. a + (+i)a) followed by one real scale.
 F512_HD float2 f2mul_w8_1(float2 a) {
-#if F512_R2TRICK && F512_PACKED && defined(__CUDA_ARCH__)
-  return __fmul2_rn(f2add(a, f2mi(a)), make_float2(F512_R2, F512_R2));
+  const float2 s = f2add(a, f2mi(a));
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fmul_rn(s.x, F512_R2), __fmul_rn(s.y, F512_R2));
 #else
-  return f2mul(a, make_float2(F512_R2, -F512_R2));
+  return make_float2(s.x * F512_R2, s.y * F512_R2);
 #endif
 }
 F512_HD float2 f2mul_w8_3(float2 a) {
-#if F512_R2TRICK && F512_PACKED && defined(__CUDA_ARCH__)
-  return __fmul2_rn(f2add(a, f2pi(a)), make_float2(-F512_R2, -F512_R2));
+  const float2 s = f2add(a, f2pi(a));
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fmul_rn(s.x, -F512_R2), __fmul_rn(s.y, -F512_R2));
 #else
-  return f2mul(a, make_float2(-F512_R2, -F512_R2));
+  return make_float2(s.x * -F512_R2, s.y * -F512_R2);
 #endif
 }
 
@@ -253,8 +239,8 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
   for (int64_t tg = blockIdx.x; tg < b.num_tiles; tg += gridDim.x) {
     const int64_t tile = b.tile_base + tg;
     const int cut = __ldg(b.tile_cut + tile) - b.batch_first;  // host-built tile->cut table: one load, no search
-    // (fetching the next tile's cut one tile ahead and prefetching its four table rows into L1 before the mel stage was measured
-    // in round 2: 3518 vs 3544 h/s — the two-load chain of this prologue is already hidden by the other warps)
+    // (fetching the next tile's cut one tile ahead and prefetching its four table rows into L1 before the mel stage did not pay:
+    // the two-load chain of this prologue is already hidden by the other warps)
     const int64_t t0 = (tile - __ldg(b.tile_off + cut)) * TILE + (int64_t)hw * SLOTS;
     const int64_t T = __ldg(b.row_off + cut + 1) - __ldg(b.row_off + cut);
     const int64_t rows_here = b.out_mode == B200FEAT_OUT_PADDED ? b.max_frames : T;
@@ -376,11 +362,7 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
           if (j0 >= L) d.x = 0.f;
           if (j0 + 1 >= L) d.y = 0.f;
           if (p.raw_energy) e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
-#if F512_PACKED
-          const float2 y = __fmul2_rn(__ffma2_rn(make_float2(dp, d.x), make_float2(-p.preemph, -p.preemph), d), w);
-#else
-          const float2 y = make_float2(fmaf(-p.preemph, dp, d.x) * w.x, fmaf(-p.preemph, d.x, d.y) * w.y);
-#endif
+          const float2 y = preemph_window2(d, dp, p.preemph, w);
           if (!p.raw_energy) e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
           v[n1] = y;
         } else {
@@ -552,12 +534,10 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
 }
 
 // ---------------------------------------------------------------------------------------------- host
-// Launch shapes measured in round 1 on the headline workload (h audio/s, profiles/README.md):
-//   {8 warps, 4 slots, twiddles in registers, 2 CTAs/SM}  3427   <- variant 0, what ships
-//   {8, 4, twiddles in shared memory, 2}                  3272
-//   {10, 2, shared, 2}  (20 warps/SM, 96 registers)       3184
-//   {8, 2, registers, 2}                                  2948   (the 2-frame P tile makes the mel loop 14 % of the loss)
-//   {6, 2, shared, 3}   (18 warps/SM)                     2912
+// Launch shapes on the headline workload (bench.py, h audio/s, H100 SXM with a 400 W power limit,
+// profiles/h100_launch_shapes.jsonl, two alternating runs each):
+//   {8 warps, 4 slots, twiddles in registers, 2 CTAs/SM}  2355 / 2338   <- variant 0, what ships
+//   {10, 2, shared, 2}  (20 warps/SM, 96 registers)       2267 / 2262
 // Only variants 0 and 2 stay instantiated; B200FEAT_FAST_VARIANT=2 selects the high-occupancy shape for A/B runs.
 struct Fast512Variant { int warps, slots, tws, minb; };
 static const Fast512Variant kFast512Variants[] = {

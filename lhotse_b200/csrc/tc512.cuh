@@ -1,32 +1,34 @@
 // Tensor-core kernel for fft_length N = 512 (kernel = "tc"): the 512-point real DFT of every frame is a two-stage
-// Cooley-Tukey factorisation 512 = 32 x 16 whose two stages are GEMMs on the 5th-generation tensor cores
-// (tcgen05.mma.kind::tf32, accumulators in TMEM), made fp32-accurate by the 3xTF32 split
-//     A*B ~= A_hi*B_hi + (A_hi*B_lo + A_lo*B_hi),   x_hi = x & 0xffffe000,  x_lo = x - x_hi.
+// Cooley-Tukey factorisation 512 = 32 x 16 whose two stages are GEMMs on the Hopper tensor cores
+// (wgmma.mma_async .tf32, fp32 accumulators in registers), made fp32-accurate by the 3xTF32 split
+//     A*B ~= A_hi*B_hi + (A_hi*B_lo + A_lo*B_hi),   x_hi = rna_tf32(x),  x_lo = rna_tf32(x - x_hi).
 //
 //   sample n = 16*n1 + n2 of the pre-processed frame v (n1 = 0..31, zero for n >= L; n2 = 0..15), bin k = k1 + 32*k2:
 //     stage 1   Y[n2][k1]  = sum_n1 v[16 n1 + n2] * W32^(n1 k1)          k1 = 0..16 (real input: the rest is the conjugate)
 //     twiddle   Y'[n2][k1] = Y[n2][k1] * W512^(n2 k1)                     (CUDA cores, between the two GEMMs)
 //     stage 2   X[k1 + 32 k2] = sum_n2 Y'[n2][k1] * W16^(n2 k2)           k2 = 0..15; k2 >= 8 is conj X[512 - k]
 //
-//   GEMM 1:  D1[(frame, n2)][.] = A1[(frame, n2)][n1 = 0..31] * B1[n1][.]          128 rows = 8 frames
-//            A1 is the frame itself, an MN-major operand in the SWIZZLE_128B_BASE32B canonical layout (the only MN-major
-//            layout tcgen05 accepts for tf32): a K-row holds the 16 samples of n1 for TWO frames (128 B), 4 K-rows per
-//            512-byte atom, 32-byte granules XOR-swizzled with the K-row index — the pre-processing threads store float4
-//            chunks in sample order.  B1 columns: {Re Y0, Y16, Re Y1, Im Y1, ..., Re Y15, Im Y15} (Im Y0 = Im Y16 = 0).
-//   GEMM 2:  D2[(frame, k1)][.] = A2[(frame, k1 = 0..15)][(n2, re/im)] * B2[(n2, re/im)][(k2, re/im)]   (K-major, 128 B swizzle)
+//   GEMM 1:  D1[(frame, n2)][.] = A1[(frame, n2)][n1 = 0..31] * B1[n1][.]
+//            B1 columns: {Re Y0, Y16, Re Y1, Im Y1, ..., Re Y15, Im Y15} (Im Y0 = Im Y16 = 0).
+//   GEMM 2:  D2[(frame, k1)][.] = A2[(frame, k1 = 0..15)][(n2, re/im)] * B2[(n2, re/im)][(k2, re/im)]
 //            the k1 = 16 column (bins 16 + 32 k2, 8 of the 257) is a 16-tap real-input DFT done on CUDA cores.
-//   Per K-step two instructions: A_hi x [B_hi | B_lo] (N = 64: columns 0..31 hi*hi, 32..63 hi*lo) and A_lo x B_hi accumulated
-//   into columns 32..63; the consumer adds the two column groups.
+//   Per K-step two instructions: A_hi x [B_hi | B_lo] (N = 64: columns 0..31 hi*hi, 32..63 hi*lo) and A_lo x B_hi (N = 32,
+//   its own accumulator); the epilogue adds hi*hi + (hi*lo + lo*hi).
 //
-// One persistent CTA per SM, warp-specialised; a tile is 8 consecutive frames of one cut and flows through a ring of
-// double-buffered stages connected by mbarriers, so every stage works on a different tile at the same time:
-//   PRE    (warps 8-11)  global (next tile prefetched into registers) -> DC removal, pre-emphasis, window
-//                        (layers.py:151-186) -> hi / lo -> A1[b]
-//   ISSUE  (warp 16)     one thread: tcgen05.mma GEMM 1 of tile i+1, then GEMM 2 of tile i; tcgen05.commit -> mbarriers
-//   INTER  (warps 0-3)   tcgen05.ld D1[b] (thread = (frame, n2)) -> twiddle -> hi / lo -> A2[b] (swizzled STS.64), Y16[b]
-//   POWER  (warps 4-7)   tcgen05.ld D2[b] (thread = (frame, k1)) -> |X|^2 -> P[b][frame][bin] (layers.py:38-42) + the k1 = 16 bins
-//   MEL    (warps 12-15) lane = frame: every quarter-warp owns a set of filters, weights are broadcast operands
-//                        (layers.py:565-578) -> log -> staged tile -> coalesced rows (or DCT + lifter for MFCC, :708-724)
+// wgmma takes tf32 operands from shared memory only in K-major order, and the frame is MN-major for GEMM 1 (consecutive
+// samples are consecutive rows), so both A operands come from registers: every warp stages its frame (GEMM 1) or its
+// twiddled stage-1 output (GEMM 2) in shared memory and loads the m64k8 fragments from there, splitting hi / lo on the
+// way.  B1 and B2 (hi and lo) are K-major 128-byte-swizzled images in shared memory, fetched once per CTA by one bulk
+// asynchronous copy (TMA) completing on an mbarrier.
+//
+// A tile is 8 consecutive frames of one cut.  A CTA is two warpgroups; warpgroup w computes frames 4 w .. 4 w + 3 of every
+// tile of the CTA's contiguous tile range, one frame per warp: rows 16 q .. 16 q + 15 of an m64 operand belong to warp q,
+// so between the warpgroup-wide MMAs a warp only ever exchanges data with itself.  A warp's tile step:
+//   PRE    global (next tile's frame prefetched into registers) -> DC removal, pre-emphasis, window (layers.py:151-186) -> V
+//   GEMM 1 V -> A1 fragments -> D1 (registers) -> twiddle -> Y' (shared), Y16
+//   GEMM 2 Y' -> A2 fragments -> D2 -> |X|^2 -> P[bin] (layers.py:38-42) + the k1 = 16 bins from Y16
+//   MEL    lane = filter: P x mel weights (layers.py:565-578) -> log -> the output row (or DCT + lifter for MFCC, :708-724)
+// Several CTAs share an SM, so one warpgroup's global loads and MMAs overlap another's CUDA-core work.
 // HBM traffic: 4*S bytes in (the frame overlap is served by L1/L2), 4*F bytes out per frame; no intermediate leaves the SM.
 #pragma once
 #include <string.h>
@@ -37,14 +39,11 @@
 #include "common.cuh"
 
 #define TC_NF 8                      // frames per tile
-#define TC_THREADS 544               // 17 warps
-#define TC_PP 260                    // floats per P row (= 4 mod 32: the frame-lanes of a 128-bit P load hit disjoint banks)
-// shared memory map (bytes); A buffers need 1024-byte alignment (128-byte swizzle atoms)
-#define TC_OFF_A1 0                  // [2][hi 16 KB | lo 16 KB]: 4 frame pairs x 4 KB each
-#define TC_OFF_A2 (64 * 1024)        // [2][hi 16 KB | lo 16 KB]: 128 rows x 128 B
-#define TC_OFF_CONST (128 * 1024)    // constant blob: B1 hi/lo, B2 hi/lo (4 KB each), twiddles, mel tables
-#define TC_HALF (16 * 1024)
-#define TC_TMEM_COLS 256             // D1[2] at columns 0 / 64, D2[2] at 128 / 192 (64 columns each: [hi*hi | cross terms])
+#define TC_THREADS 256               // two warpgroups, one frame per warp
+#define TC_PP 260                    // floats per P row (257 bins + zeroed pad a 128-bit mel load may touch)
+#define TC_VS 24                     // floats per 16-sample row of a staged frame (16 + 8 pad: the A1 fragment loads of a
+                                     // warp hit 32 distinct banks)
+#define TC_YS 36                     // floats per k1 row of Y' (32 + 4 pad: the A2 fragment loads hit 32 distinct banks)
 
 struct Tc512Tables {
   const void *cblob;      // [B1hi 4K][B1lo 4K][B2hi 4K][B2lo 4K][tw 2K][mel descriptors][mel weights]
@@ -52,6 +51,7 @@ struct Tc512Tables {
   int off_tw, off_md, off_mw;  // byte offsets inside the blob
   int fpu;                // filters per unit = ceil(M / 16)
   int Mpad;               // M rounded up to 4
+  int warp_bytes;         // shared memory of one warp: V, Y', P, Y16, log-mel row
   const float *win4;      // [512] window, zero beyond L
   const float *c16;       // [16][16]: cos / -sin of 2 pi n2 (1 + 2 k2) / 32 at [2 k2 + part][n2] (the k1 = 16 column)
 };
@@ -59,78 +59,57 @@ struct Tc512Tables {
 __device__ __forceinline__ uint32_t tc_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // tf32 (10 explicit mantissa bits) nearest to x, in an fp32 container.  hi = rna(x) and lo = rna(x - hi) leave a
 // representation error of 2^-24 |x| (masking the low bits instead would leave 2^-22: the tensor core truncates whatever it is
-// given), which is what keeps bins 70 dB under a frame's peak inside the parity gate.
+// given), which keeps bins 70 dB under a frame's peak within the fp32 reference's tolerance.
 __device__ __forceinline__ float tc_hi(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return __uint_as_float(u);
 }
-
-// shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp: SmemDescriptor): start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 |
-// version 1 << 46 | layout << 61 (1 = SWIZZLE_128B_BASE32B, 2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t tc_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) |
-         (1ull << 46) | ((uint64_t)layout << 61);
+// hi / lo tf32 parts of four fragment elements
+__device__ __forceinline__ void tc_split4(const float (&x)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float h = tc_hi(x[i]);
+    hi[i] = __float_as_uint(h);
+    lo[i] = __float_as_uint(tc_hi(x[i] - h));
+  }
 }
-// instruction descriptor, kind::tf32, fp32 accumulate (InstrDescriptor): M = 128; bit 15 = A is MN-major
-#define TC_IDESC(a_mn, n) ((1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(a_mn) << 15) | (((uint32_t)(n) >> 3) << 17) | ((128u >> 4) << 24))
 
-__device__ __forceinline__ void tc_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0;\n"
-               "  tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p; }\n"
-               ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+// wgmma shared-memory matrix descriptor of a K-major operand in the 128-byte swizzle: start >> 4 | LBO (unused: 1) << 16 |
+// SBO (1024 B between 8-row groups) >> 4 << 32 | layout 1 (SWIZZLE_128B) << 62.  A K-step of 8 tf32 advances the start by 32 B.
+__device__ __forceinline__ uint64_t tc_desc_k128(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// m64nNk8 tf32 MMAs, A from registers (fragment of lane l in warp q: rows 16 q + l / 4 (+ 8), columns l % 4 (+ 4)),
+// fp32 accumulator d (lane l of warp q holds rows 16 q + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1))
+__device__ __forceinline__ void tc_wgmma_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %37, 0;\n"
+               "  wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1; }\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void tc_wgmma_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %21, 0;\n"
+               "  wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1; }\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void tc_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void tc_wgmma_commit_wait() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+// keeps the compiler from moving accesses of accumulator registers across the wgmma fence / wait above
+template <int N>
+__device__ __forceinline__ void tc_pin(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __device__ __forceinline__ void tc_wait(uint32_t bar, uint32_t parity) {
   unsigned done = 0;
   while (!done)
     asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
                  : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tc_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// 32 consecutive TMEM columns of this thread's lane (tcgen05.ld.32x32b.x32): warp w reads lanes 32 (w % 4) ...; no wait
-__device__ __forceinline__ void tc_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                 "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-                 "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-                 "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {  // single load + wait (the bring-up probes)
-  tc_ld32_nowait(taddr, r);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// accumulator row of this thread: columns [0, 32) + [32, 64) (hi*hi plus the two cross terms); both loads in flight together
-__device__ __forceinline__ void tc_ld_acc(uint32_t taddr, float (&v)[32]) {
-  uint32_t a[32], c[32];
-  tc_ld32_nowait(taddr, a);
-  tc_ld32_nowait(taddr + 32, c);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(a[i]) + __uint_as_float(c[i]);
-}
-
-// 16 consecutive TMEM columns (tcgen05.ld.32x32b.x16), no wait
-__device__ __forceinline__ void tc_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                 "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(taddr));
-}
-// half an accumulator row: columns [16 h, 16 h + 16) of the hi*hi group + the same columns of the cross-term group
-__device__ __forceinline__ void tc_ld_acc_half(uint32_t taddr, int h, float (&v)[16]) {
-  uint32_t a[16], c[16];
-  tc_ld16_nowait(taddr + 16 * h, a);
-  tc_ld16_nowait(taddr + 32 + 16 * h, c);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(a[i]) + __uint_as_float(c[i]);
 }
 
 template <int DT>
@@ -179,33 +158,24 @@ __device__ __forceinline__ TcTile tc_tile(const DevBatch &b, TcCut &m, int64_t t
   return t;
 }
 
-// barrier slots (8 bytes each) after the constant blob
-enum { TCB_CONST = 0, TCB_A1F = 1, TCB_D1F = 3, TCB_D1E = 5, TCB_A2F = 7, TCB_D2F = 9, TCB_D2E = 11, TCB_PF = 13, TCB_PE = 15, TCB_COUNT = 17 };
-
-// DBG == 1: the raw accumulators of the FIRST tile of block 0 go to `dbg` ([128][32] D1 | [128][32] D2 | [8][TC_PP] P)
-template <int DT, int DBG>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-b200feat_tc512_kernel(const DevPlan p, const Tc512Tables tt, const DevBatch b, float *dbg) {
-  extern __shared__ __align__(1024) unsigned char tc_smem[];
+template <int DT>
+__global__ void __launch_bounds__(TC_THREADS, 2)
+b200feat_tc512_kernel(const DevPlan p, const Tc512Tables tt, const DevBatch b) {
+  extern __shared__ unsigned char tc_smem_raw[];
+  // the swizzled B images need a 1024-byte-aligned base (the launch reserves the slack)
+  unsigned char *sC = tc_smem_raw + ((1024u - (tc_smem_u32(tc_smem_raw) & 1023u)) & 1023u);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  unsigned char *sC = tc_smem + TC_OFF_CONST;
-  unsigned long long *bars = reinterpret_cast<unsigned long long *>(sC + tt.cblob_bytes);
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + TCB_COUNT);
-  float *Pall = reinterpret_cast<float *>(bars + TCB_COUNT + 3);             // [2][8][TC_PP], 16-byte aligned
-  float *Y16 = Pall + 2 * TC_NF * TC_PP;                                     // [2][8][16]
-  float *Eall = Y16 + 2 * TC_NF * 16;                                        // [2][8][Mpad]
-  const uint32_t bar0 = tc_smem_u32(bars);
-#define TC_BAR(slot, buf) (bar0 + 8u * (uint32_t)((slot) + (buf)))
+  const int f = warp;                            // this warp's frame in every tile (warpgroup warp / 4 owns frames 4 (warp / 4) ..)
+  const int g = lane >> 2, tq = lane & 3;        // fragment row (and row + 8) / fragment column (and column + 4)
+  const uint32_t bar0 = tc_smem_u32(sC + tt.cblob_bytes);
+  float *V = reinterpret_cast<float *>(sC + tt.cblob_bytes + 16 + (size_t)warp * tt.warp_bytes);  // [32 n1][TC_VS]
+  float *Yp = V + 32 * TC_VS;                    // [16 k1][TC_YS]: (Re, Im) Y'[n2][k1] at 2 n2
+  float *Pf = Yp + 16 * TC_YS;                   // [TC_PP]
+  float *Y16 = Pf + TC_PP;                       // [16]
+  float *E = Y16 + 16;                           // [Mpad]
 
   if (tid == 0) {
-    auto init = [&](int slot, int count) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar0 + 8u * (uint32_t)slot), "r"(count));
-    };
-    init(TCB_CONST, 1);
-    for (int k = 0; k < 2; ++k) {
-      init(TCB_A1F + k, 128); init(TCB_D1F + k, 1); init(TCB_D1E + k, 128); init(TCB_A2F + k, 128);
-      init(TCB_D2F + k, 1); init(TCB_D2E + k, 128); init(TCB_PF + k, 128); init(TCB_PE + k, 128);
-    }
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -214,364 +184,238 @@ b200feat_tc512_kernel(const DevPlan p, const Tc512Tables tt, const DevBatch b, f
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(tc_smem_u32(sC)), "l"(tt.cblob), "r"(tt.cblob_bytes), "r"(bar0) : "memory");
   }
-  if (warp == 16) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(tmem_slot)), "n"(TC_TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   tc_wait(bar0, 0);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tm = *tmem_slot;
   const int64_t tile_begin = b.tile_base + b.num_tiles * (int64_t)blockIdx.x / gridDim.x;
   const int64_t my_tiles = b.tile_base + b.num_tiles * (int64_t)(blockIdx.x + 1) / gridDim.x - tile_begin;
-  // DBG == 2: lane 0 of every role's first warp adds {cycles waiting on mbarriers, cycles in its tile loop} to dbg[2 role ...]
-  long long t_wait = 0, t_loop = 0;
-#define TC_WAITM(bar, parity) do { if (DBG == 2 && lane == 0) { const long long c0_ = clock64(); tc_wait(bar, parity); t_wait += clock64() - c0_; } \
-                                   else tc_wait(bar, parity); } while (0)
-#define TC_ROLE_BEGIN() do { if (DBG == 2 && lane == 0) t_loop = clock64(); } while (0)
-#define TC_ROLE_END(role) do { if (DBG == 2 && lane == 0) { unsigned long long *g_ = reinterpret_cast<unsigned long long *>(dbg); \
-      atomicAdd(g_ + 2 * (role), (unsigned long long)t_wait); atomicAdd(g_ + 2 * (role) + 1, (unsigned long long)(clock64() - t_loop)); \
-      if ((role) == 0) atomicAdd(g_ + 15, (unsigned long long)my_tiles); } } while (0)
 
-  if (warp >= 8 && warp < 12) {
-    // ============================================================ PRE: frames 2 pw, 2 pw + 1 of every tile -> A1[buf]
-    const int pw = warp - 8;
-    const int L = p.L, NCH = (L + 3) >> 2;
-    float4 wreg[4];
-    uint32_t aoff[4];  // byte offset of chunk c = lane + 32 j inside its frame pair's 4 KB (without the granule term)
+  const uint32_t cb = tc_smem_u32(sC);
+  const float2 *s_tw = reinterpret_cast<const float2 *>(sC + tt.off_tw);  // [k1 - 1][n2]: W512^(n2 k1), k1 = 1..16
+  const int4 *s_md = reinterpret_cast<const int4 *>(sC + tt.off_md);      // [unit][slot] {first bin, float4 groups, weight index, filter}
+  const float4 *s_mw4 = reinterpret_cast<const float4 *>(sC + tt.off_mw);
+  const float lgk = p.log10_mel ? 0.30102999566398119521f : 0.69314718055994530942f;
+  const int L = p.L, NCH = (L + 3) >> 2;
+  const float inv_L = 1.0f / (float)L, pre = p.preemph;
+  const int pad = p.snip_edges ? 0 : p.pad_left;
+  float4 wreg[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) wreg[j] = __ldg(reinterpret_cast<const float4 *>(tt.win4) + lane + 32 * j);
+  const float4 *c16 = reinterpret_cast<const float4 *>(tt.c16) + (lane & 15) * 4;  // row o = lane % 16: 2 k2 + part, part 0 = Re (cos), 1 = Im (-sin)
+
+  float4 xn[4];
+  bool inn = false;
+  auto fetch = [&](const TcTile &t) {  // interior frames: 4 vector loads per lane, issued early; edge frames are gathered later
+    const int64_t sb = (t.t0 + f) * p.S - pad;
+    inn = f < t.nv && sb >= 0 && sb + 4 * NCH <= t.n && (((t.xoff + sb) & 3) == 0);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const int c = lane + 32 * j, n1 = c >> 2, q = c & 3;
-      wreg[j] = __ldg(reinterpret_cast<const float4 *>(tt.win4) + c);
-      aoff[j] = (uint32_t)((n1 >> 2) * 512 + (n1 & 3) * 128 + (q & 1) * 16);
+      const int c = lane + 32 * j;
+      xn[j] = (inn && c < NCH) ? tc_ld_chunk<DT>(b.samples, t.xoff + sb + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    const float inv_L = 1.0f / (float)L, pre = p.preemph;
-    const int pad = p.snip_edges ? 0 : p.pad_left;
-    float4 xn[2][4];
-    bool inn[2] = {false, false};
-    auto fetch = [&](const TcTile &t) {  // interior frames: 4 vector loads per lane, issued early; edge frames are gathered later
+  };
+  TcTile cur{};
+  TcCut cm{};
+  if (my_tiles > 0) { tc_first_cut(b, tile_begin, cm); cur = tc_tile(b, cm, tile_begin); fetch(cur); }
+  for (int64_t it = 0; it < my_tiles; ++it) {
+    float4 x[4];
 #pragma unroll
-      for (int ff = 0; ff < 2; ++ff) {
-        const int f = 2 * pw + ff;
-        const int64_t sb = (t.t0 + f) * p.S - pad;
-        inn[ff] = f < t.nv && sb >= 0 && sb + 4 * NCH <= t.n && (((t.xoff + sb) & 3) == 0);
+    for (int j = 0; j < 4; ++j) x[j] = xn[j];
+    const bool in = inn;
+    const TcTile t = cur;
+    if (it + 1 < my_tiles) { cur = tc_tile(b, cm, tile_begin + it + 1); fetch(cur); }  // next tile's samples fly while this one is processed
+
+    // ---------------------------------------------------------------- PRE: frame f -> V (missing frames: zeros)
+    if (f < t.nv && !in) {  // cut edge (or an unaligned cut): per-sample reflection (layers.py:753-772)
+      const int64_t sb = (t.t0 + f) * p.S - pad;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int c = lane + 32 * j;
-          xn[ff][j] = (inn[ff] && c < NCH) ? tc_ld_chunk<DT>(b.samples, t.xoff + sb + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-    };
-    TcTile cur{};
-    TcCut cm{};
-    if (my_tiles > 0) { tc_first_cut(b, tile_begin, cm); cur = tc_tile(b, cm, tile_begin); fetch(cur); }
-    if (pw == 0) TC_ROLE_BEGIN();
-    for (int64_t it = 0; it < my_tiles; ++it) {
-      const int buf = (int)(it & 1);
-      const uint32_t par = (uint32_t)((it >> 1) & 1);
-      float4 x[2][4];
-      bool in[2];
-#pragma unroll
-      for (int ff = 0; ff < 2; ++ff) {
-        in[ff] = inn[ff];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) x[ff][j] = xn[ff][j];
-      }
-      const TcTile t = cur;
-      if (it + 1 < my_tiles) { cur = tc_tile(b, cm, tile_begin + it + 1); fetch(cur); }  // next tile's samples fly while this one is processed
-      TC_WAITM(TC_BAR(TCB_D1F, buf), par ^ 1);  // GEMM 1 of tile it - 2 has consumed A1[buf]
-      unsigned char *sA = tc_smem + TC_OFF_A1 + buf * 2 * TC_HALF;
-#pragma unroll
-      for (int ff = 0; ff < 2; ++ff) {
-        const int f = 2 * pw + ff;
-        if (f >= t.nv) continue;  // rows of missing frames keep stale (finite or not: rows are independent) data
-        if (!in[ff]) {            // cut edge (or an unaligned cut): per-sample reflection (layers.py:753-772)
-          const int64_t sb = (t.t0 + f) * p.S - pad;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int c = lane + 32 * j;
-            float e[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int i = 4 * c + q;
-              e[q] = 0.f;
-              if (i < L) {
-                int64_t s = sb + i;
-                if (!p.snip_edges) s = reflect_index(s, t.n, p.pad_mode);
-                e[q] = ld_sample<DT>(b.samples, t.xoff + s);
-              }
-            }
-            x[ff][j] = make_float4(e[0], e[1], e[2], e[3]);
-          }
-        }
-        if (L & 3) {  // taps >= L inside the last chunk are not part of the frame
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int i0 = 4 * (lane + 32 * j);
-            if (i0 + 1 >= L) x[ff][j].y = 0.f;
-            if (i0 + 2 >= L) x[ff][j].z = 0.f;
-            if (i0 + 3 >= L) x[ff][j].w = 0.f;
-          }
-        }
-        // the tap before chunk c is the last tap of chunk c - 1: the neighbour lane's .w (lane 0: lane 31 of the round before)
-        float pv[4];
-        {
-          float last = x[ff][0].x;  // lane 0, chunk 0: replicate-left (layers.py:166)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float up = __shfl_up_sync(0xffffffffu, x[ff][j].w, 1);
-            pv[j] = lane == 0 ? last : up;
-            last = __shfl_sync(0xffffffffu, x[ff][j].w, 31);
-          }
-        }
-        float s = 0.f;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s += (x[ff][j].x + x[ff][j].y) + (x[ff][j].z + x[ff][j].w);
-        const float mu = p.remove_dc ? warp_sum(s) * inv_L : 0.f;
-        unsigned char *fr = sA + (f >> 1) * 4096;  // frame pair f / 2 owns 4 KB; frame f % 2 the granules 2 h, 2 h + 1 of every K-row
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float d0 = x[ff][j].x - mu, d1 = x[ff][j].y - mu, d2 = x[ff][j].z - mu, d3 = x[ff][j].w - mu, dp = pv[j] - mu;
-          float4 v;
-          v.x = fmaf(-pre, dp, d0) * wreg[j].x;
-          v.y = fmaf(-pre, d0, d1) * wreg[j].y;
-          v.z = fmaf(-pre, d1, d2) * wreg[j].z;
-          v.w = fmaf(-pre, d2, d3) * wreg[j].w;
-          const int c = lane + 32 * j, n1 = c >> 2, q = c & 3;
-          if (c >= NCH) v = make_float4(0.f, 0.f, 0.f, 0.f);  // K-rows beyond the frame are exact zeros
-          const float4 h = make_float4(tc_hi(v.x), tc_hi(v.y), tc_hi(v.z), tc_hi(v.w));
-          unsigned char *dst = fr + aoff[j] + (((((f & 1) << 1) | (q >> 1)) ^ (n1 & 3)) << 5);
-          *reinterpret_cast<float4 *>(dst) = h;
-          *reinterpret_cast<float4 *>(dst + TC_HALF) = make_float4(tc_hi(v.x - h.x), tc_hi(v.y - h.y), tc_hi(v.z - h.z), tc_hi(v.w - h.w));
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core's async proxy
-      tc_arrive(TC_BAR(TCB_A1F, buf));
-    }
-    if (pw == 0) TC_ROLE_END(2);
-  } else if (warp == 16) {
-    // ============================================================ ISSUE: GEMM 1 of tile it + 1 before GEMM 2 of tile it
-    if (lane == 0) {
-      const uint32_t a1 = tc_smem_u32(tc_smem + TC_OFF_A1), a2 = tc_smem_u32(tc_smem + TC_OFF_A2), cb = tc_smem_u32(sC);
-      auto gemm1 = [&](int64_t it) {
-        const int buf = (int)(it & 1);
-        const uint32_t par = (uint32_t)((it >> 1) & 1);
-        TC_WAITM(TC_BAR(TCB_A1F, buf), par);        // PRE has filled A1[buf]
-        TC_WAITM(TC_BAR(TCB_D1E, buf), par ^ 1);    // INTER has drained D1[buf] (tile it - 2)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t ahi = a1 + buf * 2 * TC_HALF, alo = ahi + TC_HALF, d = tm + 64 * buf;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          // MN-major: 32 rows (a frame pair) per 4 KB (LBO), 4 K-rows per 512-byte atom (SBO), K = 8 = two atoms per step
-          const uint64_t db = tc_desc(cb + ks * 32, 16, 1024, 2);                                   // rows 0..31 B1_hi, 32..63 B1_lo
-          tc_mma(d, tc_desc(ahi + ks * 1024, 4096, 512, 1), db, TC_IDESC(1, 64), ks ? 1u : 0u);      // [hi*hi | hi*lo]
-          tc_mma(d + 32, tc_desc(alo + ks * 1024, 4096, 512, 1), db, TC_IDESC(1, 32), 1u);           //          + lo*hi
-        }
-        tc_commit(TC_BAR(TCB_D1F, buf));
-      };
-      auto gemm2 = [&](int64_t it) {
-        const int buf = (int)(it & 1);
-        const uint32_t par = (uint32_t)((it >> 1) & 1);
-        TC_WAITM(TC_BAR(TCB_A2F, buf), par);        // INTER has filled A2[buf]
-        TC_WAITM(TC_BAR(TCB_D2E, buf), par ^ 1);    // POWER has drained D2[buf] (tile it - 2)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t ahi = a2 + buf * 2 * TC_HALF, alo = ahi + TC_HALF, d = tm + 128 + 64 * buf;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint64_t db = tc_desc(cb + 8192 + ks * 32, 16, 1024, 2);                             // rows 0..31 B2_hi, 32..63 B2_lo
-          tc_mma(d, tc_desc(ahi + ks * 32, 16, 1024, 2), db, TC_IDESC(0, 64), ks ? 1u : 0u);
-          tc_mma(d + 32, tc_desc(alo + ks * 32, 16, 1024, 2), db, TC_IDESC(0, 32), 1u);
-        }
-        tc_commit(TC_BAR(TCB_D2F, buf));
-      };
-      TC_ROLE_BEGIN();
-      if (my_tiles > 0) gemm1(0);
-      for (int64_t it = 0; it < my_tiles; ++it) {
-        if (it + 1 < my_tiles) gemm1(it + 1);
-        gemm2(it);
-      }
-      TC_ROLE_END(4);
-    }
-  } else if (warp < 4) {
-    // ============================================================ INTER: thread = (frame row / 16, n2 = row % 16)
-    const int row = warp * 32 + lane, fl = row >> 4, n2 = row & 15, ch = n2 >> 1;
-    const float2 *s_tw = reinterpret_cast<const float2 *>(sC + tt.off_tw);  // [k1 - 1][n2]: W512^(n2 k1), k1 = 1..16
-    const uint32_t tlane = tm + ((uint32_t)(warp * 32) << 16);
-    if (warp == 0) TC_ROLE_BEGIN();
-    for (int64_t it = 0; it < my_tiles; ++it) {
-      const int buf = (int)(it & 1);
-      const uint32_t par = (uint32_t)((it >> 1) & 1);
-      TC_WAITM(TC_BAR(TCB_D1F, buf), par);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      TC_WAITM(TC_BAR(TCB_D2E, buf), par ^ 1);  // POWER is done with D2[buf] / Y16[buf] of tile it - 2 => GEMM 2 has consumed A2[buf]
-      // rows r = 16 fl + k1: atom (r / 8) = 2 fl + (k1 >> 3), row in atom = k1 & 7; 16-byte chunk (n2 / 2) ^ (k1 & 7)
-      unsigned char *base = tc_smem + TC_OFF_A2 + buf * 2 * TC_HALF + fl * 2048 + (n2 & 1) * 8;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {  // columns of k1 = 8 h .. 8 h + 7 (two passes keep the live registers low)
-        float r[16];
-        tc_ld_acc_half(tlane + 64 * buf, h, r);
-        if (h == 1) {
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          tc_arrive(TC_BAR(TCB_D1E, buf));
-        }
-        if (DBG == 1 && blockIdx.x == 0 && it == 0) {
-#pragma unroll
-          for (int c = 0; c < 16; ++c) dbg[row * 32 + 16 * h + c] = r[c];
-        }
-        if (h == 0) Y16[(buf * TC_NF + fl) * 16 + n2] = r[1];  // the k1 = 16 column (real): finished by the POWER warps
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const int k1 = 8 * h + kk;
-          float yr, yi;
-          if (k1 == 0) { yr = r[0]; yi = 0.f; }
-          else {
-            const float a = r[2 * kk], bq = r[2 * kk + 1];
-            const float2 w = s_tw[(k1 - 1) * 16 + n2];
-            yr = fmaf(a, w.x, -bq * w.y);
-            yi = fmaf(a, w.y, bq * w.x);
-          }
-          const float hr = tc_hi(yr), hi_ = tc_hi(yi);
-          unsigned char *dst = base + h * 1024 + kk * 128 + ((ch ^ kk) << 4);
-          *reinterpret_cast<float2 *>(dst) = make_float2(hr, hi_);
-          *reinterpret_cast<float2 *>(dst + TC_HALF) = make_float2(tc_hi(yr - hr), tc_hi(yi - hi_));
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      tc_arrive(TC_BAR(TCB_A2F, buf));
-    }
-    if (warp == 0) TC_ROLE_END(0);
-  } else if (warp < 8) {
-    // ============================================================ POWER: thread = (frame row / 16, k1 = row % 16)
-    const int row = (warp - 4) * 32 + lane, fl = row >> 4, k1 = row & 15;
-    const uint32_t tlane = tm + ((uint32_t)((warp - 4) * 32) << 16);
-    float c16[16];  // this thread's share of the k1 = 16 column: output 2 k2 + part, part 0 = Re (cos), 1 = Im (-sin)
-#pragma unroll
-    for (int i = 0; i < 16; ++i) c16[i] = __ldg(tt.c16 + k1 * 16 + i);
-    if (warp == 4) TC_ROLE_BEGIN();
-    for (int64_t it = 0; it < my_tiles; ++it) {
-      const int buf = (int)(it & 1);
-      const uint32_t par = (uint32_t)((it >> 1) & 1);
-      TC_WAITM(TC_BAR(TCB_A2F, buf), par);  // Y16[buf] (written by INTER) is visible
-      TC_WAITM(TC_BAR(TCB_D2F, buf), par);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      float v16 = 0.f;
-      {
-        const float4 *y = reinterpret_cast<const float4 *>(Y16 + (buf * TC_NF + fl) * 16);
+      for (int j = 0; j < 4; ++j) {
+        const int c = lane + 32 * j;
+        float e[4];
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const float4 a = y[q];
-          v16 = fmaf(a.x, c16[4 * q], fmaf(a.y, c16[4 * q + 1], fmaf(a.z, c16[4 * q + 2], fmaf(a.w, c16[4 * q + 3], v16))));
+          const int i = 4 * c + q;
+          e[q] = 0.f;
+          if (i < L) {
+            int64_t s = sb + i;
+            if (!p.snip_edges) s = reflect_index(s, t.n, p.pad_mode);
+            e[q] = ld_sample<DT>(b.samples, t.xoff + s);
+          }
         }
+        x[j] = make_float4(e[0], e[1], e[2], e[3]);
       }
-      TC_WAITM(TC_BAR(TCB_PE, buf), par ^ 1);  // MEL has read P[buf] of tile it - 2
-      float *Pf = Pall + (buf * TC_NF + fl) * TC_PP;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {  // bins of k2 = 8 h .. 8 h + 7
-        float r[16];
-        tc_ld_acc_half(tlane + 128 + 64 * buf, h, r);
-        if (h == 1) {
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          tc_arrive(TC_BAR(TCB_D2E, buf));
-        }
-        if (DBG == 1 && blockIdx.x == 0 && it == 0) {
-#pragma unroll
-          for (int c = 0; c < 16; ++c) dbg[128 * 32 + row * 32 + 16 * h + c] = r[c];
-        }
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const int k2 = 8 * h + kk;
-          const float re = r[2 * kk], im = r[2 * kk + 1];
-          float pw = fmaf(re, re, im * im);
-          if (p.use_mag) pw = sqrtf(pw);
-          const int bin = k2 < 8 ? k1 + 32 * k2 : 512 - k1 - 32 * k2;
-          if (k1 != 0 || k2 <= 8) Pf[k1 == 0 ? 32 * k2 : bin] = pw;
-        }
-      }
-      {
-        const float o = __shfl_xor_sync(0xffffffffu, v16, 1);
-        float pw = fmaf(v16, v16, o * o);
-        if (p.use_mag) pw = sqrtf(pw);
-        if ((k1 & 1) == 0) Pf[16 + 32 * (k1 >> 1)] = pw;
-      }
-      if (k1 == 0) Pf[257] = Pf[258] = Pf[259] = 0.f;  // row padding a 128-bit mel load may touch (weight 0): never stale NaNs
-      tc_arrive(TC_BAR(TCB_PF, buf));
     }
-    if (warp == 4) TC_ROLE_END(1);
-  } else if (warp >= 12 && warp < 16) {
-    // ============================================================ MEL: lane = frame (lane % 8), unit = 4 mw + lane / 8 owns filters unit + 16 j
-    const int mw = warp - 12, f = lane & 7, unit = 4 * mw + (lane >> 3), mt = tid - 12 * 32;
-    const int4 *s_md = reinterpret_cast<const int4 *>(sC + tt.off_md);      // [unit][slot] {first bin, float4 groups, weight index, filter}
-    const float4 *s_mw4 = reinterpret_cast<const float4 *>(sC + tt.off_mw);
-    const float lgk = p.log10_mel ? 0.30102999566398119521f : 0.69314718055994530942f;
-    const int Mpad = tt.Mpad;
-    TcCut cm{};
-    if (my_tiles > 0) tc_first_cut(b, tile_begin, cm);
-    if (mw == 0) TC_ROLE_BEGIN();
-    for (int64_t it = 0; it < my_tiles; ++it) {
-      const int buf = (int)(it & 1);
-      const uint32_t par = (uint32_t)((it >> 1) & 1);
-      const TcTile t = tc_tile(b, cm, tile_begin + it);
-      float *out = b.out + t.row0 * p.F;
-      float *E = Eall + buf * TC_NF * Mpad;
-      TC_WAITM(TC_BAR(TCB_PF, buf), par);
-      if (DBG == 1 && blockIdx.x == 0 && it == 0)
-        for (int i = mt; i < TC_NF * TC_PP; i += 128) dbg[2 * 128 * 32 + i] = Pall[i];
-      const float *Pf = Pall + (buf * TC_NF + f) * TC_PP;
-      for (int j = 0; j < tt.fpu; ++j) {
-        const int4 md = s_md[unit * tt.fpu + j];
-        if (md.w < 0) continue;
-        const float4 *pp = reinterpret_cast<const float4 *>(Pf + md.x);
-        const float4 *wp = s_mw4 + md.z;
-        float a0 = 0.f, a1 = 0.f;
-        int i = 0;
-        for (; i + 1 < md.y; i += 2) {  // two independent chains
-          const float4 w0 = wp[i], q0 = pp[i], w1 = wp[i + 1], q1 = pp[i + 1];
-          a0 = fmaf(q0.w, w0.w, fmaf(q0.z, w0.z, fmaf(q0.y, w0.y, fmaf(q0.x, w0.x, a0))));
-          a1 = fmaf(q1.w, w1.w, fmaf(q1.z, w1.z, fmaf(q1.y, w1.y, fmaf(q1.x, w1.x, a1))));
-        }
-        if (i < md.y) {
-          const float4 w0 = wp[i], q0 = pp[i];
-          a0 = fmaf(q0.w, w0.w, fmaf(q0.z, w0.z, fmaf(q0.y, w0.y, fmaf(q0.x, w0.x, a0))));
-        }
-        E[f * Mpad + md.w] = fast_lg2_normal(nanmax(a0 + a1, p.mel_floor)) * lgk;
+    if (L & 3) {  // taps >= L inside the last chunk are not part of the frame
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int i0 = 4 * (lane + 32 * j);
+        if (i0 + 1 >= L) x[j].y = 0.f;
+        if (i0 + 2 >= L) x[j].z = 0.f;
+        if (i0 + 3 >= L) x[j].w = 0.f;
       }
-      tc_arrive(TC_BAR(TCB_PE, buf));
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // the 4 MEL warps: the log-mel tile is complete (E is double-buffered)
-      if (p.feature == B200FEAT_MFCC) {
-        for (int idx = mt; idx < t.nv * p.C; idx += 128) {
-          const int ff = idx / p.C, c = idx - ff * p.C;
-          float acc = 0.f;
-          for (int m = 0; m < p.M; ++m) acc = fmaf(E[ff * Mpad + m], __ldg(p.dct + m * p.C + c), acc);
-          if (p.use_lifter) acc *= __ldg(p.lifter + c);
-          out[(int64_t)ff * p.F + c] = post_affine(p, c, acc);
-        }
-      } else if (Mpad == p.M && ((t.row0 * p.F) & 3) == 0 && !p.post_scale) {  // rows are contiguous in the tile and in the output: 128-bit copies
-        const float4 *src = reinterpret_cast<const float4 *>(E);
-        float4 *dst = reinterpret_cast<float4 *>(out);
-        for (int i = mt; i < t.nv * (p.M >> 2); i += 128) dst[i] = src[i];
-      } else {
-        for (int ff = 0; ff < t.nv; ++ff)
-          for (int m = mt; m < p.M; m += 128) out[(int64_t)ff * p.F + m] = post_affine(p, m, E[ff * Mpad + m]);
-      }
-      for (int i = t.nv * p.F + mt; i < t.nrows * p.F; i += 128) out[i] = post_affine(p, i % p.F, b.pad_value);
     }
-    if (mw == 0) TC_ROLE_END(3);
-  }
+    {
+      // the tap before chunk c is the last tap of chunk c - 1: the neighbour lane's .w (lane 0: lane 31 of the round before)
+      float pv[4];
+      float last = x[0].x;  // lane 0, chunk 0: replicate-left (layers.py:166)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float up = __shfl_up_sync(0xffffffffu, x[j].w, 1);
+        pv[j] = lane == 0 ? last : up;
+        last = __shfl_sync(0xffffffffu, x[j].w, 31);
+      }
+      float s = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s += (x[j].x + x[j].y) + (x[j].z + x[j].w);
+      const float mu = p.remove_dc ? warp_sum(s) * inv_L : 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float d0 = x[j].x - mu, d1 = x[j].y - mu, d2 = x[j].z - mu, d3 = x[j].w - mu, dp = pv[j] - mu;
+        float4 v;
+        v.x = fmaf(-pre, dp, d0) * wreg[j].x;
+        v.y = fmaf(-pre, d0, d1) * wreg[j].y;
+        v.z = fmaf(-pre, d1, d2) * wreg[j].z;
+        v.w = fmaf(-pre, d2, d3) * wreg[j].w;
+        const int c = lane + 32 * j;
+        if (c >= NCH || f >= t.nv) v = make_float4(0.f, 0.f, 0.f, 0.f);  // K-rows beyond the frame are exact zeros
+        *reinterpret_cast<float4 *>(V + (c >> 2) * TC_VS + 4 * (c & 3)) = v;
+      }
+    }
+    __syncwarp();
 
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 16) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tm), "n"(TC_TMEM_COLS));
-#undef TC_BAR
-#undef TC_WAITM
-#undef TC_ROLE_BEGIN
-#undef TC_ROLE_END
+    // ---------------------------------------------------------------- GEMM 1: rows (frame f, n2 = g / g + 8), K = n1
+    float d1[32], e1[16];
+    {
+      uint32_t ah[4][4], al[4][4];
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const float *v0 = V + (8 * ks + tq) * TC_VS + g, *v4 = v0 + 4 * TC_VS;
+        const float a[4] = {v0[0], v0[8], v4[0], v4[8]};
+        tc_split4(a, ah[ks], al[ks]);
+      }
+      tc_wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t db = tc_desc_k128(cb + ks * 32);  // rows 0..31 B1_hi, 32..63 B1_lo
+        tc_wgmma_n64(d1, ah[ks], db, ks ? 1u : 0u);     // [hi*hi | hi*lo]
+        tc_wgmma_n32(e1, al[ks], db, ks ? 1u : 0u);     // lo*hi
+      }
+      tc_wgmma_commit_wait();
+      tc_pin(d1);
+      tc_pin(e1);
+    }
+    // twiddle: lane holds Y[n2][k1] for n2 = g + 8 r, k1 = 4 j + tq (columns 2 k1, 2 k1 + 1)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int n2 = g + 8 * r;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int k1 = 4 * j + tq, i = 4 * j + 2 * r;
+        const float a = d1[i] + (d1[16 + i] + e1[i]), bq = d1[i + 1] + (d1[17 + i] + e1[i + 1]);
+        float yr, yi;
+        if (k1 == 0) { yr = a; yi = 0.f; Y16[n2] = bq; }  // the k1 = 16 column (real): finished on CUDA cores below
+        else {
+          const float2 w = s_tw[(k1 - 1) * 16 + n2];
+          yr = fmaf(a, w.x, -bq * w.y);
+          yi = fmaf(a, w.y, bq * w.x);
+        }
+        *reinterpret_cast<float2 *>(Yp + k1 * TC_YS + 2 * n2) = make_float2(yr, yi);
+      }
+    }
+    __syncwarp();
+
+    // ---------------------------------------------------------------- GEMM 2: rows (frame f, k1 = g / g + 8), K = (n2, re/im)
+    float d2[32], e2[16];
+    {
+      uint32_t ah[4][4], al[4][4];
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const float *y0 = Yp + g * TC_YS + 8 * ks + tq, *y8 = y0 + 8 * TC_YS;
+        const float a[4] = {y0[0], y8[0], y0[4], y8[4]};
+        tc_split4(a, ah[ks], al[ks]);
+      }
+      tc_wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t db = tc_desc_k128(cb + 8192 + ks * 32);  // rows 0..31 B2_hi, 32..63 B2_lo
+        tc_wgmma_n64(d2, ah[ks], db, ks ? 1u : 0u);
+        tc_wgmma_n32(e2, al[ks], db, ks ? 1u : 0u);
+      }
+      tc_wgmma_commit_wait();
+      tc_pin(d2);
+      tc_pin(e2);
+    }
+    // power: lane holds X[k1 + 32 k2] for k1 = g + 8 r, k2 = 4 j + tq
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int k1 = g + 8 * r;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int k2 = 4 * j + tq, i = 4 * j + 2 * r;
+        const float re = d2[i] + (d2[16 + i] + e2[i]), im = d2[i + 1] + (d2[17 + i] + e2[i + 1]);
+        float pw = fmaf(re, re, im * im);
+        if (p.use_mag) pw = sqrtf(pw);
+        const int bin = k2 < 8 ? k1 + 32 * k2 : 512 - k1 - 32 * k2;
+        if (k1 != 0 || k2 <= 8) Pf[k1 == 0 ? 32 * k2 : bin] = pw;
+      }
+    }
+    {  // bins 16 + 32 k2: lane o = lane % 16 computes part o % 2 of k2 = o / 2
+      float v16 = 0.f;
+      const float4 *y = reinterpret_cast<const float4 *>(Y16);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float4 a = y[q], c = __ldg(c16 + q);
+        v16 = fmaf(a.x, c.x, fmaf(a.y, c.y, fmaf(a.z, c.z, fmaf(a.w, c.w, v16))));
+      }
+      const float o = __shfl_xor_sync(0xffffffffu, v16, 1);
+      float pw = fmaf(v16, v16, o * o);
+      if (p.use_mag) pw = sqrtf(pw);
+      if (lane < 16 && (lane & 1) == 0) Pf[16 + 32 * (lane >> 1)] = pw;
+      if (lane == 0) Pf[257] = Pf[258] = Pf[259] = 0.f;  // row padding a 128-bit mel load may touch (weight 0): never stale NaNs
+    }
+    __syncwarp();
+
+    // ---------------------------------------------------------------- MEL: lane = filter (unit-major descriptor order)
+    for (int idx = lane; idx < 16 * tt.fpu; idx += 32) {
+      const int4 md = s_md[idx];
+      if (md.w < 0) continue;
+      const float4 *pp = reinterpret_cast<const float4 *>(Pf + md.x);
+      const float4 *wp = s_mw4 + md.z;
+      float a0 = 0.f, a1 = 0.f;
+      int i = 0;
+      for (; i + 1 < md.y; i += 2) {  // two independent chains
+        const float4 w0 = wp[i], q0 = pp[i], w1 = wp[i + 1], q1 = pp[i + 1];
+        a0 = fmaf(q0.w, w0.w, fmaf(q0.z, w0.z, fmaf(q0.y, w0.y, fmaf(q0.x, w0.x, a0))));
+        a1 = fmaf(q1.w, w1.w, fmaf(q1.z, w1.z, fmaf(q1.y, w1.y, fmaf(q1.x, w1.x, a1))));
+      }
+      if (i < md.y) {
+        const float4 w0 = wp[i], q0 = pp[i];
+        a0 = fmaf(q0.w, w0.w, fmaf(q0.z, w0.z, fmaf(q0.y, w0.y, fmaf(q0.x, w0.x, a0))));
+      }
+      E[md.w] = fast_lg2_normal(nanmax(a0 + a1, p.mel_floor)) * lgk;
+    }
+    __syncwarp();
+    float *out = b.out + (t.row0 + f) * p.F;
+    if (f < t.nv) {
+      if (p.feature == B200FEAT_MFCC) {
+        for (int c = lane; c < p.C; c += 32) {
+          float acc = 0.f;
+          for (int m = 0; m < p.M; ++m) acc = fmaf(E[m], __ldg(p.dct + m * p.C + c), acc);
+          if (p.use_lifter) acc *= __ldg(p.lifter + c);
+          out[c] = post_affine(p, c, acc);
+        }
+      } else {
+        for (int m = lane; m < p.M; m += 32) out[m] = post_affine(p, m, E[m]);
+      }
+    } else if (f < t.nrows) {
+      for (int i = lane; i < p.F; i += 32) out[i] = post_affine(p, i, b.pad_value);
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------- host
 struct Tc512Host {
   Tc512Tables t;
   size_t smem;
+  int ctas_per_sm;  // resident CTAs per SM (the persistent grid is this many per SM)
 };
 
 static inline bool tc512_supported(const DevPlan &p) {
@@ -601,7 +445,7 @@ static int tc_upload(const std::vector<T> &h, std::vector<void *> &allocs, const
   return 0;
 }
 
-// host images of the constant tables (no CUDA calls: the probe uses it too)
+// host images of the constant tables
 struct Tc512Image {
   std::vector<unsigned char> blob;
   std::vector<float> win4, c16;
@@ -693,17 +537,22 @@ static inline int tc512_build_image(const DevPlan &p, const std::vector<float> &
   return 0;
 }
 
-static inline size_t tc512_smem_bytes(const Tc512Tables &t) {
-  return (size_t)TC_OFF_CONST + (size_t)t.cblob_bytes + 8 * (TCB_COUNT + 3) + 4 * (2 * TC_NF * TC_PP + 2 * TC_NF * 16 + 2 * TC_NF * (size_t)t.Mpad) + 16;
+static inline int tc512_warp_bytes(int Mpad) { return 4 * (32 * TC_VS + 16 * TC_YS + TC_PP + 16 + Mpad); }
+static inline size_t tc512_smem_bytes(const Tc512Tables &t) {  // 1024 B of alignment slack + tables + mbarrier + per-warp buffers
+  return 1024 + (size_t)t.cblob_bytes + 16 + (size_t)(TC_THREADS / 32) * (size_t)t.warp_bytes;
 }
 
-template <int DT, int DBG>
+template <int DT>
 static int tc512_go(bool launch, size_t smem, const DevPlan &p, const Tc512Tables &t, const DevBatch &b, dim3 grid, cudaStream_t stream,
-                    float *dbg) {
-  auto kern = b200feat_tc512_kernel<DT, DBG>;
-  if (!launch)
-    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
-  kern<<<grid, dim3(TC_THREADS), smem, stream>>>(p, t, b, dbg);
+                    int *ctas_per_sm) {
+  auto kern = b200feat_tc512_kernel<DT>;
+  if (!launch) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return B200FEAT_ECUDA;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, kern, TC_THREADS, smem) != cudaSuccess || *ctas_per_sm < 1)
+      return B200FEAT_ECUDA;
+    return 0;
+  }
+  kern<<<grid, dim3(TC_THREADS), smem, stream>>>(p, t, b);
   return 0;
 }
 
@@ -718,13 +567,16 @@ static inline int tc512_prepare(DevPlan &p, const std::vector<float> &bank, std:
   hst.t.cblob = d;
   hst.t.cblob_bytes = (int)img.blob.size();
   hst.t.off_tw = img.off_tw; hst.t.off_md = img.off_md; hst.t.off_mw = img.off_mw; hst.t.fpu = img.fpu; hst.t.Mpad = img.Mpad;
+  hst.t.warp_bytes = tc512_warp_bytes(img.Mpad);
   if ((rc = tc_upload(img.win4, allocs, &hst.t.win4))) return rc;
   if ((rc = tc_upload(img.c16, allocs, &hst.t.c16))) return rc;
   hst.smem = tc512_smem_bytes(hst.t);
   if (hst.smem > (size_t)227 * 1024) return B200FEAT_EUNSUPPORTED;
   DevBatch none{};
-  if (tc512_go<B200FEAT_F32, 0>(false, hst.smem, p, hst.t, none, dim3(1), nullptr, nullptr)) return B200FEAT_ECUDA;
-  if (tc512_go<B200FEAT_I16, 0>(false, hst.smem, p, hst.t, none, dim3(1), nullptr, nullptr)) return B200FEAT_ECUDA;
+  int occ_f32 = 0, occ_i16 = 0;
+  if (tc512_go<B200FEAT_F32>(false, hst.smem, p, hst.t, none, dim3(1), nullptr, &occ_f32)) return B200FEAT_ECUDA;
+  if (tc512_go<B200FEAT_I16>(false, hst.smem, p, hst.t, none, dim3(1), nullptr, &occ_i16)) return B200FEAT_ECUDA;
+  hst.ctas_per_sm = std::min(occ_f32, occ_i16);
   *out = hst;
   *frames_per_tile = TC_NF;
   return 0;
@@ -732,8 +584,9 @@ static inline int tc512_prepare(DevPlan &p, const std::vector<float> &bank, std:
 
 static inline int tc512_launch(const DevPlan &p, const Tc512Host &hst, const DevBatch &b, int dt, int sm_count, cudaStream_t stream) {
   int64_t blocks = b.num_tiles;
-  if (blocks > sm_count) blocks = sm_count;  // persistent: one CTA per SM
-  if (dt == B200FEAT_I16) tc512_go<B200FEAT_I16, 0>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream, nullptr);
-  else tc512_go<B200FEAT_F32, 0>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream, nullptr);
+  const int64_t cap = (int64_t)sm_count * hst.ctas_per_sm;  // persistent: every resident CTA walks a contiguous tile range
+  if (blocks > cap) blocks = cap;
+  if (dt == B200FEAT_I16) tc512_go<B200FEAT_I16>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream, nullptr);
+  else tc512_go<B200FEAT_F32>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream, nullptr);
   return (int)cudaGetLastError();
 }

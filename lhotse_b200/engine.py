@@ -2,7 +2,7 @@
 ctypes binding of ``libb200feat.so`` (include/b200feat.h) + the host-side staging of ragged
 batches.  torch is used here for device memory, pinned memory and streams only.
 
-There is NO CPU fallback: if the library is missing, or no sm_100 GPU is visible, creating an
+There is NO CPU fallback: if the library is missing, or no sm_90 GPU is visible, creating an
 ``Engine`` raises.  (The CPU oracle under ``oracle/`` is test infrastructure and is never
 imported from this package.)
 """
@@ -384,7 +384,7 @@ class Engine:
 
 # ---- host staging --------------------------------------------------------------------------------------------------
 # Gathering B separately allocated waveforms into one pinned buffer is a plain memcpy, and ONE host thread moves only a
-# fraction of what PCIe 5 takes (profiles/README.md "list routes"), so the copies are spread over a small thread pool
+# fraction of what PCIe takes, so the copies are spread over a small thread pool
 # (numpy / torch copies release the GIL) and overlapped with the transfer of the previous group.
 STAGING_THREADS = max(1, min(8, (os.cpu_count() or 2) // 2, int(os.environ.get("B200FEAT_STAGING_THREADS", "8"))))
 _POOL = None

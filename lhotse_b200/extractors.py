@@ -1,5 +1,5 @@
 """
-B200-native counterparts of lhotse's Kaldi-family extractors, behind the unchanged
+H100-native counterparts of lhotse's Kaldi-family extractors, behind the unchanged
 ``FeatureExtractor`` API (lhotse/features/base.py:37-222):
 
     reference class (lhotse/features/kaldi/extractors.py)      here

@@ -13,7 +13,7 @@ against the imported reference and against ``tests/golden/*.npz`` generated from
 makes its timing representative of the reference's CPU implementation.  A plain-C second
 restatement lives in ``oracle/fbank_oracle.c``.
 
-Reference citations (relative to /root/reference):
+Reference citations (relative to the reference lhotse tree):
   frame count ............ lhotse/utils.py:424-434, lhotse/features/kaldi/layers.py:747-753
   reflect framing ........ lhotse/features/kaldi/layers.py:727-772
   DC / energy / preemph .. lhotse/features/kaldi/layers.py:151-186, :859-870

@@ -1,7 +1,8 @@
 """TEST / BASELINE INFRASTRUCTURE (never imported by `lhotse_b200/`): makes the *reference* (lhotse) importable where
-`soundfile`, `intervaltree` and `cytoolz` are absent (SURVEY.md §8c).  In the build container the reference is the
-read-only tree `/root/reference`; on the GPU box it is the archive `oracle/_ref/lhotse_ref.zip` that `oracle/make_ref.py`
-packs from that tree (git-ignored, travels with the snapshot; imported through zipimport).
+`soundfile`, `intervaltree` and `cytoolz` are absent (SURVEY.md §8c).  The reference is an unmodified lhotse source tree named
+by LHOTSE_REFERENCE_ROOT, or else the archive `oracle/_ref/lhotse_ref.zip` that `oracle/make_ref.py` (run by `build()`) packs
+from such a tree (git-ignored; imported through zipimport).  Where neither exists, `reference_available()` is False and the
+tests that need lhotse itself skip.
 Users: `tests/refshim.py` (the parity tests) and `bench.py`'s CPU reference legs (`cpu_baseline`, `--impl reference`)."""
 import os
 import sys
@@ -15,8 +16,6 @@ def _resolve_root() -> str:
     env = os.environ.get("LHOTSE_REFERENCE_ROOT")
     if env:
         return env
-    if os.path.isdir("/root/reference/lhotse"):
-        return "/root/reference"
     return REFERENCE_ZIP
 
 

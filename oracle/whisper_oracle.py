@@ -16,7 +16,7 @@ bit-for-bit against ``transformers.audio_utils.mel_filter_bank(norm="slaney", me
 (present in this image; upstream tests that function against librosa), and the golden vectors were
 generated with the reference's own code running on that transformers table.
 
-Reference citations (relative to /root/reference):
+Reference citations (relative to the reference lhotse tree):
   constants (16 kHz, n_fft 400, hop 160, periodic Hann) ... lhotse/features/whisper_fbank.py:107-123
   centred STFT, last frame dropped ....................... lhotse/features/whisper_fbank.py:62-63
   mel, log10, clamp to max - 8, (x + 4) / 4 ............... lhotse/features/whisper_fbank.py:65-69

@@ -1,7 +1,7 @@
 // CPU check of the FFT stages of lhotse_b200/csrc/fast2048.cuh: the __host__ __device__ stage functions are run lane by lane
 // (32 emulated lanes, the exchange tile a plain array) and the resulting |2 X[k]|^2, k = 0..1024, is compared with a float64
 // DFT of the same 2048 real samples.  No GPU needed:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -o /tmp/f2k_host_check scripts/micro/f2k_host_check.cu && /tmp/f2k_host_check
+//   nvcc -gencode arch=compute_90a,code=sm_90a -o f2k_host_check scripts/micro/f2k_host_check.cu && ./f2k_host_check
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>

@@ -1,13 +1,13 @@
-"""Numerical model (numpy, CPU) of moving the 512-point real FFT of the headline path onto tcgen05 tensor cores as two
-radix-16 stages of small GEMMs (DESIGN.md §6 item 4): what accuracy do plain TF32, the 3xTF32 split (A_hi*B_hi + A_lo*B_hi +
-A_hi*B_lo, verified on the B200 by scripts/micro/umma_tf32_probe.cu) and a 2xBF16-style split give on the quantities the
+"""Numerical model (numpy, CPU) of moving the 512-point real FFT of the headline path onto tensor cores as two
+stages of small GEMMs (DESIGN.md §3.1e): what accuracy do plain TF32, the 3xTF32 split (A_hi*B_hi + A_lo*B_hi +
+A_hi*B_lo) and a 2xBF16-style split give on the quantities the
 parity gate looks at (power bins, log-mel)?  Operands are rounded exactly as `cvt.rna.tf32.f32` does (10 explicit mantissa
 bits, round to nearest, ties away); products are exact (tensor cores multiply TF32 exactly), accumulation is float32.
 
 Pipeline modelled (same algebra as csrc/fast512.cuh): z[n] = y[2n] + i*y[2n+1] (256 complex points) = 16 x 16;
 stage A: DFT16 over n1 for every n2 as a (32 x 32 real) x (32 x 16) GEMM; twiddle W256^(n2*k1) on CUDA cores (fp32);
 stage B: DFT16 over n2 as a second GEMM; real-FFT split, |X|^2, mel (80 filters), log — all fp32.
-Run: python scripts/micro/tf32_dft_model.py  ->  profiles/r1_tf32_dft_model.txt
+Run: python scripts/micro/tf32_dft_model.py  (prints the table)
 """
 import os
 import sys
@@ -111,8 +111,6 @@ def main():
             lines.append(f"{mode:8s} power-bin err / frame peak: {rel.max():.2e}    max|d log-mel|: {np.abs(mel - mel64).max():.2e}")
     out = "\n".join(lines) + "\n"
     print(out)
-    with open(os.path.join(ROOT, "profiles", "r1_tf32_dft_model.txt"), "w") as f:
-        f.write(out)
 
 
 if __name__ == "__main__":

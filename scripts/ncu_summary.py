@@ -1,4 +1,4 @@
-"""Summarises an .ncu-rep (raw + SASS source pages) into a small text report for profiles/."""
+"""Summarises an .ncu-rep (raw + SASS source pages) into a small text report on stdout."""
 import collections, csv, subprocess, sys, io
 rep = sys.argv[1]; frames = int(sys.argv[2]) if len(sys.argv) > 2 else 512000
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

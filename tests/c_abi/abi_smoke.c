@@ -6,7 +6,7 @@
  * <dir> holds float32 little-endian files written by the test that drives this program (tests/test_c_abi.py):
  *   window.f32 (L), bank.f32 (K x M row-major), samples.f32 (the cuts back to back), lens.i64 (B cut lengths).
  * Writes <dir>/out.f32 (packed (sum T_i, F) features) and <dir>/rows.i64 (B frame counts).
- * Exit codes: 0 ok; 3 = b200feat_create said B200FEAT_ENODEVICE (no sm_100 GPU: the library has no CPU fallback);
+ * Exit codes: 0 ok; 3 = b200feat_create said B200FEAT_ENODEVICE (no sm_90 GPU: the library has no CPU fallback);
  *             1 = anything else went wrong (message on stderr).
  */
 #include <stdint.h>

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generates tests/golden/golden_v1.npz by running the REAL reference (lhotse imported from
-/root/reference, CPU, float32) on seeded inputs.  Run in the build container only:
+the reference lhotse tree, CPU, float32) on seeded inputs.  Run in the build container only:
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 

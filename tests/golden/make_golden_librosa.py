@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generates tests/golden/golden_librosa_v1.npz by running the REAL reference class
-`lhotse.features.librosa_fbank.LibrosaFbank` (imported from /root/reference, CPU) on seeded inputs.  Build container only:
+`lhotse.features.librosa_fbank.LibrosaFbank` (imported from the reference lhotse tree, CPU) on seeded inputs.  Build container only:
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden_librosa.py
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generates tests/golden/golden_whisper_v1.npz by running the REAL reference class
-`lhotse.features.whisper_fbank.WhisperFbank` (imported from /root/reference, CPU, float32) on seeded inputs.
+`lhotse.features.whisper_fbank.WhisperFbank` (imported from the reference lhotse tree, CPU, float32) on seeded inputs.
 Build container only:
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden_whisper.py

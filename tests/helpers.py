@@ -12,7 +12,7 @@ GOLDEN = os.path.join(HERE, "golden", "golden_v1.npz")
 
 # north_star: "within 1e-4 relative (float32)".  Element-wise that cannot hold against an fp32
 # reference whose own distance to the float64 truth reaches 8e-4 abs on log-mel values
-# (measured: profiles/r2_parity_report.json, DESIGN.md "Parity tolerance"), so the gate is, per element,
+# (DESIGN.md "Parity tolerance"), so the gate is, per element,
 #   |ours - truth64| / tol <= max(1, NOISE_X * N(frame)),   tol = ATOL + RTOL*|truth64|
 # where N(frame) is the largest |ref32 - truth64| / tol over the element's own frame and its two neighbours: a noisy
 # frame of the reference (a near-cancelling bin, a frame at the mel floor) relaxes the bound for that neighbourhood

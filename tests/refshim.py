@@ -1,7 +1,7 @@
 """Test-only helper: make the *reference* (lhotse) importable where `soundfile`, `intervaltree` and `cytoolz` are
-absent (SURVEY.md §8c).  In the build container the reference is the read-only tree `/root/reference`; on the GPU box
-it is the archive `oracle/_ref/lhotse_ref.zip` that `oracle/make_ref.py` packs from that tree (git-ignored, travels with
-the snapshot; imported through zipimport).  Never used by the product."""
+absent (SURVEY.md §8c).  The reference is the tree named by LHOTSE_REFERENCE_ROOT or the archive
+`oracle/_ref/lhotse_ref.zip` that `oracle/make_ref.py` packs from it during `build()` (see oracle/refimport.py); tests that
+need lhotse itself skip where neither exists.  Never used by the product."""
 import os
 import sys
 import types

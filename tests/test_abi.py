@@ -34,7 +34,7 @@ def test_version_and_struct_layout():
     assert lib.b200feat_meta_words(10) == 42
 
 
-def test_library_is_sm100a_only():
+def test_library_is_sm90a_only():
     import shutil
     import subprocess
 
@@ -43,7 +43,7 @@ def test_library_is_sm100a_only():
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "-lelf", engine.lib_path()], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_no_gpu_means_loud_failure():

@@ -1,6 +1,6 @@
 """The drop-in boundary from plain C: tests/c_abi/abi_smoke.c is compiled with gcc against include/b200feat.h and linked
 to the in-tree libb200feat.so — no Python, torch or C++ on the caller's side.  CPU tier: it builds, links, loads, and
-`b200feat_create` refuses loudly without an sm_100 GPU (no CPU fallback).  GPU tier: its output equals the Python
+`b200feat_create` refuses loudly without an sm_90 GPU (no CPU fallback).  GPU tier: its output equals the Python
 extractor's, bit for bit."""
 import os
 import shutil

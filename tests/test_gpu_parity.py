@@ -128,8 +128,7 @@ def test_headline_size_properties():
 
 def test_mfcc_config3_tolerance():
     """BASELINE config 3: Mfcc(num_ceps=13, num_mel_bins=23) at the reference's own tolerance (test/features/
-    test_kaldi_features.py:122: rtol 1e-3, atol 1e-4), on every kernel.  Measured (profiles/r2_parity_report.json): the smallest
-    atol that passes at rtol 1e-3 is 2.6e-5 (generic), 3.0e-5 (fast), 7.3e-5 (tc)."""
+    test_kaldi_features.py:122: rtol 1e-3, atol 1e-4), on every kernel."""
     torch.manual_seed(1)
     x = (0.1 * torch.randn(8, 160000)).numpy()
     cfg = O.OracleConfig(feature="mfcc", num_ceps=13, num_filters=23)
@@ -203,7 +202,7 @@ def test_long_recording_and_many_tiny_cuts():
         got = y[a0:a1]
         want = ref[a0 - shift:a1 - shift]
         assert got.shape == want.shape and got.shape[0] > 50
-        np.testing.assert_allclose(got, want, rtol=1e-4, atol=1e-3)  # measured worst |ours - ref32| on noise: 6.8e-4 (r2_parity_report)
+        np.testing.assert_allclose(got, want, rtol=1e-4, atol=1e-3)
     lens = rs.randint(3200, 19200, size=5000)
     xs = [(0.1 * rs.randn(m)).astype(np.float32) for m in lens]
     out = ext.extract_batch(xs, 16000)
@@ -568,7 +567,7 @@ def test_random_configs_auto_kernel_vs_oracle(i, feature, cfg):
 
 
 def test_tensor_core_kernel_at_headline_size():
-    """kernel="tc" (tcgen05 two-stage DFT, csrc/tc512.cuh) on BASELINE configs[1] inputs: against the register-FFT kernel
+    """kernel="tc" (wgmma two-stage DFT, csrc/tc512.cuh) on BASELINE configs[1] inputs: against the register-FFT kernel
     (two independent CUDA implementations of layers.py:151-186, :32-42, :565-578) and against the oracle on a sample of cuts;
     deterministic, cuts independent, padded mode and MFCC epilogue included."""
     torch.manual_seed(0)
