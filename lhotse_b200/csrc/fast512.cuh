@@ -6,7 +6,7 @@
 //   radix-16 DFT over n1 in registers  -> Y[k1][l], times W256^(l*k1)
 //   16x16 transpose through a padded shared-memory tile (the only FFT traffic that leaves registers)
 //   lane k1 holds Y'[k1][0..15], radix-16 DFT over n2 -> Z[k1 + 16*k2]
-//   real-FFT split against the mirrored lane (16 - k1) with half-warp shuffles -> |X[k]|^2
+//   real-FFT split against the mirrored lane (16 - k1), whose slots come through the idle transpose tile -> |X[k]|^2
 //   power spectrum of 4 consecutive frames staged as P[k][4] -> sparse mel bank with the weights
 //   shared by the 4 frames (LDS.128) -> log -> coalesced 64-byte row segments.
 //
@@ -49,7 +49,7 @@ struct Fast512Tables {  // derived once per handle
   int cblob_bytes;
   int off_tw1, off_rdesc, off_mw;  // byte offsets inside the blob
   const float2 *tw1;    // [16][16] W256^(l*k1) (global copy: loaded into registers by the default variant)
-  const float2 *w512;   // [16]     W512^l
+  const float2 *w512;   // [8][16]  W512^(l + 16 i): the real-FFT split twiddle of lane l's pair i
   int mel_rounds;       // ceil(M / 16)
   int mel_wrows;        // sum of the rounds' trip counts
 };
@@ -115,10 +115,28 @@ F512_HD float2 f2mul_w8_3(float2 a) {
 #endif
 }
 
+// dft4 whose inputs a2 (Z2) and / or a3 (Z3) are known to be +0: the adds with them are left out (x + 0 = x except
+// for the sign of a zero, which no power spectrum keeps)
+template <bool Z2, bool Z3>
+F512_HD void dft4z(float2 &a0, float2 &a1, float2 &a2, float2 &a3) {
+  const float2 s02 = Z2 ? a0 : f2add(a0, a2), d02 = Z2 ? a0 : f2sub(a0, a2);
+  const float2 s13 = Z3 ? a1 : f2add(a1, a3), d13 = Z3 ? a1 : f2sub(a1, a3);
+  a0 = f2add(s02, s13);
+  a2 = f2sub(s02, s13);
+  a1 = f2add(d02, f2mi(d13));
+  a3 = f2add(d02, f2pi(d13));
+}
+
 // forward 16-point DFT in registers (radix 4x4).  Input v[n]; output X[k] lands in v[4*(k&3) + (k>>2)].
+// Inputs v[NZ..15] are +0 (a frame shorter than 32 * 16 taps): the first radix-4 pass skips them.
+template <int NZ = 16>
 F512_HD void dft16(float2 (&v)[16]) {
 #pragma unroll
-  for (int b = 0; b < 4; ++b) dft4(v[b], v[4 + b], v[8 + b], v[12 + b]);
+  for (int b = 0; b < 4; ++b) {
+    if (8 + b >= NZ) dft4z<true, true>(v[b], v[4 + b], v[8 + b], v[12 + b]);
+    else if (12 + b >= NZ) dft4z<false, true>(v[b], v[4 + b], v[8 + b], v[12 + b]);
+    else dft4(v[b], v[4 + b], v[8 + b], v[12 + b]);
+  }
   // v[4c + b] = y[b][c]; twiddle by W16^(b*c), W16^m = (cos(pi m/8), -sin(pi m/8))
   v[5] = f2mul(v[5], make_float2(F512_C1, -F512_S1));    // W^1
   v[6] = f2mul_w8_1(v[6]);                               // W^2
@@ -131,6 +149,18 @@ F512_HD void dft16(float2 (&v)[16]) {
   v[15] = f2mul(v[15], make_float2(-F512_C1, F512_S1));  // W^9
 #pragma unroll
   for (int c = 0; c < 4; ++c) dft4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
+}
+
+// Pre-emphasis and window of the DC-free taps (x - mu), two adjacent taps per lane.  Pre-emphasis is linear, so
+// pre(x - mu)[j] = x[j] - preemph * x[j-1] - cmu with cmu = mu * (1 - preemph), the replicate-left first tap included:
+// three operations per tap, each rounded on its own.
+F512_HD float2 preemph_window_dc(float2 x, float xp, float preemph, float cmu, float2 w) {
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fmul_rn(__fadd_rn(__fmaf_rn(xp, -preemph, x.x), -cmu), w.x),
+                     __fmul_rn(__fadd_rn(__fmaf_rn(x.x, -preemph, x.y), -cmu), w.y));
+#else
+  return make_float2((fmaf(xp, -preemph, x.x) - cmu) * w.x, (fmaf(x.x, -preemph, x.y) - cmu) * w.y);
+#endif
 }
 // register holding output bin k of dft16
 #define F512_OUT(k) (4 * ((k) & 3) + ((k) >> 2))
@@ -178,9 +208,15 @@ static inline size_t fast512_smem_bytes(const DevPlan &p, const Fast512Tables &t
   return (b + 15) & ~(size_t)15;
 }
 
-template <int DT, int LCT, int WARPS, int SLOTS, int TWS, int MINB>
+// PLAIN: the host has established that the plan is a log-mel fbank without energy column or magnitude spectrum, that
+// no output affine is set and that the output is packed; those options then cost no instructions or registers.
+template <int DT, int LCT, int WARPS, int SLOTS, int TWS, int MINB, bool PLAIN>
 __global__ void __launch_bounds__(WARPS * 32, MINB)
 b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch b) {
+  const bool use_energy = !PLAIN && p.use_energy;
+  const bool use_mag = !PLAIN && p.use_mag;
+  const bool padded = !PLAIN && b.out_mode == B200FEAT_OUT_PADDED;
+  const int feature = PLAIN ? B200FEAT_FBANK : p.feature;
   constexpr int HW = 2 * WARPS;               // half-warps per CTA
   constexpr int TILE = HW * SLOTS;            // frames per tile
   constexpr int PBINS = F512_PBINS(SLOTS);
@@ -225,7 +261,9 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
 #pragma unroll
     for (int k1 = 1; k1 < 16; ++k1) tw1[TWS ? 0 : k1] = __ldg(ft.tw1 + k1 * 16 + l);
   }
-  const float2 w512l = __ldg(ft.w512 + l);
+  float2 wsplit[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) wsplit[i] = __ldg(ft.w512 + i * 16 + l);
   const int partner = (16 - l) & 15;
   const float inv_L = 1.0f / (float)L;
   {  // every thread observes the completion of the bulk copy (phase 0 of the mbarrier) before touching the tables
@@ -243,11 +281,11 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
     // the two-load chain of this prologue is already hidden by the other warps)
     const int64_t t0 = (tile - __ldg(b.tile_off + cut)) * TILE + (int64_t)hw * SLOTS;
     const int64_t T = __ldg(b.row_off + cut + 1) - __ldg(b.row_off + cut);
-    const int64_t rows_here = b.out_mode == B200FEAT_OUT_PADDED ? b.max_frames : T;
+    const int64_t rows_here = padded ? b.max_frames : T;
     if (!__any_sync(F512_FULL, t0 < rows_here)) continue;  // both halves idle for this tile
     const int64_t n = __ldg(b.nsamp + cut);
     const int64_t xoff = __ldg(b.samp_off + cut);
-    const int64_t row0 = b.out_mode == B200FEAT_OUT_PADDED
+    const int64_t row0 = padded
                              ? (int64_t)(b.batch_first + cut) * b.max_frames + t0
                              : __ldg(b.row_off + cut) + t0;
     // Everything per frame below is 32-bit arithmetic relative to the half-warp's first frame `tb`:
@@ -350,6 +388,7 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
 #pragma unroll
       for (int n1 = 0; n1 < NP; ++n1) s += v[n1].x + v[n1].y;  // taps beyond L are exact zeros
       const float mu = p.remove_dc ? hw_sum(s) * inv_L : 0.f;
+      const float cmu = __fmul_rn(mu, 1.0f - p.preemph);  // the DC offset after pre-emphasis
       // ---- energy, pre-emphasis, window (layers.py:159-170); zero padding is implicit
       float e = 0.f;
 #pragma unroll
@@ -357,26 +396,30 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
         if (n1 < NP) {
           const int j0 = 32 * n1 + 2 * l;
           const float2 w = s_win[n1 * 16 + l];  // zero beyond L
-          float2 d = f2add(v[n1], make_float2(-mu, -mu));  // (da, dc)
-          const float dp = prev[n1] - mu;
-          if (j0 >= L) d.x = 0.f;
-          if (j0 + 1 >= L) d.y = 0.f;
-          if (p.raw_energy) e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
-          const float2 y = preemph_window2(d, dp, p.preemph, w);
-          if (!p.raw_energy) e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
+          const float2 y = preemph_window_dc(v[n1], prev[n1], p.preemph, cmu, w);
+          if (use_energy) {
+            if (p.raw_energy) {
+              float2 d = f2add(v[n1], make_float2(-mu, -mu));
+              if (j0 >= L) d.x = 0.f;
+              if (j0 + 1 >= L) d.y = 0.f;
+              e = fmaf(d.x, d.x, fmaf(d.y, d.y, e));
+            } else {
+              e = fmaf(y.x, y.x, fmaf(y.y, y.y, e));
+            }
+          }
           v[n1] = y;
         } else {
           v[n1] = make_float2(0.f, 0.f);
         }
       }
-      if (p.use_energy) {  // le[] stays in registers: no dynamic indexing
+      if (use_energy) {  // le[] stays in registers: no dynamic indexing
         const float lev = log_energy_value(p, hw_sum(e));
 #pragma unroll
         for (int k = 0; k < SLOTS; ++k) le[k] = (f == k) ? lev : le[k];
       }
 
       // ---- stage 1: radix-16 over n1, twiddle, transpose
-      dft16(v);
+      dft16<NP>(v);
 #pragma unroll
       for (int k1 = 0; k1 < 16; ++k1) {
         float2 y = v[F512_OUT(k1)];
@@ -398,75 +441,69 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
       dft16(v);
       // ---- real-FFT split + power (layers.py:38-42).  With E = Z[k] + conj(Z[256-k]), O = Z[k] - conj(Z[256-k]),
       // T = W512^k * O:   2*X[k] = E - i*T   and   2*conj(X[256-k]) = E + i*T, so one (E, O, T) serves two bins.
-      // Lane l owns k = l + 16*k2 and its mirror lane 16-l owns 256-k: each lane handles its EVEN k2 and gets
-      // the mirror's ODD slots (8 complex shuffles instead of 16).  Lane 0 mirrors itself with a one-slot
-      // shift (256 - 16*j = 16*(16-j)), so it walks the pairs (0,0) (2,14) (4,12) (6,10) (8,8) (1,15) (3,13) (5,11)
-      // here and (7,9) below.  The 1/4 of |X|^2 = |2X|^2/4 is folded into the mel weights / spectrogram epilogue.
-      float *Pf = P + f * PBINS;
+      // Lane l takes the pairs k = l + 16*i, i = 0..7: Z[k] is its own slot i, and Z[256-k] is slot 15-i of lane 16-l
+      // (lanes 1..15) or lane 0's slot 16-i (mod 16).  The mirrored slots go through the transpose tile, which is idle
+      // here: every lane stores slots 8..15 and then slot 0 at positions 8..16 of its row, lane 0 one position lower,
+      // so that every lane finds its eight mirrors at positions 15..8 of its partner's row.  Bin 128 is left over.
+      // The 1/4 of |X|^2 = |2X|^2/4 is folded into the mel weights / spectrogram epilogue.
+      {
+        float2 *xs = X + l * F512_XROW - (l == 0 ? 1 : 0);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        constexpr int kOwn0[8] = {0, 2, 4, 6, 8, 1, 3, 5};
-        constexpr int kSend0[8] = {0, 14, 12, 10, 8, 15, 13, 11};
-        const float2 zo = v[F512_OUT(2 * i)], zo0 = v[F512_OUT(kOwn0[i])];
-        const float2 zs = v[F512_OUT(15 - 2 * i)], zs0 = v[F512_OUT(kSend0[i])];
-        const float2 zk = (i >= 5 && l == 0) ? zo0 : zo;
-        const float sx = l == 0 ? zs0.x : zs.x, sy = l == 0 ? zs0.y : zs.y;
-        const float2 cc = f2conj(make_float2(__shfl_sync(F512_FULL, sx, partner, 16), __shfl_sync(F512_FULL, sy, partner, 16)));
-        const float2 E = f2add(zk, cc), O = f2sub(zk, cc);
-        float2 Ow;                                    // O * W16^i; lane 0 needs W32^(own slot) once i >= 5
-#if F512_R2TRICK
-        if (i == 0) Ow = O;                           // W16^0 = 1, W16^4 = -i, W16^2 = W8^1: no general product needed
-        else if (i == 4) Ow = f2mi(O);
-        else if (i == 2) Ow = f2mul_w8_1(O);
-        else
-#endif
-        {
-          float2 wc = w32_const(2 * i);
-          if (i >= 5) { const float2 w0 = w32_const(kOwn0[i]); wc = l == 0 ? w0 : wc; }
-          Ow = f2mul(O, wc);
+        for (int s2 = 8; s2 < 16; ++s2) xs[s2] = v[F512_OUT(s2)];
+        xs[16] = v[F512_OUT(0)];
+      }
+      __syncwarp();
+      float *Pf = P + f * PBINS;
+      const float4 *mirror = reinterpret_cast<const float4 *>(X + partner * F512_XROW);
+#pragma unroll
+      for (int i = 0; i < 8; i += 2) {
+        const float4 m2 = mirror[7 - i / 2];  // positions 15 - i - 1 and 15 - i
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float2 zk = v[F512_OUT(i + h)];
+          const float2 cc = h == 0 ? make_float2(m2.z, -m2.w) : make_float2(m2.x, -m2.y);
+          const float2 E = f2add(zk, cc), O = f2sub(zk, cc);
+          const float2 mit = f2mi(f2mul(O, wsplit[i + h]));  // -i*T
+          const float2 a = f2add(E, mit);                     // 2*X[k]
+          const float2 bq = f2sub(E, mit);                    // 2*conj(X[256-k])
+          float pa = fmaf(a.x, a.x, a.y * a.y), pb = fmaf(bq.x, bq.x, bq.y * bq.y);
+          if (use_mag) { pa = sqrtf(pa); pb = sqrtf(pb); }
+          Pf[l + 16 * (i + h)] = pa;
+          Pf[256 - l - 16 * (i + h)] = pb;
         }
-        const float2 mit = f2mi(f2mul(Ow, w512l));    // -i*T
-        const float2 a = f2add(E, mit);               // 2*X[k]
-        const float2 bq = f2sub(E, mit);              // 2*conj(X[256-k])
-        float pa = fmaf(a.x, a.x, a.y * a.y), pb = fmaf(bq.x, bq.x, bq.y * bq.y);
-        if (p.use_mag) { pa = sqrtf(pa); pb = sqrtf(pb); }
-        const int k = l == 0 ? 16 * kOwn0[i] : l + 32 * i;
-        Pf[k] = pa;
-        Pf[256 - k] = pb;
       }
-      if (l == 0) {  // lane 0's last pair: slots (7, 9) -> bins 112 and 144
-        const float2 zk = v[F512_OUT(7)], cc = f2conj(v[F512_OUT(9)]);
-        const float2 E = f2add(zk, cc), O = f2sub(zk, cc);
-        const float2 mit = f2mi(f2mul(O, w32_const(7)));
-        const float2 a = f2add(E, mit), bq = f2sub(E, mit);
-        float pa = fmaf(a.x, a.x, a.y * a.y), pb = fmaf(bq.x, bq.x, bq.y * bq.y);
-        if (p.use_mag) { pa = sqrtf(pa); pb = sqrtf(pb); }
-        Pf[112] = pa;
-        Pf[144] = pb;
+      {  // bin 128 = lane 0's slot 8: X[128] = conj(Z[128]), so |2X[128]|^2 = |2 Z[128]|^2
+        const float2 z = v[F512_OUT(8)];
+        const float zx = 2.f * z.x, zy = 2.f * z.y;
+        float pm = fmaf(zx, zx, zy * zy);
+        if (use_mag) pm = sqrtf(pm);
+        if (l == 0) Pf[128] = pm;
       }
+      __syncwarp();  // the next frame's stage 1 overwrites the tile
     }
     __syncwarp();
 
     // ---- epilogue over the (up to) 4 frames of this half-warp
     const int nvalid = nv;
     const int nrows = (int)max((int64_t)0, min((int64_t)SLOTS, rows_here - t0));
-    float *out = b.out + row0 * p.F;
-    if (p.feature == B200FEAT_SPECTROGRAM || p.feature == B200FEAT_LOG_SPECTROGRAM) {
+    float *out = b.out + row0 * p.F;  // the rows below are 32-bit offsets from this per-tile base
+    auto aff = [&](int col, float x) { return PLAIN ? x : post_affine(p, col, x); };
+    if (feature == B200FEAT_SPECTROGRAM || feature == B200FEAT_LOG_SPECTROGRAM) {
       for (int f = 0; f < nrows; ++f) {
-        float *o = out + (int64_t)f * p.F;
-        if (f >= nvalid) { for (int k = l; k < p.F; k += 16) o[k] = post_affine(p, k, b.pad_value); continue; }
+        float *o = out + f * p.F;
+        if (f >= nvalid) { for (int k = l; k < p.F; k += 16) o[k] = aff(k, b.pad_value); continue; }
         for (int k = l; k < p.K; k += 16) {
-          float x = P[f * PBINS + k] * (p.use_mag ? 0.5f : 0.25f);  // P holds |2X|^2 (or |2X|)
-          if (p.feature == B200FEAT_LOG_SPECTROGRAM) x = log_spec_value(p, x);
-          if (k == 0 && p.use_energy) {
+          float x = P[f * PBINS + k] * (use_mag ? 0.5f : 0.25f);  // P holds |2X|^2 (or |2X|)
+          if (feature == B200FEAT_LOG_SPECTROGRAM) x = log_spec_value(p, x);
+          if (k == 0 && use_energy) {
 #pragma unroll
             for (int g = 0; g < SLOTS; ++g) x = (f == g) ? le[g] : x;
           }
-          o[k] = post_affine(p, k, x);
+          o[k] = aff(k, x);
         }
       }
     } else {
-      const int shift = mel_shift(p), ecol = energy_col(p);
+      const int shift = PLAIN ? 0 : mel_shift(p), ecol = energy_col(p);
       const float lgk = p.log10_mel ? 0.30102999566398119521f : 0.69314718055994530942f;  // log10 (librosa_fbank.py:126) or ln
       const int Mpad = (p.M + 3) & ~3;
       float *mlog = reinterpret_cast<float *>(X);  // the transpose tile is idle during the epilogue
@@ -491,15 +528,15 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
           float r[SLOTS];
 #pragma unroll
           for (int f = 0; f < SLOTS; ++f) r[f] = fast_lg2_normal(nanmax(acc[f], p.mel_floor)) * lgk;
-          if (p.feature != B200FEAT_MFCC) {
+          if (feature != B200FEAT_MFCC) {
             float *orow = out + m + shift;
             if (nvalid == SLOTS) {  // the common case: no per-row guards
 #pragma unroll
-              for (int f = 0; f < SLOTS; ++f) orow[(int64_t)f * p.F] = post_affine(p, m + shift, r[f]);
+              for (int f = 0; f < SLOTS; ++f) orow[f * p.F] = aff(m + shift, r[f]);
             } else {
 #pragma unroll
               for (int f = 0; f < SLOTS; ++f)
-                if (f < nvalid) orow[(int64_t)f * p.F] = post_affine(p, m + shift, r[f]);
+                if (f < nvalid) orow[f * p.F] = aff(m + shift, r[f]);
             }
           } else {
 #pragma unroll
@@ -507,37 +544,38 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
           }
         }
       }
-      if (p.feature == B200FEAT_FBANK) {
-        if (p.use_energy && l < nvalid) { float v0 = 0.f;
+      if (feature == B200FEAT_FBANK) {
+        if (use_energy && l < nvalid) { float v0 = 0.f;
 #pragma unroll
           for (int f = 0; f < SLOTS; ++f) v0 = (l == f) ? le[f] : v0;
-          out[(int64_t)l * p.F + ecol] = post_affine(p, ecol, v0); }
-      } else if (p.feature == B200FEAT_MFCC) {
+          out[l * p.F + ecol] = aff(ecol, v0); }
+      } else if (feature == B200FEAT_MFCC) {
         __syncwarp();
         for (int idx = l; idx < nvalid * p.C; idx += 16) {
           const int f = idx / p.C, c = idx - f * p.C;
           float acc = 0.f;
           for (int m = 0; m < p.M; ++m) acc = fmaf(mlog[f * Mpad + m], __ldg(p.dct + m * p.C + c), acc);
           if (p.use_lifter) acc *= __ldg(p.lifter + c);
-          if (p.use_energy && c == ecol) {
+          if (use_energy && c == ecol) {
 #pragma unroll
             for (int g = 0; g < SLOTS; ++g) acc = (f == g) ? le[g] : acc; }
-          out[(int64_t)f * p.F + c] = post_affine(p, c, acc);
+          out[f * p.F + c] = aff(c, acc);
         }
       }
-      // padded tail rows
-      for (int f = nvalid; f < nrows; ++f)
-        for (int k = l; k < p.F; k += 16) out[(int64_t)f * p.F + k] = post_affine(p, k, b.pad_value);
+      // padded tail rows (packed output has none: nrows == nvalid)
+      if (padded)
+        for (int f = nvalid; f < nrows; ++f)
+          for (int k = l; k < p.F; k += 16) out[f * p.F + k] = aff(k, b.pad_value);
     }
     __syncwarp();
   }
 }
 
 // ---------------------------------------------------------------------------------------------- host
-// Launch shapes on the headline workload (bench.py, h audio/s, H100 SXM with a 400 W power limit,
-// profiles/h100_launch_shapes.jsonl, two alternating runs each):
-//   {8 warps, 4 slots, twiddles in registers, 2 CTAs/SM}  2355 / 2338   <- variant 0, what ships
-//   {10, 2, shared, 2}  (20 warps/SM, 96 registers)       2267 / 2262
+// Launch shapes on the headline workload (kernel ms per launch of 2048 x 10 s cuts, scripts/variant_bench.py, H100 SXM with a
+// 400 W power limit, profiles/h100_launch_shapes.jsonl):
+//   {8 warps, 4 slots, twiddles in registers, 2 CTAs/SM}  1.796 / 1.767   <- variant 0, what ships
+//   {10, 2, shared, 2}  (20 warps/SM, 96 registers)       1.859
 // Only variants 0 and 2 stay instantiated; B200FEAT_FAST_VARIANT=2 selects the high-occupancy shape for A/B runs.
 struct Fast512Variant { int warps, slots, tws, minb; };
 static const Fast512Variant kFast512Variants[] = {
@@ -571,36 +609,45 @@ static int f512_upload(const std::vector<T> &h, std::vector<void *> &allocs, con
   return 0;
 }
 
-// one instantiation per (dtype, compile-time L, variant); `launch` == false only raises the shared-memory limit
-template <int DT, int LCT, int V>
+// one instantiation per (dtype, compile-time L, variant, plain log-mel or not); `launch` == false only raises the
+// shared-memory limit
+template <int DT, int LCT, int V, bool PLAIN>
 static int f512_go(bool launch, size_t smem, const DevPlan &p, const Fast512Tables &t, const DevBatch &b, dim3 grid,
                    cudaStream_t stream) {
   constexpr int W = V == 2 ? 10 : 8;
   constexpr int S = V == 2 ? 2 : 4;
   constexpr int TW = V == 2 ? 1 : 0;
   constexpr int MB = 2;
-  auto kern = b200feat_fast512_kernel<DT, LCT, W, S, TW, MB>;
+  auto kern = b200feat_fast512_kernel<DT, LCT, W, S, TW, MB, PLAIN>;
   if (!launch)
     return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
   kern<<<grid, dim3(W * 32), smem, stream>>>(p, t, b);
   return 0;
 }
 
-template <int DT, int LCT>
+template <int DT, int LCT, bool PLAIN>
 static int f512_dispatch_variant(int v, bool launch, size_t smem, const DevPlan &p, const Fast512Tables &t, const DevBatch &b,
                                  dim3 grid, cudaStream_t stream) {
-  if (v == 2) return f512_go<DT, LCT, 2>(launch, smem, p, t, b, grid, stream);
-  return f512_go<DT, LCT, 0>(launch, smem, p, t, b, grid, stream);
+  if (v == 2) return f512_go<DT, LCT, 2, PLAIN>(launch, smem, p, t, b, grid, stream);
+  return f512_go<DT, LCT, 0, PLAIN>(launch, smem, p, t, b, grid, stream);
 }
 
+template <bool PLAIN>
 static int f512_dispatch(int v, int dt, int L, bool launch, size_t smem, const DevPlan &p, const Fast512Tables &t,
                          const DevBatch &b, dim3 grid, cudaStream_t stream) {
   if (L == 400) {
-    if (dt == B200FEAT_I16) return f512_dispatch_variant<B200FEAT_I16, 400>(v, launch, smem, p, t, b, grid, stream);
-    return f512_dispatch_variant<B200FEAT_F32, 400>(v, launch, smem, p, t, b, grid, stream);
+    if (dt == B200FEAT_I16) return f512_dispatch_variant<B200FEAT_I16, 400, PLAIN>(v, launch, smem, p, t, b, grid, stream);
+    return f512_dispatch_variant<B200FEAT_F32, 400, PLAIN>(v, launch, smem, p, t, b, grid, stream);
   }
-  if (dt == B200FEAT_I16) return f512_dispatch_variant<B200FEAT_I16, 0>(v, launch, smem, p, t, b, grid, stream);
-  return f512_dispatch_variant<B200FEAT_F32, 0>(v, launch, smem, p, t, b, grid, stream);
+  if (dt == B200FEAT_I16) return f512_dispatch_variant<B200FEAT_I16, 0, PLAIN>(v, launch, smem, p, t, b, grid, stream);
+  return f512_dispatch_variant<B200FEAT_F32, 0, PLAIN>(v, launch, smem, p, t, b, grid, stream);
+}
+
+// The plain log-mel instantiation serves a launch when the plan has no energy column and no magnitude spectrum, no output
+// affine is set (b200feat_set_output_affine) and the output is packed; everything else takes the general one.
+static inline bool fast512_plain(const DevPlan &p, const DevBatch &b) {
+  return p.feature == B200FEAT_FBANK && !p.use_energy && !p.use_mag && p.post_scale == nullptr &&
+         b.out_mode == B200FEAT_OUT_PACKED;
 }
 
 static inline int fast512_prepare(DevPlan &p, const std::vector<float> &bank, std::vector<void *> &allocs,
@@ -612,7 +659,7 @@ static inline int fast512_prepare(DevPlan &p, const std::vector<float> &bank, st
     if (v >= 0 && v < F512_NUM_VARIANTS) hst.variant = v;
   }
   const Fast512Variant var = kFast512Variants[hst.variant];
-  std::vector<float2> win2(256), tw1(256), w512(16);
+  std::vector<float2> win2(256), tw1(256), w512(128);
   for (int n1 = 0; n1 < 16; ++n1)
     for (int l = 0; l < 16; ++l) {
       const int j0 = 32 * n1 + 2 * l;
@@ -623,10 +670,11 @@ static inline int fast512_prepare(DevPlan &p, const std::vector<float> &bank, st
       const double a = -2.0 * M_PI * (double)((l * k1) % 256) / 256.0;
       tw1[k1 * 16 + l] = make_float2((float)cos(a), (float)sin(a));
     }
-  for (int l = 0; l < 16; ++l) {
-    const double a = -2.0 * M_PI * (double)l / 512.0;
-    w512[l] = make_float2((float)cos(a), (float)sin(a));
-  }
+  for (int i = 0; i < 8; ++i)
+    for (int l = 0; l < 16; ++l) {
+      const double a = -2.0 * M_PI * (double)(l + 16 * i) / 512.0;
+      w512[i * 16 + l] = make_float2((float)cos(a), (float)sin(a));
+    }
   int rc;
   if ((rc = f512_upload(tw1, allocs, &hst.t.tw1))) return rc;
   if ((rc = f512_upload(w512, allocs, &hst.t.w512))) return rc;
@@ -667,7 +715,9 @@ static inline int fast512_prepare(DevPlan &p, const std::vector<float> &bank, st
   DevBatch none{};
   for (int dt = 0; dt < 2; ++dt)
     for (int L : {400, 0})
-      if (f512_dispatch(hst.variant, dt, L, false, hst.smem, p, hst.t, none, dim3(1), nullptr)) return B200FEAT_ECUDA;
+      if (f512_dispatch<false>(hst.variant, dt, L, false, hst.smem, p, hst.t, none, dim3(1), nullptr) ||
+          f512_dispatch<true>(hst.variant, dt, L, false, hst.smem, p, hst.t, none, dim3(1), nullptr))
+        return B200FEAT_ECUDA;
   *out = hst;
   *frames_per_tile = 2 * var.warps * var.slots;
   return 0;
@@ -679,6 +729,8 @@ static inline int fast512_launch(const DevPlan &p, const Fast512Host &hst, const
   int64_t blocks = b.num_tiles;
   const int64_t cap = (int64_t)sm_count * var.minb;
   if (blocks > cap) blocks = cap;
-  f512_dispatch(hst.variant, dt, p.L == 400 ? 400 : 0, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
+  const int L = p.L == 400 ? 400 : 0;
+  if (fast512_plain(p, b)) f512_dispatch<true>(hst.variant, dt, L, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
+  else f512_dispatch<false>(hst.variant, dt, L, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
   return (int)cudaGetLastError();
 }

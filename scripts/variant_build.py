@@ -25,11 +25,11 @@ def one(spec):
         return name, "FAILED\n" + res.stderr[-2000:]
     log = res.stdout + res.stderr
     regs = [ln for ln in log.splitlines() if "fast512_kernelILi0ELi400ELi8ELi4" in ln or "Used" in ln]
-    # registers / spills of the headline instantiation
+    # registers / spills of the headline instantiation (F32, L = 400, variant 0, plain log-mel)
     info = ""
     lines = log.splitlines()
     for i, ln in enumerate(lines):
-        if "Compiling entry function" in ln and "fast512_kernelILi0ELi400ELi8ELi4ELi0ELi2" in ln:
+        if "Compiling entry function" in ln and "fast512_kernelILi0ELi400ELi8ELi4ELi0ELi2ELb1E" in ln:
             info = " | ".join(x.strip() for x in lines[i + 1:i + 4])
     return name, info
 
