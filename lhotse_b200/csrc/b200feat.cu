@@ -31,7 +31,7 @@ thread_local std::string g_error;
 struct HostRing {  // grow-only staging for b200feat_extract_host
   void *d_samples = nullptr; size_t d_samples_cap = 0;
   float *d_out = nullptr; size_t d_out_cap = 0;
-  int64_t *d_meta = nullptr; size_t d_meta_cap = 0;
+  int64_t *d_meta = nullptr; size_t d_meta_cap = 0;  // bytes
   int64_t *h_meta = nullptr; size_t h_meta_cap = 0;  // pinned
   cudaStream_t streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t meta_ready = nullptr;
@@ -121,6 +121,32 @@ static void stream_copy(void *dst, const void *src, size_t bytes) {
   _mm_sfence();
 }
 
+// Makes `device` current for the guard's lifetime and then restores the caller's current device.
+class DeviceGuard {
+ public:
+  explicit DeviceGuard(int device) : device_(device) {
+    cudaGetDevice(&prev_);
+    if (prev_ != device_) cudaSetDevice(device_);
+  }
+  ~DeviceGuard() {
+    if (prev_ != device_) cudaSetDevice(prev_);
+  }
+
+ private:
+  int device_, prev_ = 0;
+};
+
+// grow-only staging buffer (device or pinned host): reallocated with 25 % headroom when `need` bytes do not fit
+cudaError_t grow(void **p, size_t *cap, size_t need, bool pinned) {
+  if (*cap >= need) return cudaSuccess;
+  if (*p) { if (pinned) cudaFreeHost(*p); else cudaFree(*p); }
+  *p = nullptr; *cap = 0;
+  const size_t want = need + need / 4;
+  cudaError_t e = pinned ? cudaMallocHost(p, want) : cudaMalloc(p, want);
+  if (e == cudaSuccess) *cap = want;
+  return e;
+}
+
 }  // namespace
 
 struct b200feat_handle {
@@ -166,12 +192,7 @@ int fail(b200feat_handle *h, int code, const std::string &msg) {
 
 template <typename T>
 int upload(b200feat_handle *h, const T *src, size_t count, const T **dst) {
-  void *d = nullptr;
-  if (count == 0) { *dst = nullptr; return 0; }
-  CU_TRY(h, cudaMalloc(&d, count * sizeof(T)));
-  h->allocs.push_back(d);
-  CU_TRY(h, cudaMemcpy(d, src, count * sizeof(T), cudaMemcpyHostToDevice));
-  *dst = reinterpret_cast<const T *>(d);
+  CU_TRY(h, upload_table(src, count, h->allocs, dst));
   return 0;
 }
 
@@ -206,6 +227,344 @@ bool framable(const b200feat_plan_desc &d, int64_t n, int64_t T) {
   const int64_t right = (T - 1) * S + L - n - left;
   return left <= n && right <= n;
 }
+
+// Frames of cut i of n samples, or B200FEAT_ESHORT (naming the cut) if it is too short to be framed.
+int64_t cut_frames(b200feat_handle *h, int i, int64_t n) {
+  const int64_t T = frames_for(h->desc, n);
+  if (!framable(h->desc, n, T))
+    return fail(h, B200FEAT_ESHORT, "cut " + std::to_string(i) + " with " + std::to_string(n) + " samples is too short to be framed");
+  return T;
+}
+
+// Everything of b200feat_create after its argument and device checks: derived plan, device tables, kernel choice.  On
+// failure the caller destroys the half-built handle.
+int setup_handle(b200feat_handle *h, const float *window, const float *mel_bank, const float *dct, const float *lifter) {
+  const b200feat_plan_desc *desc = &h->desc;
+  const int L = desc->frame_length, S = desc->frame_shift, N = desc->fft_length;
+  const bool whisper = desc->feature == B200FEAT_WHISPER_FBANK;
+  const bool log10fb = desc->feature == B200FEAT_LOG10_FBANK;
+  const bool mel = desc->feature == B200FEAT_FBANK || desc->feature == B200FEAT_MFCC || whisper || log10fb;
+  DevPlan &p = h->plan;
+  memset(&p, 0, sizeof(p));
+  p.feature = desc->feature; p.L = L; p.S = S; p.N = N; p.K = N / 2 + 1;
+  p.M = mel ? desc->num_filters : 0;
+  p.C = desc->feature == B200FEAT_MFCC ? desc->num_ceps : 0;
+  p.packed = (N % 2 == 0);
+  p.Nc = p.packed ? N / 2 : N;
+  p.pad_mode = desc->pad_mode;
+  p.whisper = whisper ? 1 : 0;
+  p.log10_mel = (whisper || log10fb) ? 1 : 0;
+  p.pad_left = desc->pad_mode == B200FEAT_PAD_CENTER ? N / 2 : (L - S) / 2;
+  p.snip_edges = desc->snip_edges; p.remove_dc = desc->remove_dc_offset;
+  p.use_energy = desc->use_energy != 0; p.raw_energy = desc->raw_energy; p.use_mag = desc->use_fft_mag;
+  p.energy_last = desc->use_energy == 2 && (desc->feature == B200FEAT_FBANK || desc->feature == B200FEAT_MFCC);
+  p.energy_style = desc->energy_style; p.use_lifter = desc->use_lifter;
+  p.preemph = desc->preemph_coeff;
+  const bool has_floor = desc->energy_style == B200FEAT_ENERGY_KALDI ? desc->energy_floor != 0.f
+                                                                      : desc->energy_floor > 0.f;
+  p.has_energy_floor = has_floor ? 1.f : 0.f;
+  p.energy_floor_log = has_floor ? (float)log((double)desc->energy_floor) : 0.f;
+  p.mel_floor = desc->mel_floor;
+  p.log_spec_eps = desc->log_spec_eps < 0.f ? 0.f : desc->log_spec_eps;
+  p.log_spec_floor = desc->log_spec_eps < 0.f ? -desc->log_spec_eps : 0.f;
+  switch (desc->feature) {
+    case B200FEAT_FBANK: p.F = p.M + (desc->use_energy ? 1 : 0); break;
+    case B200FEAT_WHISPER_FBANK: p.F = p.M; break;
+    case B200FEAT_LOG10_FBANK: p.F = p.M; break;
+    case B200FEAT_MFCC: p.F = p.C; break;
+    default: p.F = p.K;
+  }
+  std::vector<int> fac = factorize(p.Nc);
+  if ((int)fac.size() > B200_MAX_STAGES) return fail(nullptr, B200FEAT_EUNSUPPORTED, "too many FFT stages");
+  p.nstages = (int)fac.size();
+  for (int i = 0; i < p.nstages; ++i) p.radix[i] = fac[i];
+
+  // host copies kept for get_table and for the fast kernel's derived tables
+  h->h_window.assign(window, window + L);
+  if (mel) h->h_bank.assign(mel_bank, mel_bank + (size_t)p.K * p.M);
+  if (p.C) h->h_dct.assign(dct, dct + (size_t)p.M * p.C);
+  if (desc->use_lifter) h->h_lifter.assign(lifter, lifter + p.C);
+
+  int rc = 0;
+#define UP(expr) do { if ((rc = (expr))) return rc; } while (0)
+  UP(upload(h, h->h_window.data(), (size_t)L, &p.window));
+  // twiddles in double, rounded once
+  h->h_tw.resize(p.Nc);
+  for (int k = 0; k < p.Nc; ++k) {
+    const double a = -2.0 * M_PI * (double)k / (double)p.Nc;
+    h->h_tw[k] = make_float2((float)cos(a), (float)sin(a));
+  }
+  UP(upload(h, h->h_tw.data(), (size_t)p.Nc, &p.tw));
+  if (p.packed) {
+    std::vector<float2> tws(p.K);
+    for (int k = 0; k < p.K; ++k) {
+      const double a = -2.0 * M_PI * (double)k / (double)N;
+      tws[k] = make_float2((float)cos(a), (float)sin(a));
+    }
+    UP(upload(h, tws.data(), tws.size(), &p.tws));
+  }
+  std::vector<int> mstart, mlen, mwoff;
+  std::vector<float> mw;
+  if (mel) {  // sparse form: contiguous support [first, last] of each filter column
+    mstart.resize(p.M); mlen.resize(p.M); mwoff.resize(p.M);
+    for (int m = 0; m < p.M; ++m) {
+      int first, last;
+      const bool any = filter_support(mel_bank, p.K, p.M, m, &first, &last);
+      mstart[m] = any ? first : 0;
+      mlen[m] = any ? last - first + 1 : 0;
+      mwoff[m] = (int)mw.size();
+      for (int k = 0; k < mlen[m]; ++k) mw.push_back(mel_bank[(size_t)(mstart[m] + k) * p.M + m]);
+    }
+    if (mw.empty()) mw.push_back(0.f);
+    UP(upload(h, mstart.data(), mstart.size(), &p.mel_start));
+    UP(upload(h, mlen.data(), mlen.size(), &p.mel_len));
+    UP(upload(h, mwoff.data(), mwoff.size(), &p.mel_woff));
+    UP(upload(h, mw.data(), mw.size(), &p.mel_w));
+  }
+  if (p.C) UP(upload(h, h->h_dct.data(), h->h_dct.size(), &p.dct));
+  if (desc->use_lifter) UP(upload(h, h->h_lifter.data(), h->h_lifter.size(), &p.lifter));
+
+  // ---- kernel selection
+  // the whisper-fbank epilogue / centre padding exist in the generic and the fast400 kernels only; the tensor-core kernel
+  // (tc512.cuh) serves the N = 512 fbank / mfcc plans without an energy column
+  const bool tc_ok = !whisper && tc512_supported(p);
+  if (desc->kernel == B200FEAT_KERNEL_TC && !tc_ok)
+    return fail(nullptr, B200FEAT_EUNSUPPORTED, "the tensor-core kernel needs fft_length 512, fbank / mfcc without use_energy, Kaldi framing");
+  const bool fast512_ok = !whisper && fast512_supported(p);
+  const bool fast256_ok = !whisper && fast256_supported(p);
+  const bool fast1024_ok = !whisper && fast1024_supported(p);
+  const bool fast400_ok = fast400_supported(p);
+  const bool fast2048_ok = !whisper && fast2048_supported(p);
+  const bool fast_ok = fast512_ok || fast256_ok || fast1024_ok || fast2048_ok || fast400_ok;
+  if (desc->kernel == B200FEAT_KERNEL_FAST && !fast_ok)
+    return fail(nullptr, B200FEAT_EUNSUPPORTED, "fast kernels require fft_length 256, 512, 1024, 2048 or frame_length = fft_length = 400");
+  bool auto_tc = false;  // AUTO prefers the tensor-core kernel where it is the faster one (B200FEAT_AUTO_TC=0/1 overrides)
+  if (const char *e = getenv("B200FEAT_AUTO_TC")) auto_tc = atoi(e) != 0;
+  if (desc->kernel == B200FEAT_KERNEL_TC || (desc->kernel == B200FEAT_KERNEL_AUTO && tc_ok && auto_tc)) h->kernel = B200FEAT_KERNEL_TC;
+  else if (desc->kernel == B200FEAT_KERNEL_GENERIC || !fast_ok) h->kernel = B200FEAT_KERNEL_GENERIC;
+  else h->kernel = B200FEAT_KERNEL_FAST;
+
+  {  // generic launch shape: as many warps per CTA as fit ~100 KB, CTA <= 8 warps
+    const size_t per_warp = generic_smem_per_warp(p.N, p.Nc);
+    int w = (int)((100 * 1024) / per_warp);
+    if (w > 8) w = 8;
+    if (w < 1) w = 1;
+    h->generic_warps = w;
+    h->generic_smem = per_warp * w;
+    if (h->generic_smem > 227 * 1024)
+      return fail(nullptr, B200FEAT_EUNSUPPORTED, "fft_length too large for shared memory");
+    if (h->generic_smem > 48 * 1024) {
+      cudaError_t e1 = cudaFuncSetAttribute(b200feat_generic_kernel<B200FEAT_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->generic_smem);
+      cudaError_t e2 = cudaFuncSetAttribute(b200feat_generic_kernel<B200FEAT_I16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->generic_smem);
+      if (e1 != cudaSuccess || e2 != cudaSuccess)
+        return fail(nullptr, B200FEAT_ECUDA, "cudaFuncSetAttribute(generic smem) failed");
+    }
+  }
+  h->frames_per_tile = 1;
+  if (h->kernel == B200FEAT_KERNEL_TC) {
+    rc = tc512_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->tc);
+    if (rc == B200FEAT_EUNSUPPORTED && desc->kernel == B200FEAT_KERNEL_AUTO) {
+      h->kernel = fast_ok ? B200FEAT_KERNEL_FAST : B200FEAT_KERNEL_GENERIC;
+      h->frames_per_tile = 1;
+      rc = 0;
+    } else if (rc)
+      return fail(nullptr, rc, "tensor-core kernel cannot be prepared for this plan");
+  }
+  if (h->kernel == B200FEAT_KERNEL_FAST) {
+    if (h->plan.N == 256) rc = fast256_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast256);
+    else if (h->plan.N == 400) rc = fast400_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast400);
+    else if (h->plan.N == 1024) rc = fast1024_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast1024);
+    else if (h->plan.N == 2048) rc = fast2048_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast2048);
+    else rc = fast512_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast);
+    if (rc == B200FEAT_EUNSUPPORTED && desc->kernel == B200FEAT_KERNEL_AUTO) {
+      h->kernel = B200FEAT_KERNEL_GENERIC;  // e.g. the plan's tables do not fit the fast kernel's shared memory
+      h->frames_per_tile = 1;
+    } else if (rc)
+      return fail(nullptr, rc, "fast kernel cannot be prepared for this plan (shared-memory footprint?)");
+  }
+#undef UP
+  return 0;
+}
+
+// launches the selected kernel over cuts [b0, b1) of a planned batch
+int launch_range(b200feat_handle *h, const void *samples_dev, int32_t dt, const int64_t *meta_dev,
+                        int32_t B, int32_t b0, int32_t b1, int64_t tile0, int64_t tile1,
+                        int64_t max_frames, float *out_dev, int32_t out_mode, float pad_value,
+                        cudaStream_t stream, float *cut_max_dev = nullptr, int64_t norm_rows = 0) {
+  DevBatch db;
+  db.samples = samples_dev;
+  db.samp_off = meta_dev + b0;
+  db.nsamp = meta_dev + B + b0;
+  db.row_off = meta_dev + 2 * (int64_t)B + b0;
+  db.tile_off = meta_dev + 3 * (int64_t)B + 1 + b0;
+  db.tile_cut = h->frames_per_tile > 1 ? reinterpret_cast<const int32_t *>(meta_dev + 4 * (int64_t)B + 2) : nullptr;
+  db.out = out_dev;
+  db.cut_max = cut_max_dev ? cut_max_dev + b0 : nullptr;
+  db.tile_base = tile0;
+  db.num_tiles = tile1 - tile0;
+  db.max_frames = max_frames;
+  db.batch_first = b0;
+  db.B = b1 - b0;
+  db.out_mode = out_mode;
+  db.pad_value = pad_value;
+  if (db.num_tiles <= 0) return 0;
+  if (h->plan.whisper) {
+    if (!cut_max_dev) return fail(h, B200FEAT_EINVAL, "whisper-fbank: scratch missing");
+    cudaError_t e = cudaMemsetAsync(db.cut_max, 0xff, (size_t)db.B * sizeof(float), stream);  // "empty" (common.cuh)
+    if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("memset(cut_max): ") + cudaGetErrorString(e));
+  }
+  if (h->kernel == B200FEAT_KERNEL_TC || h->kernel == B200FEAT_KERNEL_FAST) {
+    const char *name;
+    int rc;
+    if (h->kernel == B200FEAT_KERNEL_TC) { name = "tc512"; rc = tc512_launch(h->plan, h->tc, db, dt, h->sm_count, stream); }
+    else if (h->plan.N == 256) { name = "fast256"; rc = fast256_launch(h->plan, h->fast256, db, dt, h->sm_count, stream); }
+    else if (h->plan.N == 400) { name = "fast400"; rc = fast400_launch(h->plan, h->fast400, db, dt, h->sm_count, stream); }
+    else if (h->plan.N == 1024) { name = "fast1024"; rc = fast1024_launch(h->plan, h->fast1024, db, dt, h->sm_count, stream); }
+    else if (h->plan.N == 2048) { name = "fast2048"; rc = fast2048_launch(h->plan, h->fast2048, db, dt, h->sm_count, stream); }
+    else { name = "fast512"; rc = fast512_launch(h->plan, h->fast, db, dt, h->sm_count, stream); }
+    if (rc) return fail(h, B200FEAT_ECUDA, std::string(name) + " launch: " + cudaGetErrorString((cudaError_t)rc));
+  } else {
+    const int w = h->generic_warps;
+    const unsigned blocks = persistent_grid((db.num_tiles + w - 1) / w, h->sm_count, 8);
+    if (dt == B200FEAT_I16)
+      b200feat_generic_kernel<B200FEAT_I16><<<blocks, w * 32, h->generic_smem, stream>>>(h->plan, db);
+    else
+      b200feat_generic_kernel<B200FEAT_F32><<<blocks, w * 32, h->generic_smem, stream>>>(h->plan, db);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("generic launch: ") + cudaGetErrorString(e));
+  }
+  if (h->plan.whisper && norm_rows > 0) {  // second launch: clamp to the cut's maximum - 8, (x + 4) / 4, zero rows
+    if (h->frames_per_tile > 1) {
+      const unsigned blocks = persistent_grid(db.num_tiles, h->sm_count, 8);
+      b200feat_whisper_normalize_tiled_kernel<<<blocks, 256, 0, stream>>>(h->plan, db, h->frames_per_tile);
+    } else {
+      const unsigned blocks = persistent_grid((norm_rows + 7) / 8, h->sm_count, 16);
+      b200feat_whisper_normalize_kernel<<<blocks, 256, 0, stream>>>(h->plan, db, norm_rows);
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("whisper normalise launch: ") + cudaGetErrorString(e));
+  }
+  return 0;
+}
+
+// Copies cuts [b0, b1) into the pinned slot `stage` at their planned offsets relative to the chunk's first sample, with
+// the alignment gaps zeroed: one task per ~1 MB piece so that long and short cuts balance over the pool's threads.
+void gather_chunk(GatherPool *pool, unsigned char *stage, const void *const *cuts, const int64_t *soff, const int64_t *num_samples,
+                  int b0, int b1, size_t esz) {
+  struct Piece { const unsigned char *src; unsigned char *dst; size_t bytes; };
+  std::vector<Piece> pieces;
+  const int64_t e0 = soff[b0];
+  for (int i = b0; i < b1; ++i) {
+    const unsigned char *src = static_cast<const unsigned char *>(cuts[i]);
+    unsigned char *dst = stage + (size_t)(soff[i] - e0) * esz;
+    size_t left = (size_t)num_samples[i] * esz;
+    while (left) {
+      const size_t take = std::min(left, (size_t)1 << 20);
+      pieces.push_back({src, dst, take});
+      src += take; dst += take; left -= take;
+    }
+    if (i + 1 < b1) {  // alignment gap before the next cut: defined bytes only
+      const size_t gap = (size_t)(soff[i + 1] - soff[i] - num_samples[i]) * esz;
+      if (gap) memset(stage + (size_t)(soff[i] + num_samples[i] - e0) * esz, 0, gap);
+    }
+  }
+  const std::function<void(int)> job = [&](int k) { stream_copy(pieces[k].dst, pieces[k].src, pieces[k].bytes); };
+  pool->parallel_for((int)pieces.size(), job);
+}
+
+// b200feat_extract_host_at / _ptrs after their argument checks.  The samples come either from one host buffer `src` laid
+// out as the batch's offsets say (copied a chunk at a time, verbatim), or from one pointer per cut `cuts` (gathered a chunk
+// at a time into one of two pinned slots while the other slot's copy is in flight).
+int extract_staged(b200feat_handle *h, const void *src, const void *const *cuts, int32_t dt, const int64_t *num_samples,
+                   const int64_t *sample_offsets, int32_t B, float *out_host, int32_t out_mode, float pad_value) {
+  HostRing &r = h->ring;
+  std::lock_guard<std::mutex> guard(r.mu);
+  DeviceGuard on(h->device);
+
+  const size_t esz = dt == B200FEAT_I16 ? 2 : 4;
+  // gathered cuts start on a 16-byte boundary of the device buffer; a caller's buffer keeps its own layout on the device
+  const int32_t align = cuts ? (dt == B200FEAT_I16 ? 8 : 4) : 1;
+  const int64_t words = b200feat_plan_words(h, num_samples, B, out_mode);
+  if (words < 0) return (int)words;
+  if (r.h_meta_cap < (size_t)words) {
+    if (r.h_meta) cudaFreeHost(r.h_meta);
+    r.h_meta = nullptr; r.h_meta_cap = 0;
+    CU_TRY(h, cudaMallocHost((void **)&r.h_meta, (size_t)words * 8));
+    r.h_meta_cap = (size_t)words;
+  }
+  b200feat_batch_totals tot;
+  int rc = b200feat_plan_batch(h, num_samples, sample_offsets, B, align, out_mode, r.h_meta, words, &tot);
+  if (rc) return rc;
+  for (auto &s : r.streams) if (!s) CU_TRY(h, cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  if (!r.meta_ready) CU_TRY(h, cudaEventCreateWithFlags(&r.meta_ready, cudaEventDisableTiming));
+  if (cuts) {
+    for (int k = 0; k < 2; ++k)
+      if (!r.stage_free[k]) CU_TRY(h, cudaEventCreateWithFlags(&r.stage_free[k], cudaEventDisableTiming));
+    if (!h->pool) {
+      int nthreads = 8;
+      if (const char *e = getenv("B200FEAT_STAGING_THREADS")) nthreads = std::max(1, atoi(e));
+      h->pool = new GatherPool(nthreads - 1);  // the calling thread works too
+    }
+  }
+  CU_TRY(h, grow(&r.d_samples, &r.d_samples_cap, (size_t)tot.span_samples * esz + 16, false));
+  CU_TRY(h, grow((void **)&r.d_out, &r.d_out_cap, (size_t)tot.out_floats * 4 + 16, false));
+  CU_TRY(h, grow((void **)&r.d_meta, &r.d_meta_cap, (size_t)words * 8, false));
+  CU_TRY(h, cudaMemcpyAsync(r.d_meta, r.h_meta, (size_t)words * 8, cudaMemcpyHostToDevice, r.streams[0]));
+  CU_TRY(h, cudaEventRecord(r.meta_ready, r.streams[0]));
+
+  // chunks of cuts with ~32 MB of samples each, round-robin over 3 streams so that H2D(i+1), kernel(i) and D2H(i-1)
+  // overlap (PCIe is the end-to-end bound, SURVEY.md §7)
+  const int64_t *soff = r.h_meta, *roff = r.h_meta + 2 * (int64_t)B, *toff = r.h_meta + 3 * (int64_t)B + 1;
+  const int64_t chunk_elems = (32ll << 20) / (int64_t)esz;
+  std::vector<int> cb{0};  // chunk boundaries
+  for (int b0 = 0; b0 < B;) {
+    int b1 = b0 + 1;
+    while (b1 < B && (soff[b1] + num_samples[b1]) - soff[b0] <= chunk_elems) ++b1;
+    cb.push_back(b1);
+    b0 = b1;
+  }
+  const size_t nchunks = cb.size() - 1;
+  if (cuts) {  // the staging slots must hold the largest chunk
+    size_t max_bytes = 0;
+    for (size_t c = 0; c < nchunks; ++c)
+      max_bytes = std::max(max_bytes, (size_t)((soff[cb[c + 1] - 1] + num_samples[cb[c + 1] - 1]) - soff[cb[c]]) * esz);
+    for (int k = 0; k < 2; ++k) CU_TRY(h, grow(&r.h_stage[k], &r.h_stage_cap[k], max_bytes + 64, true));
+  }
+
+  float *scratch = h->plan.whisper ? r.d_out + (tot.out_floats - B) : nullptr;
+  int launches = 0;
+  for (size_t c = 0; c < nchunks; ++c) {
+    const int b0 = cb[c], b1 = cb[c + 1], slot = (int)(c & 1);
+    cudaStream_t st = r.streams[c % 3];
+    if (c < 3) CU_TRY(h, cudaStreamWaitEvent(st, r.meta_ready, 0));
+    const int64_t e0 = soff[b0], e1 = soff[b1 - 1] + num_samples[b1 - 1];
+    const void *chunk = static_cast<const char *>(src) + e0 * esz;
+    if (cuts) {
+      if (c >= 2) CU_TRY(h, cudaEventSynchronize(r.stage_free[slot]));  // the H2D copy out of this slot (chunk c - 2) is done
+      gather_chunk(h->pool, static_cast<unsigned char *>(r.h_stage[slot]), cuts, soff, num_samples, b0, b1, esz);
+      chunk = r.h_stage[slot];
+    }
+    CU_TRY(h, cudaMemcpyAsync((char *)r.d_samples + e0 * esz, chunk, (size_t)(e1 - e0) * esz, cudaMemcpyHostToDevice, st));
+    if (cuts) CU_TRY(h, cudaEventRecord(r.stage_free[slot], st));
+    int64_t f0, f1;
+    if (out_mode == B200FEAT_OUT_PADDED) { f0 = (int64_t)b0 * tot.max_frames; f1 = (int64_t)b1 * tot.max_frames; }
+    else { f0 = roff[b0]; f1 = roff[b1]; }
+    rc = launch_range(h, r.d_samples, dt, r.d_meta, B, b0, b1, toff[b0], toff[b1], tot.max_frames, r.d_out, out_mode, pad_value, st,
+                      scratch, f1 - f0);
+    if (rc) return rc;
+    launches += h->plan.whisper ? 2 : 1;
+    CU_TRY(h, cudaMemcpyAsync(out_host + f0 * h->plan.F, r.d_out + f0 * h->plan.F, (size_t)(f1 - f0) * h->plan.F * 4,
+                              cudaMemcpyDeviceToHost, st));
+  }
+  for (auto &s : r.streams) CU_TRY(h, cudaStreamSynchronize(s));
+  {
+    std::lock_guard<std::mutex> g(h->stats_mu);
+    h->stats.calls++; h->stats.cuts += B; h->stats.frames += tot.total_rows;
+    h->stats.samples += tot.span_samples; h->stats.kernel_launches += launches;
+  }
+  return B200FEAT_OK;
+}
+
 
 }  // namespace
 
@@ -258,186 +617,34 @@ int b200feat_create(const b200feat_plan_desc *desc, const float *window, const f
   h->desc = *desc;
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
-  int prev = 0;
-  cudaGetDevice(&prev);
-  cudaSetDevice(device);
-
-  DevPlan &p = h->plan;
-  memset(&p, 0, sizeof(p));
-  p.feature = desc->feature; p.L = L; p.S = S; p.N = N; p.K = N / 2 + 1;
-  p.M = mel ? desc->num_filters : 0;
-  p.C = desc->feature == B200FEAT_MFCC ? desc->num_ceps : 0;
-  p.packed = (N % 2 == 0);
-  p.Nc = p.packed ? N / 2 : N;
-  p.pad_mode = desc->pad_mode;
-  p.whisper = whisper ? 1 : 0;
-  p.log10_mel = (whisper || log10fb) ? 1 : 0;
-  p.pad_left = desc->pad_mode == B200FEAT_PAD_CENTER ? N / 2 : (L - S) / 2;
-  p.snip_edges = desc->snip_edges; p.remove_dc = desc->remove_dc_offset;
-  p.use_energy = desc->use_energy != 0; p.raw_energy = desc->raw_energy; p.use_mag = desc->use_fft_mag;
-  p.energy_last = desc->use_energy == 2 && (desc->feature == B200FEAT_FBANK || desc->feature == B200FEAT_MFCC);
-  p.energy_style = desc->energy_style; p.use_lifter = desc->use_lifter;
-  p.preemph = desc->preemph_coeff;
-  const bool has_floor = desc->energy_style == B200FEAT_ENERGY_KALDI ? desc->energy_floor != 0.f
-                                                                      : desc->energy_floor > 0.f;
-  p.has_energy_floor = has_floor ? 1.f : 0.f;
-  p.energy_floor_log = has_floor ? (float)log((double)desc->energy_floor) : 0.f;
-  p.mel_floor = desc->mel_floor;
-  p.log_spec_eps = desc->log_spec_eps < 0.f ? 0.f : desc->log_spec_eps;
-  p.log_spec_floor = desc->log_spec_eps < 0.f ? -desc->log_spec_eps : 0.f;
-  switch (desc->feature) {
-    case B200FEAT_FBANK: p.F = p.M + (desc->use_energy ? 1 : 0); break;
-    case B200FEAT_WHISPER_FBANK: p.F = p.M; break;
-    case B200FEAT_LOG10_FBANK: p.F = p.M; break;
-    case B200FEAT_MFCC: p.F = p.C; break;
-    default: p.F = p.K;
+  DeviceGuard on(device);
+  const int rc = setup_handle(h, window, mel_bank, dct, lifter);
+  if (rc) {
+    b200feat_destroy(h);
+    return rc;
   }
-  std::vector<int> fac = factorize(p.Nc);
-  if ((int)fac.size() > B200_MAX_STAGES) { delete h; return fail(nullptr, B200FEAT_EUNSUPPORTED, "too many FFT stages"); }
-  p.nstages = (int)fac.size();
-  for (int i = 0; i < p.nstages; ++i) p.radix[i] = fac[i];
-
-  // host copies kept for get_table and for the fast kernel's derived tables
-  h->h_window.assign(window, window + L);
-  if (mel) h->h_bank.assign(mel_bank, mel_bank + (size_t)p.K * p.M);
-  if (p.C) h->h_dct.assign(dct, dct + (size_t)p.M * p.C);
-  if (desc->use_lifter) h->h_lifter.assign(lifter, lifter + p.C);
-
-  int rc = 0;
-#define UP(expr) do { rc = (expr); if (rc) { cudaSetDevice(prev); b200feat_destroy(h); return rc; } } while (0)
-  UP(upload(h, h->h_window.data(), (size_t)L, &p.window));
-  // twiddles in double, rounded once
-  h->h_tw.resize(p.Nc);
-  for (int k = 0; k < p.Nc; ++k) {
-    const double a = -2.0 * M_PI * (double)k / (double)p.Nc;
-    h->h_tw[k] = make_float2((float)cos(a), (float)sin(a));
-  }
-  UP(upload(h, h->h_tw.data(), (size_t)p.Nc, &p.tw));
-  if (p.packed) {
-    std::vector<float2> tws(p.K);
-    for (int k = 0; k < p.K; ++k) {
-      const double a = -2.0 * M_PI * (double)k / (double)N;
-      tws[k] = make_float2((float)cos(a), (float)sin(a));
-    }
-    UP(upload(h, tws.data(), tws.size(), &p.tws));
-  }
-  std::vector<int> mstart, mlen, mwoff;
-  std::vector<float> mw;
-  if (mel) {  // sparse form: contiguous support [first, last] of each filter column
-    mstart.resize(p.M); mlen.resize(p.M); mwoff.resize(p.M);
-    for (int m = 0; m < p.M; ++m) {
-      int first = -1, last = -1;
-      for (int k = 0; k < p.K; ++k)
-        if (mel_bank[(size_t)k * p.M + m] != 0.f) { if (first < 0) first = k; last = k; }
-      mstart[m] = first < 0 ? 0 : first;
-      mlen[m] = first < 0 ? 0 : last - first + 1;
-      mwoff[m] = (int)mw.size();
-      for (int k = 0; k < mlen[m]; ++k) mw.push_back(mel_bank[(size_t)(mstart[m] + k) * p.M + m]);
-    }
-    if (mw.empty()) mw.push_back(0.f);
-    UP(upload(h, mstart.data(), mstart.size(), &p.mel_start));
-    UP(upload(h, mlen.data(), mlen.size(), &p.mel_len));
-    UP(upload(h, mwoff.data(), mwoff.size(), &p.mel_woff));
-    UP(upload(h, mw.data(), mw.size(), &p.mel_w));
-  }
-  if (p.C) UP(upload(h, h->h_dct.data(), h->h_dct.size(), &p.dct));
-  if (desc->use_lifter) UP(upload(h, h->h_lifter.data(), h->h_lifter.size(), &p.lifter));
-
-  // ---- kernel selection
-  // the whisper-fbank epilogue / centre padding exist in the generic and the fast400 kernels only; the tensor-core kernel
-  // (tc512.cuh) serves the N = 512 fbank / mfcc plans without an energy column
-  const bool tc_ok = !whisper && tc512_supported(p);
-  if (desc->kernel == B200FEAT_KERNEL_TC && !tc_ok) {
-    cudaSetDevice(prev); b200feat_destroy(h);
-    return fail(nullptr, B200FEAT_EUNSUPPORTED, "the tensor-core kernel needs fft_length 512, fbank / mfcc without use_energy, Kaldi framing");
-  }
-  const bool fast512_ok = !whisper && fast512_supported(p);
-  const bool fast256_ok = !whisper && fast256_supported(p);
-  const bool fast1024_ok = !whisper && fast1024_supported(p);
-  const bool fast400_ok = fast400_supported(p);
-  const bool fast2048_ok = !whisper && fast2048_supported(p);
-  const bool fast_ok = fast512_ok || fast256_ok || fast1024_ok || fast2048_ok || fast400_ok;
-  if (desc->kernel == B200FEAT_KERNEL_FAST && !fast_ok) {
-    cudaSetDevice(prev); b200feat_destroy(h);
-    return fail(nullptr, B200FEAT_EUNSUPPORTED, "fast kernels require fft_length 256, 512, 1024, 2048 or frame_length = fft_length = 400");
-  }
-  bool auto_tc = false;  // AUTO prefers the tensor-core kernel where it is the faster one (B200FEAT_AUTO_TC=0/1 overrides)
-  if (const char *e = getenv("B200FEAT_AUTO_TC")) auto_tc = atoi(e) != 0;
-  if (desc->kernel == B200FEAT_KERNEL_TC || (desc->kernel == B200FEAT_KERNEL_AUTO && tc_ok && auto_tc)) h->kernel = B200FEAT_KERNEL_TC;
-  else if (desc->kernel == B200FEAT_KERNEL_GENERIC || !fast_ok) h->kernel = B200FEAT_KERNEL_GENERIC;
-  else h->kernel = B200FEAT_KERNEL_FAST;
-
-  {  // generic launch shape: as many warps per CTA as fit ~100 KB, CTA <= 8 warps
-    const size_t per_warp = generic_smem_per_warp(p.N, p.Nc);
-    int w = (int)((100 * 1024) / per_warp);
-    if (w > 8) w = 8;
-    if (w < 1) w = 1;
-    h->generic_warps = w;
-    h->generic_smem = per_warp * w;
-    if (h->generic_smem > 227 * 1024) {
-      cudaSetDevice(prev); b200feat_destroy(h);
-      return fail(nullptr, B200FEAT_EUNSUPPORTED, "fft_length too large for shared memory");
-    }
-    if (h->generic_smem > 48 * 1024) {
-      cudaError_t e1 = cudaFuncSetAttribute(b200feat_generic_kernel<B200FEAT_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->generic_smem);
-      cudaError_t e2 = cudaFuncSetAttribute(b200feat_generic_kernel<B200FEAT_I16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->generic_smem);
-      if (e1 != cudaSuccess || e2 != cudaSuccess) {
-        cudaSetDevice(prev); b200feat_destroy(h);
-        return fail(nullptr, B200FEAT_ECUDA, "cudaFuncSetAttribute(generic smem) failed");
-      }
-    }
-  }
-  h->frames_per_tile = 1;
-  if (h->kernel == B200FEAT_KERNEL_TC) {
-    rc = tc512_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->tc);
-    if (rc == B200FEAT_EUNSUPPORTED && desc->kernel == B200FEAT_KERNEL_AUTO) {
-      h->kernel = fast_ok ? B200FEAT_KERNEL_FAST : B200FEAT_KERNEL_GENERIC;
-      h->frames_per_tile = 1;
-      rc = 0;
-    } else if (rc) {
-      cudaSetDevice(prev); b200feat_destroy(h);
-      return fail(nullptr, rc, "tensor-core kernel cannot be prepared for this plan");
-    }
-  }
-  if (h->kernel == B200FEAT_KERNEL_FAST) {
-    if (h->plan.N == 256) rc = fast256_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast256);
-    else if (h->plan.N == 400) rc = fast400_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast400);
-    else if (h->plan.N == 1024) rc = fast1024_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast1024);
-    else if (h->plan.N == 2048) rc = fast2048_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast2048);
-    else rc = fast512_prepare(h->plan, h->h_bank, h->allocs, &h->frames_per_tile, h->h_window, &h->fast);
-    if (rc == B200FEAT_EUNSUPPORTED && desc->kernel == B200FEAT_KERNEL_AUTO) {
-      h->kernel = B200FEAT_KERNEL_GENERIC;  // e.g. the plan's tables do not fit the fast kernel's shared memory
-      h->frames_per_tile = 1;
-    } else if (rc) {
-      cudaSetDevice(prev); b200feat_destroy(h);
-      return fail(nullptr, rc, "fast kernel cannot be prepared for this plan (shared-memory footprint?)");
-    }
-  }
-#undef UP
-  cudaSetDevice(prev);
   *out = h;
   return B200FEAT_OK;
 }
 
 void b200feat_destroy(b200feat_handle *h) {
   if (!h) return;
-  int prev = 0;
-  cudaGetDevice(&prev);
-  cudaSetDevice(h->device);
-  for (void *p : h->allocs) cudaFree(p);
-  HostRing &r = h->ring;
-  if (r.d_samples) cudaFree(r.d_samples);
-  if (r.d_out) cudaFree(r.d_out);
-  if (r.d_meta) cudaFree(r.d_meta);
-  if (r.h_meta) cudaFreeHost(r.h_meta);
-  for (auto &s : r.streams) if (s) cudaStreamDestroy(s);
-  if (r.meta_ready) cudaEventDestroy(r.meta_ready);
-  for (int k = 0; k < 2; ++k) {
-    if (r.h_stage[k]) cudaFreeHost(r.h_stage[k]);
-    if (r.stage_free[k]) cudaEventDestroy(r.stage_free[k]);
+  {
+    DeviceGuard on(h->device);
+    for (void *p : h->allocs) cudaFree(p);
+    HostRing &r = h->ring;
+    if (r.d_samples) cudaFree(r.d_samples);
+    if (r.d_out) cudaFree(r.d_out);
+    if (r.d_meta) cudaFree(r.d_meta);
+    if (r.h_meta) cudaFreeHost(r.h_meta);
+    for (auto &s : r.streams) if (s) cudaStreamDestroy(s);
+    if (r.meta_ready) cudaEventDestroy(r.meta_ready);
+    for (int k = 0; k < 2; ++k) {
+      if (r.h_stage[k]) cudaFreeHost(r.h_stage[k]);
+      if (r.stage_free[k]) cudaEventDestroy(r.stage_free[k]);
+    }
+    delete h->pool;
   }
-  delete h->pool;
-  cudaSetDevice(prev);
   delete h;
 }
 
@@ -468,10 +675,8 @@ int64_t b200feat_plan_words(const b200feat_handle *hc, const int64_t *num_sample
   if (ft <= 1) return words;
   int64_t tmax = 0, tiles = 0;
   for (int i = 0; i < B; ++i) {
-    const int64_t T = frames_for(h->desc, num_samples[i]);
-    if (!framable(h->desc, num_samples[i], T))
-      return fail(h, B200FEAT_ESHORT, "cut " + std::to_string(i) + " with " + std::to_string(num_samples[i]) +
-                                          " samples is too short to be framed");
+    const int64_t T = cut_frames(h, i, num_samples[i]);
+    if (T < 0) return T;
     if (T > tmax) tmax = T;
     tiles += (T + ft - 1) / ft;
   }
@@ -491,10 +696,8 @@ int b200feat_plan_batch(const b200feat_handle *hc, const int64_t *num_samples,
   int64_t cur = 0, rows = 0, tmax = 0, span = 0;
   for (int i = 0; i < B; ++i) {
     const int64_t n = num_samples[i];
-    const int64_t T = frames_for(h->desc, n);
-    if (!framable(h->desc, n, T))
-      return fail(h, B200FEAT_ESHORT, "cut " + std::to_string(i) + " with " + std::to_string(n) +
-                                          " samples is too short to be framed");
+    const int64_t T = cut_frames(h, i, n);
+    if (T < 0) return (int)T;
     if (sample_offsets) soff[i] = sample_offsets[i];
     else { cur = (cur + align - 1) / align * align; soff[i] = cur; cur += n; }
     ns[i] = n;
@@ -528,94 +731,17 @@ int b200feat_plan_batch(const b200feat_handle *hc, const int64_t *num_samples,
   return B200FEAT_OK;
 }
 
-// launches the selected kernel over cuts [b0, b1) of a planned batch
-static int launch_range(b200feat_handle *h, const void *samples_dev, int32_t dt, const int64_t *meta_dev,
-                        int32_t B, int32_t b0, int32_t b1, int64_t tile0, int64_t tile1,
-                        int64_t max_frames, float *out_dev, int32_t out_mode, float pad_value,
-                        cudaStream_t stream, float *cut_max_dev = nullptr, int64_t norm_rows = 0) {
-  DevBatch db;
-  db.samples = samples_dev;
-  db.samp_off = meta_dev + b0;
-  db.nsamp = meta_dev + B + b0;
-  db.row_off = meta_dev + 2 * (int64_t)B + b0;
-  db.tile_off = meta_dev + 3 * (int64_t)B + 1 + b0;
-  db.tile_cut = h->frames_per_tile > 1 ? reinterpret_cast<const int32_t *>(meta_dev + 4 * (int64_t)B + 2) : nullptr;
-  db.out = out_dev;
-  db.cut_max = cut_max_dev ? cut_max_dev + b0 : nullptr;
-  db.tile_base = tile0;
-  db.num_tiles = tile1 - tile0;
-  db.max_frames = max_frames;
-  db.batch_first = b0;
-  db.B = b1 - b0;
-  db.out_mode = out_mode;
-  db.pad_value = pad_value;
-  if (db.num_tiles <= 0) return 0;
-  if (h->plan.whisper) {
-    if (!cut_max_dev) return fail(h, B200FEAT_EINVAL, "whisper-fbank: scratch missing");
-    cudaError_t e = cudaMemsetAsync(db.cut_max, 0xff, (size_t)db.B * sizeof(float), stream);  // "empty" (common.cuh)
-    if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("memset(cut_max): ") + cudaGetErrorString(e));
-  }
-  if (h->kernel == B200FEAT_KERNEL_TC) {
-    int rc = tc512_launch(h->plan, h->tc, db, dt, h->sm_count, stream);
-    if (rc) return fail(h, B200FEAT_ECUDA, std::string("tc512 launch: ") + cudaGetErrorString((cudaError_t)rc));
-  } else if (h->kernel == B200FEAT_KERNEL_FAST && h->plan.N == 256) {
-    int rc = fast256_launch(h->plan, h->fast256, db, dt, h->sm_count, stream);
-    if (rc) return fail(h, B200FEAT_ECUDA, std::string("fast256 launch: ") + cudaGetErrorString((cudaError_t)rc));
-  } else if (h->kernel == B200FEAT_KERNEL_FAST && h->plan.N == 400) {
-    int rc = fast400_launch(h->plan, h->fast400, db, dt, h->sm_count, stream);
-    if (rc) return fail(h, B200FEAT_ECUDA, std::string("fast400 launch: ") + cudaGetErrorString((cudaError_t)rc));
-  } else if (h->kernel == B200FEAT_KERNEL_FAST && h->plan.N == 1024) {
-    int rc = fast1024_launch(h->plan, h->fast1024, db, dt, h->sm_count, stream);
-    if (rc) return fail(h, B200FEAT_ECUDA, std::string("fast1024 launch: ") + cudaGetErrorString((cudaError_t)rc));
-  } else if (h->kernel == B200FEAT_KERNEL_FAST && h->plan.N == 2048) {
-    int rc = fast2048_launch(h->plan, h->fast2048, db, dt, h->sm_count, stream);
-    if (rc) return fail(h, B200FEAT_ECUDA, std::string("fast2048 launch: ") + cudaGetErrorString((cudaError_t)rc));
-  } else if (h->kernel == B200FEAT_KERNEL_FAST) {
-    int rc = fast512_launch(h->plan, h->fast, db, dt, h->sm_count, stream);
-    if (rc) return fail(h, B200FEAT_ECUDA, std::string("fast512 launch: ") + cudaGetErrorString((cudaError_t)rc));
-  } else {
-    const int w = h->generic_warps;
-    int64_t blocks = (db.num_tiles + w - 1) / w;
-    const int64_t cap = (int64_t)h->sm_count * 8;
-    if (blocks > cap) blocks = cap;
-    if (dt == B200FEAT_I16)
-      b200feat_generic_kernel<B200FEAT_I16><<<(unsigned)blocks, w * 32, h->generic_smem, stream>>>(h->plan, db);
-    else
-      b200feat_generic_kernel<B200FEAT_F32><<<(unsigned)blocks, w * 32, h->generic_smem, stream>>>(h->plan, db);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("generic launch: ") + cudaGetErrorString(e));
-  }
-  if (h->plan.whisper && norm_rows > 0) {  // second launch: clamp to the cut's maximum - 8, (x + 4) / 4, zero rows
-    if (h->frames_per_tile > 1) {
-      int64_t blocks = db.num_tiles;
-      const int64_t cap = (int64_t)h->sm_count * 8;
-      if (blocks > cap) blocks = cap;
-      b200feat_whisper_normalize_tiled_kernel<<<(unsigned)blocks, 256, 0, stream>>>(h->plan, db, h->frames_per_tile);
-    } else {
-      int64_t blocks = (norm_rows + 7) / 8;
-      const int64_t cap = (int64_t)h->sm_count * 16;
-      if (blocks > cap) blocks = cap;
-      b200feat_whisper_normalize_kernel<<<(unsigned)blocks, 256, 0, stream>>>(h->plan, db, norm_rows);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("whisper normalise launch: ") + cudaGetErrorString(e));
-  }
-  return 0;
-}
 
 int b200feat_extract(b200feat_handle *h, const void *samples_dev, int32_t dt, const int64_t *meta_dev,
                      int32_t B, const b200feat_batch_totals *tot, float *out_dev, int32_t out_mode,
                      float pad_value, void *stream) {
   if (!h || !samples_dev || !meta_dev || !tot || !out_dev || B <= 0) return fail(h, B200FEAT_EINVAL, "extract: bad arguments");
   if (dt != B200FEAT_F32 && dt != B200FEAT_I16) return fail(h, B200FEAT_EINVAL, "bad sample dtype");
-  int prev = 0;
-  cudaGetDevice(&prev);
-  if (prev != h->device) cudaSetDevice(h->device);
+  DeviceGuard on(h->device);
   const int64_t all_rows = out_mode == B200FEAT_OUT_PADDED ? (int64_t)B * tot->max_frames : tot->total_rows;
   float *scratch = h->plan.whisper ? out_dev + all_rows * h->plan.F : nullptr;
   int rc = launch_range(h, samples_dev, dt, meta_dev, B, 0, B, 0, tot->total_tiles, tot->max_frames, out_dev,
                         out_mode, pad_value, (cudaStream_t)stream, scratch, all_rows);
-  if (prev != h->device) cudaSetDevice(prev);
   if (rc) return rc;
   {
     std::lock_guard<std::mutex> g(h->stats_mu);
@@ -624,6 +750,7 @@ int b200feat_extract(b200feat_handle *h, const void *samples_dev, int32_t dt, co
   }
   return B200FEAT_OK;
 }
+
 
 int b200feat_extract_host(b200feat_handle *h, const void *samples_host, int32_t dt,
                           const int64_t *num_samples, int32_t B, float *out_host, int32_t out_mode,
@@ -643,79 +770,7 @@ int b200feat_extract_host_at(b200feat_handle *h, const void *samples_host, int32
     }
   }
   if (dt != B200FEAT_F32 && dt != B200FEAT_I16) return fail(h, B200FEAT_EINVAL, "bad sample dtype");
-  HostRing &r = h->ring;
-  std::lock_guard<std::mutex> guard(r.mu);
-  int prev = 0;
-  cudaGetDevice(&prev);
-  cudaSetDevice(h->device);
-  struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
-
-  const size_t esz = dt == B200FEAT_I16 ? 2 : 4;
-  const int64_t words = b200feat_plan_words(h, num_samples, B, out_mode);
-  if (words < 0) return (int)words;
-  if (r.h_meta_cap < (size_t)words) {
-    if (r.h_meta) cudaFreeHost(r.h_meta);
-    r.h_meta = nullptr; r.h_meta_cap = 0;
-    CU_TRY(h, cudaMallocHost((void **)&r.h_meta, (size_t)words * 8));
-    r.h_meta_cap = (size_t)words;
-  }
-  b200feat_batch_totals tot;
-  // the host layout (back to back unless the caller supplied offsets) is kept on the device: chunks are copied verbatim
-  int rc = b200feat_plan_batch(h, num_samples, sample_offsets, B, 1, out_mode, r.h_meta, words, &tot);
-  if (rc) return rc;
-  for (auto &s : r.streams) if (!s) CU_TRY(h, cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-  if (!r.meta_ready) CU_TRY(h, cudaEventCreateWithFlags(&r.meta_ready, cudaEventDisableTiming));
-  auto grow = [&](void **p, size_t *cap, size_t need) -> cudaError_t {
-    if (*cap >= need) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    size_t want = need + need / 4;
-    cudaError_t e = cudaMalloc(p, want);
-    if (e == cudaSuccess) *cap = want;
-    return e;
-  };
-  CU_TRY(h, grow(&r.d_samples, &r.d_samples_cap, (size_t)tot.span_samples * esz + 16));
-  CU_TRY(h, grow((void **)&r.d_out, &r.d_out_cap, (size_t)tot.out_floats * 4 + 16));
-  {
-    size_t capb = r.d_meta_cap * 8;
-    CU_TRY(h, grow((void **)&r.d_meta, &capb, (size_t)words * 8));
-    r.d_meta_cap = capb / 8;
-  }
-  CU_TRY(h, cudaMemcpyAsync(r.d_meta, r.h_meta, (size_t)words * 8, cudaMemcpyHostToDevice, r.streams[0]));
-  CU_TRY(h, cudaEventRecord(r.meta_ready, r.streams[0]));
-
-  // chunk over cuts: ~32 MB of samples per chunk, round-robin over 3 streams so that
-  // H2D(i+1), kernel(i) and D2H(i-1) overlap (PCIe is the end-to-end bound, SURVEY.md §7)
-  const int64_t *soff = r.h_meta, *roff = r.h_meta + 2 * (int64_t)B, *toff = r.h_meta + 3 * (int64_t)B + 1;
-  const int64_t chunk_elems = (32ll << 20) / (int64_t)esz;
-  float *scratch = h->plan.whisper ? r.d_out + (tot.out_floats - B) : nullptr;
-  int b0 = 0, ci = 0, launches = 0;
-  while (b0 < B) {
-    int b1 = b0 + 1;
-    while (b1 < B && (soff[b1] + num_samples[b1]) - soff[b0] <= chunk_elems) ++b1;
-    cudaStream_t st = r.streams[ci % 3];
-    if (ci < 3) CU_TRY(h, cudaStreamWaitEvent(st, r.meta_ready, 0));
-    const int64_t e0 = soff[b0], e1 = soff[b1 - 1] + num_samples[b1 - 1];
-    CU_TRY(h, cudaMemcpyAsync((char *)r.d_samples + e0 * esz, (const char *)samples_host + e0 * esz,
-                              (size_t)(e1 - e0) * esz, cudaMemcpyHostToDevice, st));
-    int64_t f0, f1;
-    if (out_mode == B200FEAT_OUT_PADDED) { f0 = (int64_t)b0 * tot.max_frames; f1 = (int64_t)b1 * tot.max_frames; }
-    else { f0 = roff[b0]; f1 = roff[b1]; }
-    rc = launch_range(h, r.d_samples, dt, r.d_meta, B, b0, b1, toff[b0], toff[b1], tot.max_frames, r.d_out,
-                      out_mode, pad_value, st, scratch, f1 - f0);
-    if (rc) return rc;
-    launches += h->plan.whisper ? 2 : 1;
-    CU_TRY(h, cudaMemcpyAsync(out_host + f0 * h->plan.F, r.d_out + f0 * h->plan.F,
-                              (size_t)(f1 - f0) * h->plan.F * 4, cudaMemcpyDeviceToHost, st));
-    b0 = b1; ++ci;
-  }
-  for (auto &s : r.streams) CU_TRY(h, cudaStreamSynchronize(s));
-  {
-    std::lock_guard<std::mutex> g(h->stats_mu);
-    h->stats.calls++; h->stats.cuts += B; h->stats.frames += tot.total_rows;
-    h->stats.samples += tot.span_samples; h->stats.kernel_launches += launches;
-  }
-  return B200FEAT_OK;
+  return extract_staged(h, samples_host, nullptr, dt, num_samples, sample_offsets, B, out_host, out_mode, pad_value);
 }
 
 int b200feat_extract_host_ptrs(b200feat_handle *h, const void *const *cuts, int32_t dt, const int64_t *num_samples, int32_t B,
@@ -724,125 +779,13 @@ int b200feat_extract_host_ptrs(b200feat_handle *h, const void *const *cuts, int3
   if (dt != B200FEAT_F32 && dt != B200FEAT_I16) return fail(h, B200FEAT_EINVAL, "bad sample dtype");
   for (int i = 0; i < B; ++i)
     if (!cuts[i] && num_samples[i] > 0) return fail(h, B200FEAT_EINVAL, "extract_host_ptrs: null cut pointer");
-  HostRing &r = h->ring;
-  std::lock_guard<std::mutex> guard(r.mu);
-  int prev = 0;
-  cudaGetDevice(&prev);
-  cudaSetDevice(h->device);
-  struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
-
-  const size_t esz = dt == B200FEAT_I16 ? 2 : 4;
-  const int32_t align = dt == B200FEAT_I16 ? 8 : 4;  // every cut starts on a 16-byte boundary of the device buffer
-  const int64_t words = b200feat_plan_words(h, num_samples, B, out_mode);
-  if (words < 0) return (int)words;
-  if (r.h_meta_cap < (size_t)words) {
-    if (r.h_meta) cudaFreeHost(r.h_meta);
-    r.h_meta = nullptr; r.h_meta_cap = 0;
-    CU_TRY(h, cudaMallocHost((void **)&r.h_meta, (size_t)words * 8));
-    r.h_meta_cap = (size_t)words;
-  }
-  b200feat_batch_totals tot;
-  int rc = b200feat_plan_batch(h, num_samples, nullptr, B, align, out_mode, r.h_meta, words, &tot);
-  if (rc) return rc;
-  for (auto &s : r.streams) if (!s) CU_TRY(h, cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-  if (!r.meta_ready) CU_TRY(h, cudaEventCreateWithFlags(&r.meta_ready, cudaEventDisableTiming));
-  for (int k = 0; k < 2; ++k)
-    if (!r.stage_free[k]) CU_TRY(h, cudaEventCreateWithFlags(&r.stage_free[k], cudaEventDisableTiming));
-  if (!h->pool) {
-    int nthreads = 8;
-    if (const char *e = getenv("B200FEAT_STAGING_THREADS")) nthreads = std::max(1, atoi(e));
-    h->pool = new GatherPool(nthreads - 1);  // the calling thread works too
-  }
-  auto grow = [&](void **p, size_t *cap, size_t need, bool host) -> cudaError_t {
-    if (*cap >= need) return cudaSuccess;
-    if (*p) { if (host) cudaFreeHost(*p); else cudaFree(*p); }
-    *p = nullptr; *cap = 0;
-    const size_t want = need + need / 4;
-    cudaError_t e = host ? cudaMallocHost(p, want) : cudaMalloc(p, want);
-    if (e == cudaSuccess) *cap = want;
-    return e;
-  };
-  CU_TRY(h, grow(&r.d_samples, &r.d_samples_cap, (size_t)tot.span_samples * esz + 16, false));
-  CU_TRY(h, grow((void **)&r.d_out, &r.d_out_cap, (size_t)tot.out_floats * 4 + 16, false));
-  {
-    size_t capb = r.d_meta_cap * 8;
-    CU_TRY(h, grow((void **)&r.d_meta, &capb, (size_t)words * 8, false));
-    r.d_meta_cap = capb / 8;
-  }
-  CU_TRY(h, cudaMemcpyAsync(r.d_meta, r.h_meta, (size_t)words * 8, cudaMemcpyHostToDevice, r.streams[0]));
-  CU_TRY(h, cudaEventRecord(r.meta_ready, r.streams[0]));
-
-  const int64_t *soff = r.h_meta, *roff = r.h_meta + 2 * (int64_t)B, *toff = r.h_meta + 3 * (int64_t)B + 1;
-  const int64_t chunk_elems = (32ll << 20) / (int64_t)esz;
-  // chunk boundaries first: the staging slots must hold the largest chunk
-  std::vector<int> cb{0};
-  for (int b0 = 0; b0 < B;) {
-    int b1 = b0 + 1;
-    while (b1 < B && (soff[b1] + num_samples[b1]) - soff[b0] <= chunk_elems) ++b1;
-    cb.push_back(b1);
-    b0 = b1;
-  }
-  size_t max_bytes = 0;
-  for (size_t c = 0; c + 1 < cb.size(); ++c)
-    max_bytes = std::max(max_bytes, (size_t)((soff[cb[c + 1] - 1] + num_samples[cb[c + 1] - 1]) - soff[cb[c]]) * esz);
-  for (int k = 0; k < 2; ++k) CU_TRY(h, grow(&r.h_stage[k], &r.h_stage_cap[k], max_bytes + 64, true));
-
-  float *scratch = h->plan.whisper ? r.d_out + (tot.out_floats - B) : nullptr;
-  int launches = 0;
-  for (size_t c = 0; c + 1 < cb.size(); ++c) {
-    const int b0 = cb[c], b1 = cb[c + 1], slot = (int)(c & 1);
-    cudaStream_t st = r.streams[c % 3];
-    if (c < 3) CU_TRY(h, cudaStreamWaitEvent(st, r.meta_ready, 0));
-    if (c >= 2) CU_TRY(h, cudaEventSynchronize(r.stage_free[slot]));  // the H2D copy out of this slot (chunk c - 2) is done
-    unsigned char *stage = static_cast<unsigned char *>(r.h_stage[slot]);
-    const int64_t e0 = soff[b0], e1 = soff[b1 - 1] + num_samples[b1 - 1];
-    // gather: one task per ~1 MB piece so that long and short cuts balance over the threads
-    struct Piece { const unsigned char *src; unsigned char *dst; size_t bytes; };
-    std::vector<Piece> pieces;
-    for (int i = b0; i < b1; ++i) {
-      const unsigned char *src = static_cast<const unsigned char *>(cuts[i]);
-      unsigned char *dst = stage + (size_t)(soff[i] - e0) * esz;
-      size_t left = (size_t)num_samples[i] * esz;
-      while (left) {
-        const size_t take = std::min(left, (size_t)1 << 20);
-        pieces.push_back({src, dst, take});
-        src += take; dst += take; left -= take;
-      }
-      if (i + 1 < b1) {  // alignment gap before the next cut: defined bytes only
-        const size_t gap = (size_t)(soff[i + 1] - soff[i] - num_samples[i]) * esz;
-        if (gap) memset(stage + (size_t)(soff[i] + num_samples[i] - e0) * esz, 0, gap);
-      }
-    }
-    const std::function<void(int)> job = [&](int k) { stream_copy(pieces[k].dst, pieces[k].src, pieces[k].bytes); };
-    h->pool->parallel_for((int)pieces.size(), job);
-    CU_TRY(h, cudaMemcpyAsync((char *)r.d_samples + e0 * esz, stage, (size_t)(e1 - e0) * esz, cudaMemcpyHostToDevice, st));
-    CU_TRY(h, cudaEventRecord(r.stage_free[slot], st));
-    int64_t f0, f1;
-    if (out_mode == B200FEAT_OUT_PADDED) { f0 = (int64_t)b0 * tot.max_frames; f1 = (int64_t)b1 * tot.max_frames; }
-    else { f0 = roff[b0]; f1 = roff[b1]; }
-    rc = launch_range(h, r.d_samples, dt, r.d_meta, B, b0, b1, toff[b0], toff[b1], tot.max_frames, r.d_out, out_mode, pad_value, st,
-                      scratch, f1 - f0);
-    if (rc) return rc;
-    launches += h->plan.whisper ? 2 : 1;
-    CU_TRY(h, cudaMemcpyAsync(out_host + f0 * h->plan.F, r.d_out + f0 * h->plan.F, (size_t)(f1 - f0) * h->plan.F * 4,
-                              cudaMemcpyDeviceToHost, st));
-  }
-  for (auto &s : r.streams) CU_TRY(h, cudaStreamSynchronize(s));
-  {
-    std::lock_guard<std::mutex> g(h->stats_mu);
-    h->stats.calls++; h->stats.cuts += B; h->stats.frames += tot.total_rows;
-    h->stats.samples += tot.span_samples; h->stats.kernel_launches += launches;
-  }
-  return B200FEAT_OK;
+  return extract_staged(h, nullptr, cuts, dt, num_samples, nullptr, B, out_host, out_mode, pad_value);
 }
 
 int64_t b200feat_get_table(b200feat_handle *h, int32_t which, float *out, int64_t cap) {
   if (!h || !out) return B200FEAT_EINVAL;
   const DevPlan &p = h->plan;
-  int prev = 0;
-  cudaGetDevice(&prev);
-  cudaSetDevice(h->device);
-  struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
+  DeviceGuard on(h->device);
   auto pull = [&](const void *src, int64_t count) -> int64_t {
     if (count > cap) return fail(h, B200FEAT_EINVAL, "get_table: capacity too small");
     if (cudaMemcpy(out, src, (size_t)count * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
@@ -882,10 +825,7 @@ int b200feat_set_output_affine(b200feat_handle *h, const float *scale, const flo
     h->plan.post_scale = h->plan.post_shift = nullptr;
     return B200FEAT_OK;
   }
-  int prev = 0;
-  cudaGetDevice(&prev);
-  cudaSetDevice(h->device);
-  struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore{prev};
+  DeviceGuard on(h->device);
   const size_t bytes = (size_t)h->plan.F * sizeof(float);
   if (!h->d_affine) {
     CU_TRY(h, cudaMalloc((void **)&h->d_affine, 2 * bytes));

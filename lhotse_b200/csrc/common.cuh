@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
 #include <vector>
@@ -145,7 +147,106 @@ __device__ __forceinline__ float log_energy_value(const DevPlan &p, float e) {
   return le;
 }
 
-// ---- host-side helper shared by the N = 512 kernels --------------------------------------------------------------
+// ---- constant tables: one bulk asynchronous copy (TMA) global -> shared per CTA, completion signalled on an mbarrier
+__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
+
+// Thread 0 initialises the mbarrier at shared address `bar` and starts the copy of `bytes` bytes (a multiple of 16) from
+// `src` to `dst`; the copy completes phase 0 of the barrier.  Every thread of the CTA must call it (__syncthreads inside).
+__device__ __forceinline__ void blob_copy_start(unsigned bar, void *dst, const void *src, int bytes) {
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(bar) : "memory");
+  }
+}
+
+// spins until the calling thread observes the completion of phase `parity` of the mbarrier at `bar`
+__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
+  unsigned done = 0;
+  while (!done)
+    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+}
+
+// ---- host helpers shared by the kernels' prepare and launch code ---------------------------------------------------
+// Copies `count` elements to a new device allocation recorded in `allocs` (freed with the handle); *dst is nullptr when
+// count is 0.
+template <typename T>
+static inline cudaError_t upload_table(const T *src, size_t count, std::vector<void *> &allocs, const T **dst) {
+  *dst = nullptr;
+  if (count == 0) return cudaSuccess;
+  void *d = nullptr;
+  cudaError_t e = cudaMalloc(&d, count * sizeof(T));
+  if (e != cudaSuccess) return e;
+  allocs.push_back(d);
+  e = cudaMemcpy(d, src, count * sizeof(T), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) *dst = reinterpret_cast<const T *>(d);
+  return e;
+}
+template <typename T>
+static inline cudaError_t upload_table(const std::vector<T> &h, std::vector<void *> &allocs, const T **dst) {
+  return upload_table(h.data(), h.size(), allocs, dst);
+}
+
+// The constant tables a kernel fetches with blob_copy_start: sections back to back, each padded to 16 bytes.
+struct ConstBlob {
+  std::vector<unsigned char> bytes;
+  int append(const void *src, size_t n) {  // returns the section's byte offset
+    const size_t off = bytes.size();
+    bytes.resize(off + ((n + 15) & ~(size_t)15), 0);
+    if (n) memcpy(bytes.data() + off, src, n);
+    return (int)off;
+  }
+  template <typename T>
+  int append(const std::vector<T> &v) { return append(v.data(), v.size() * sizeof(T)); }
+  // cudaMalloc storage is 256-byte aligned, more than the bulk copy needs
+  cudaError_t upload(std::vector<void *> &allocs, const void **dst, int *nbytes) const {
+    const unsigned char *d = nullptr;
+    const cudaError_t e = upload_table(bytes, allocs, &d);
+    *dst = d;
+    *nbytes = (int)bytes.size();
+    return e;
+  }
+};
+
+// First and last FFT bin with a non-zero weight in column m of the (K x M) mel bank; false for an all-zero filter.
+static inline bool filter_support(const float *bank, int K, int M, int m, int *first, int *last) {
+  *first = *last = -1;
+  for (int k = 0; k < K; ++k)
+    if (bank[(size_t)k * M + m] != 0.f) { if (*first < 0) *first = k; *last = k; }
+  return *first >= 0;
+}
+
+// Grid of a persistent kernel: one CTA per work unit, at most `ctas_per_sm` on every SM.
+static inline unsigned persistent_grid(int64_t units, int sm_count, int ctas_per_sm) {
+  return (unsigned)std::min(units, (int64_t)sm_count * ctas_per_sm);
+}
+
+// At prepare time (launch == false) raises the kernel's dynamic shared-memory limit to `smem`; otherwise launches it.
+template <typename Tables>
+static int configure_or_launch(void (*kern)(DevPlan, Tables, DevBatch), int threads, bool launch, size_t smem,
+                               const DevPlan &p, const Tables &t, const DevBatch &b, dim3 grid, cudaStream_t stream) {
+  if (!launch)
+    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
+  kern<<<grid, dim3(threads), smem, stream>>>(p, t, b);
+  return 0;
+}
+
+// Launch-shape override of a kernel for A/B runs: the value of environment variable `name` if it is a shape index in
+// [0, count), else -1 (no override).
+static inline int launch_shape_override(const char *name, int count) {
+  const char *e = getenv(name);
+  if (!e) return -1;
+  const int v = atoi(e);
+  return v >= 0 && v < count ? v : -1;
+}
+
+// ---- mel bank packings shared by the fast kernels -------------------------------------------------------------------
 // The (K x M) mel bank re-packed for a `lanes`-wide epilogue (16 or 8): round j serves `lanes` consecutive filters, one per lane, with a common
 // trip count (the round's longest filter); weights beyond a filter's own support are zero, so a shorter filter simply
 // keeps accumulating zeros.  `scale` (an exact power of two) is folded into the weights.
@@ -174,12 +275,8 @@ static inline MelRounds pack_mel_rounds(const std::vector<float> &bank, int K, i
     for (int l = 0; l < lanes; ++l) {
       const int m = l + lanes * j;
       first[l] = 0; len[l] = 0;
-      if (m < M) {
-        int f0 = -1, f1 = -1;
-        for (int k = 0; k < K; ++k)
-          if (bank[(size_t)k * M + m] != 0.f) { if (f0 < 0) f0 = k; f1 = k; }
-        if (f0 >= 0) { first[l] = f0 / align * align; len[l] = f1 - first[l] + 1; }
-      }
+      int f0, f1;
+      if (m < M && filter_support(bank.data(), K, M, m, &f0, &f1)) { first[l] = f0 / align * align; len[l] = f1 - first[l] + 1; }
       mx = std::max(mx, len[l]);
       r.rstart[j * lanes + l] = first[l];
     }
@@ -205,6 +302,18 @@ static inline MelRounds pack_mel_rounds(const std::vector<float> &bank, int K, i
   if (r.wdense.empty()) r.wdense.assign(lanes, 0.f);
   r.rows = r.rounds ? (int)(r.wdense.size() / lanes) : 0;
   return r;
+}
+
+// Per (round, lane) descriptors of a 16-lane MelRounds with align 4: {first bin, trip count, float4 index of the lane's
+// first weights in wdense ([row / 4][lane][4]), 0}, one int4 each.
+static inline std::vector<int> mel_round_descs(const MelRounds &mr) {
+  std::vector<int> rdesc((size_t)std::max(mr.rounds, 1) * 16 * 4, 0);
+  for (int j = 0; j < mr.rounds; ++j)
+    for (int l = 0; l < 16; ++l) {
+      int *d = &rdesc[((size_t)j * 16 + l) * 4];
+      d[0] = mr.rstart[j * 16 + l]; d[1] = mr.rlen[j]; d[2] = mr.rrow[j] * 4 + l;
+    }
+  return rdesc;
 }
 
 // ---- the same bank cut into balanced work items (fast2048.cuh) -----------------------------------------------------
@@ -234,11 +343,9 @@ static inline MelItems pack_mel_items_T(const std::vector<float> &bank, int K, i
   std::vector<Item> items;
   r.qfirst.assign(M, 0); r.qcount.assign(M, 0);
   for (int m = 0; m < M; ++m) {
-    int f0 = -1, f1 = -1;
-    for (int k = 0; k < K; ++k)
-      if (bank[(size_t)k * M + m] != 0.f) { if (f0 < 0) f0 = k; f1 = k; }
+    int f0, f1;
     r.qfirst[m] = (int)items.size();
-    if (f0 < 0) continue;
+    if (!filter_support(bank.data(), K, M, m, &f0, &f1)) continue;
     const int s0 = f0 / align * align, end = f1 + 1;
     for (int a = s0; a < end; a += T) items.push_back({m, a, std::min(T, end - a)});
     r.qcount[m] = (int)items.size() - r.qfirst[m];
@@ -283,6 +390,17 @@ static inline MelItems pack_mel_items_T(const std::vector<float> &bank, int K, i
   if (r.wdense.empty()) r.wdense.assign(lanes * align, 0.f);
   r.rows = r.rounds ? (int)(r.wdense.size() / lanes) : 0;
   return r;
+}
+
+// Per filter table of a MelItems over M filters: M int2 {first item, items}, then per 32 filters int2 {max items, 0}
+static inline std::vector<int> mel_item_descs(const MelItems &mr, int M) {
+  std::vector<int> fdesc((size_t)(std::max(M, 1) + (M + 31) / 32 + 1) * 2, 0);
+  for (int m = 0; m < M; ++m) {
+    fdesc[2 * m] = mr.qfirst[m]; fdesc[2 * m + 1] = mr.qcount[m];
+    int &mx = fdesc[2 * (M + m / 32)];
+    mx = std::max(mx, mr.qcount[m]);
+  }
+  return fdesc;
 }
 
 static inline MelItems pack_mel_items(const std::vector<float> &bank, int K, int M, float scale, int lanes = 32, int align = 4) {

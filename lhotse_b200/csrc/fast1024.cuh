@@ -116,17 +116,8 @@ b200feat_fast1024_kernel(const DevPlan p, const Fast1024Tables ft, const DevBatc
   float2 *X = reinterpret_cast<float2 *>(xall + (size_t)w * ft.xfloats);  // per warp exchange tile (xfloats is a multiple of 4)
   float *P = pall + (size_t)w * (F1W_PBINS * SLOTS);             // per warp: [slot][F1W_PBINS]
 
-  const unsigned bar = f512_smem_u32(s_bar);
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) {  // constant tables: one TMA bulk copy
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(ft.cblob_bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(f512_smem_u32(s_const)), "l"(ft.cblob), "r"(ft.cblob_bytes), "r"(bar) : "memory");
-  }
+  const unsigned bar = smem_u32(s_bar);
+  blob_copy_start(bar, s_const, ft.cblob, ft.cblob_bytes);  // constant tables: one TMA bulk copy
   for (int i = tid; i < WARPS * (F1W_PBINS * SLOTS) + F1W_PTAIL; i += blockDim.x) pall[i] = 0.f;
   // per-lane twiddles kept in registers for the whole kernel
   float2 tw2[16];  // W512^(n3*(k1 + 16*k2)): [0..7] for n3 = 2h, [8..15] for n3 = 2h + 1
@@ -134,12 +125,7 @@ b200feat_fast1024_kernel(const DevPlan p, const Fast1024Tables ft, const DevBatc
   for (int i = 0; i < 16; ++i) tw2[i] = __ldg(ft.tw2 + lane * 16 + i);
   const float inv_L = 1.0f / (float)L;
   const int up_lane = (lane + 31) & 31;
-  {
-    unsigned done = 0;
-    while (!done)
-      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                   : "=r"(done) : "r"(bar), "r"(0u) : "memory");
-  }
+  mbar_wait(bar, 0);
   __syncthreads();
 
   for (int64_t tg = blockIdx.x; tg < b.num_tiles; tg += gridDim.x) {
@@ -373,7 +359,7 @@ struct Fast1024Host {
   int shape;
 };
 
-// launch shapes {warps per CTA, frames per warp, CTAs per SM}: B200FEAT_FAST1024W_SHAPE selects (A/B runs)
+// launch shapes {warps per CTA, frames per warp, CTAs per SM}: B200FEAT_FAST1024_VARIANT selects one (A/B runs)
 struct F1wShape { int warps, slots, minb; };
 #define F1W_NUM_SHAPES 4
 static const F1wShape kF1wShapes[F1W_NUM_SHAPES] = {{8, 3, 2}, {6, 4, 2}, {10, 2, 2}, {12, 3, 1}};
@@ -406,11 +392,7 @@ static inline bool fast1024_supported(const DevPlan &p) {
 
 template <int DT, int LCT, int WARPS, int SLOTS, int MINB>
 static int f1w_go(bool launch, size_t smem, const DevPlan &p, const Fast1024Tables &t, const DevBatch &b, dim3 grid, cudaStream_t stream) {
-  auto kern = b200feat_fast1024_kernel<DT, LCT, WARPS, SLOTS, MINB>;
-  if (!launch)
-    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
-  kern<<<grid, dim3(WARPS * 32), smem, stream>>>(p, t, b);
-  return 0;
+  return configure_or_launch(b200feat_fast1024_kernel<DT, LCT, WARPS, SLOTS, MINB>, WARPS * 32, launch, smem, p, t, b, grid, stream);
 }
 
 template <int DT, int LCT>
@@ -444,41 +426,22 @@ static inline int fast1024_prepare(DevPlan &p, const std::vector<float> &bank, s
       win2[n1 * 32 + l] = make_float2(j < p.L ? window[j] : 0.f, j + 1 < p.L ? window[j + 1] : 0.f);
     }
   f1w_fft_tables(tw1, tw2, w1k);
-  int rc;
-  if ((rc = f512_upload(tw2, allocs, &hst.t.tw2))) return rc;
+  if (upload_table(tw2, allocs, &hst.t.tw2)) return B200FEAT_ECUDA;
   MelItems mr = pack_mel_items_T(bank, p.K, p.M, p.use_mag ? 0.5f : 0.25f, 32, 4, F1W_PIECE, /*uniform=*/true);
   if (mr.max_reach > F1W_PBINS) return B200FEAT_EUNSUPPORTED;
   hst.t.mel_rounds = mr.rounds;
-  {
-    std::vector<unsigned char> blob;
-    auto append = [&](const void *src, size_t bytes) -> int {
-      const size_t off = blob.size();
-      blob.resize(off + ((bytes + 15) & ~(size_t)15), 0);
-      if (bytes) memcpy(blob.data() + off, src, bytes);
-      return (int)off;
-    };
-    append(win2.data(), win2.size() * sizeof(float2));
-    hst.t.off_tw1 = append(tw1.data(), tw1.size() * sizeof(float2));
-    hst.t.off_w1k = append(w1k.data(), w1k.size() * sizeof(float2));
-    hst.t.off_rstart = append(mr.rstart.data(), mr.rstart.size() * sizeof(int));
-    std::vector<int> fdesc((size_t)(std::max(p.M, 1) + (p.M + 31) / 32 + 1) * 2, 0);  // M x {first item, items}, then per 32 filters {max items, 0}
-    for (int m = 0; m < p.M; ++m) {
-      fdesc[2 * m] = mr.qfirst[m]; fdesc[2 * m + 1] = mr.qcount[m];
-      int &mx = fdesc[2 * (p.M + m / 32)];
-      mx = std::max(mx, mr.qcount[m]);
-    }
-    hst.t.off_fdesc = append(fdesc.data(), fdesc.size() * sizeof(int));
-    hst.t.off_mw = append(mr.wdense.data(), mr.wdense.size() * sizeof(float));
-    const unsigned char *d = nullptr;
-    if ((rc = f512_upload(blob, allocs, &d))) return rc;
-    hst.t.cblob = d;
-    hst.t.cblob_bytes = (int)blob.size();
-  }
-  int forced = -1;
-  if (const char *e = getenv("B200FEAT_FAST1024_VARIANT")) forced = atoi(e);
+  ConstBlob blob;
+  blob.append(win2);
+  hst.t.off_tw1 = blob.append(tw1);
+  hst.t.off_w1k = blob.append(w1k);
+  hst.t.off_rstart = blob.append(mr.rstart);
+  hst.t.off_fdesc = blob.append(mel_item_descs(mr, p.M));
+  hst.t.off_mw = blob.append(mr.wdense);
+  if (blob.upload(allocs, &hst.t.cblob, &hst.t.cblob_bytes)) return B200FEAT_ECUDA;
+  const int forced = launch_shape_override("B200FEAT_FAST1024_VARIANT", F1W_NUM_SHAPES);
   hst.shape = -1;
   for (int v = 0; v < F1W_NUM_SHAPES; ++v) {
-    if (forced >= 0 && forced < F1W_NUM_SHAPES && v != forced) continue;
+    if (forced >= 0 && v != forced) continue;
     const F1wShape sh = kF1wShapes[v];
     hst.t.xfloats = std::max(F1W_XBUF * 2, sh.slots * (mr.rounds * 32 + ((p.M + 3) & ~3)));
     if (fast1024_smem_bytes(hst.t, sh.warps, sh.slots) <= (size_t)(227 * 1024 / sh.minb) - 1024) { hst.shape = v; break; }
@@ -495,10 +458,7 @@ static inline int fast1024_prepare(DevPlan &p, const std::vector<float> &bank, s
 }
 
 static inline int fast1024_launch(const DevPlan &p, const Fast1024Host &hst, const DevBatch &b, int dt, int sm_count, cudaStream_t stream) {
-  const F1wShape shape = kF1wShapes[hst.shape];
-  int64_t blocks = b.num_tiles;
-  const int64_t cap = (int64_t)sm_count * shape.minb;
-  if (blocks > cap) blocks = cap;
-  f1w_dispatch(dt, f1w_ct_length(p.L), hst.shape, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
+  const dim3 grid(persistent_grid(b.num_tiles, sm_count, kF1wShapes[hst.shape].minb));
+  f1w_dispatch(dt, f1w_ct_length(p.L), hst.shape, true, hst.smem, p, hst.t, b, grid, stream);
   return (int)cudaGetLastError();
 }

@@ -189,26 +189,12 @@ b200feat_fast2048_kernel(const DevPlan p, const Fast2048Tables ft, const DevBatc
   float2 *X = xall + (size_t)w * F2K_XBUF;                       // per warp exchange tile
   float *P = pall + (size_t)w * (F2K_PBINS * SLOTS);             // per warp: [slot][F2K_PBINS]
 
-  const unsigned bar = f512_smem_u32(s_bar);
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) {  // constant tables: one TMA bulk copy
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(ft.cblob_bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(f512_smem_u32(s_const)), "l"(ft.cblob), "r"(ft.cblob_bytes), "r"(bar) : "memory");
-  }
+  const unsigned bar = smem_u32(s_bar);
+  blob_copy_start(bar, s_const, ft.cblob, ft.cblob_bytes);  // constant tables: one TMA bulk copy
   for (int i = tid; i < WARPS * (F2K_PBINS * SLOTS) + F2K_PTAIL; i += blockDim.x) pall[i] = 0.f;
   const float inv_L = 1.0f / (float)L;
   const int up_lane = (lane + 31) & 31;
-  {
-    unsigned done = 0;
-    while (!done)
-      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                   : "=r"(done) : "r"(bar), "r"(0u) : "memory");
-  }
+  mbar_wait(bar, 0);
   __syncthreads();
 
   for (int64_t tg = blockIdx.x; tg < b.num_tiles; tg += gridDim.x) {
@@ -490,11 +476,7 @@ static inline bool fast2048_supported(const DevPlan &p) {
 
 template <int DT, int LCT, int WARPS, int SLOTS>
 static int f2k_go(bool launch, size_t smem, const DevPlan &p, const Fast2048Tables &t, const DevBatch &b, dim3 grid, cudaStream_t stream) {
-  auto kern = b200feat_fast2048_kernel<DT, LCT, WARPS, SLOTS>;
-  if (!launch)
-    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
-  kern<<<grid, dim3(WARPS * 32), smem, stream>>>(p, t, b);
-  return 0;
+  return configure_or_launch(b200feat_fast2048_kernel<DT, LCT, WARPS, SLOTS>, WARPS * 32, launch, smem, p, t, b, grid, stream);
 }
 
 template <int DT, int LCT>
@@ -560,38 +542,19 @@ static inline int fast2048_prepare(DevPlan &p, const std::vector<float> &bank, s
   if (mr.max_reach > F2K_PBINS || 3 * (mr.rounds * 32 + ((p.M + 3) & ~3)) > F2K_XBUF * 2) return B200FEAT_EUNSUPPORTED;
   hst.t.mel_rounds = mr.rounds;
   hst.t.mel_qmax = qmax;
-  int rc;
-  {
-    std::vector<unsigned char> blob;
-    auto append = [&](const void *src, size_t bytes) -> int {
-      const size_t off = blob.size();
-      blob.resize(off + ((bytes + 15) & ~(size_t)15), 0);
-      if (bytes) memcpy(blob.data() + off, src, bytes);
-      return (int)off;
-    };
-    append(win2.data(), win2.size() * sizeof(float2));
-    hst.t.off_tw1 = append(tw1.data(), tw1.size() * sizeof(float2));
-    hst.t.off_tw2 = append(tw2.data(), tw2.size() * sizeof(float2));
-    hst.t.off_w2k = append(w2k.data(), w2k.size() * sizeof(float2));
-    hst.t.off_rstart = append(mr.rstart.data(), mr.rstart.size() * sizeof(int));
-    std::vector<int> fdesc((size_t)(std::max(p.M, 1) + (p.M + 31) / 32 + 1) * 2, 0);  // M x {first item, items}, then per 32 filters {max items, 0}
-    for (int m = 0; m < p.M; ++m) {
-      fdesc[2 * m] = mr.qfirst[m]; fdesc[2 * m + 1] = mr.qcount[m];
-      int &mx = fdesc[2 * (p.M + m / 32)];
-      mx = std::max(mx, mr.qcount[m]);
-    }
-    hst.t.off_fdesc = append(fdesc.data(), fdesc.size() * sizeof(int));
-    hst.t.off_mw = append(mr.wdense.data(), mr.wdense.size() * sizeof(float));
-    const unsigned char *d = nullptr;
-    if ((rc = f512_upload(blob, allocs, &d))) return rc;
-    hst.t.cblob = d;
-    hst.t.cblob_bytes = (int)blob.size();
-  }
-  int forced = -1;
-  if (const char *e = getenv("B200FEAT_FAST2048_VARIANT")) forced = atoi(e);
+  ConstBlob blob;
+  blob.append(win2);
+  hst.t.off_tw1 = blob.append(tw1);
+  hst.t.off_tw2 = blob.append(tw2);
+  hst.t.off_w2k = blob.append(w2k);
+  hst.t.off_rstart = blob.append(mr.rstart);
+  hst.t.off_fdesc = blob.append(mel_item_descs(mr, p.M));
+  hst.t.off_mw = blob.append(mr.wdense);
+  if (blob.upload(allocs, &hst.t.cblob, &hst.t.cblob_bytes)) return B200FEAT_ECUDA;
+  const int forced = launch_shape_override("B200FEAT_FAST2048_VARIANT", F2K_NUM_VARIANTS);
   hst.variant = -1;
   for (int v = 0; v < F2K_NUM_VARIANTS; ++v) {
-    if (forced >= 0 && forced < F2K_NUM_VARIANTS && v != forced) continue;
+    if (forced >= 0 && v != forced) continue;
     if (fast2048_smem_bytes(hst.t, kF2kVariants[v].warps, kF2kVariants[v].slots) <= (size_t)226 * 1024) { hst.variant = v; break; }
   }
   if (hst.variant < 0) return B200FEAT_EUNSUPPORTED;
@@ -606,8 +569,7 @@ static inline int fast2048_prepare(DevPlan &p, const std::vector<float> &bank, s
 }
 
 static inline int fast2048_launch(const DevPlan &p, const Fast2048Host &hst, const DevBatch &b, int dt, int sm_count, cudaStream_t stream) {
-  int64_t blocks = b.num_tiles;
-  if (blocks > sm_count) blocks = sm_count;
-  f2k_dispatch(dt, f2k_ct_length(p.L), hst.variant, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
+  const dim3 grid(persistent_grid(b.num_tiles, sm_count, 1));
+  f2k_dispatch(dt, f2k_ct_length(p.L), hst.variant, true, hst.smem, p, hst.t, b, grid, stream);
   return (int)cudaGetLastError();
 }

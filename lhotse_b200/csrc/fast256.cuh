@@ -83,17 +83,8 @@ b200feat_fast256_kernel(const DevPlan p, const Fast256Tables ft, const DevBatch 
   float2 *X = xall + (size_t)qw * F256_XBUF;
   float *P = pall + (size_t)qw * F256_PBUF;  // [slot][F256_PBINS]
 
-  const unsigned bar = f512_smem_u32(s_bar);
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) {  // constant tables: one TMA bulk copy
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(ft.cblob_bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(f512_smem_u32(s_const)), "l"(ft.cblob), "r"(ft.cblob_bytes), "r"(bar) : "memory");
-  }
+  const unsigned bar = smem_u32(s_bar);
+  blob_copy_start(bar, s_const, ft.cblob, ft.cblob_bytes);  // constant tables: one TMA bulk copy
   for (int i = tid; i < F256_QW * F256_PBUF + F256_PTAIL; i += blockDim.x) pall[i] = 0.f;  // never NaN under zero weights
 
   float2 tw1[16];
@@ -102,12 +93,7 @@ b200feat_fast256_kernel(const DevPlan p, const Fast256Tables ft, const DevBatch 
   const float2 w256l = __ldg(ft.w256 + l);
   const int partner = (8 - l) & 7;
   const float inv_L = 1.0f / (float)L;
-  {
-    unsigned done = 0;
-    while (!done)
-      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                   : "=r"(done) : "r"(bar), "r"(0u) : "memory");
-  }
+  mbar_wait(bar, 0);
   __syncthreads();
 
   for (int64_t tg = blockIdx.x; tg < b.num_tiles; tg += gridDim.x) {
@@ -375,11 +361,7 @@ static inline bool fast256_supported(const DevPlan &p) {
 
 template <int DT, int LCT>
 static int f256_go(bool launch, size_t smem, const DevPlan &p, const Fast256Tables &t, const DevBatch &b, dim3 grid, cudaStream_t stream) {
-  auto kern = b200feat_fast256_kernel<DT, LCT>;
-  if (!launch)
-    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
-  kern<<<grid, dim3(F256_WARPS * 32), smem, stream>>>(p, t, b);
-  return 0;
+  return configure_or_launch(b200feat_fast256_kernel<DT, LCT>, F256_WARPS * 32, launch, smem, p, t, b, grid, stream);
 }
 
 static int f256_dispatch(int dt, int L, bool launch, size_t smem, const DevPlan &p, const Fast256Tables &t, const DevBatch &b,
@@ -408,31 +390,18 @@ static inline int fast256_prepare(DevPlan &p, const std::vector<float> &bank, st
     const double a = -2.0 * M_PI * (double)l / 256.0;
     w256[l] = make_float2((float)cos(a), (float)sin(a));
   }
-  int rc;
-  if ((rc = f512_upload(tw1, allocs, &hst.t.tw1))) return rc;
-  if ((rc = f512_upload(w256, allocs, &hst.t.w256))) return rc;
+  if (upload_table(tw1, allocs, &hst.t.tw1) || upload_table(w256, allocs, &hst.t.w256)) return B200FEAT_ECUDA;
   const MelRounds mr = pack_mel_rounds(bank, p.K, p.M, p.use_mag ? 0.5f : 0.25f, 8, 2, F256_PBINS);  // 64-bit mel loads
   if (mr.max_reach > F256_PBINS) return B200FEAT_EUNSUPPORTED;
   hst.t.mel_rounds = mr.rounds;
   hst.t.mel_wrows = mr.rows;
-  {
-    std::vector<unsigned char> blob;
-    auto append = [&](const void *src, size_t bytes) -> int {
-      const size_t off = blob.size();
-      blob.resize(off + ((bytes + 15) & ~(size_t)15), 0);
-      memcpy(blob.data() + off, src, bytes);
-      return (int)off;
-    };
-    append(win2.data(), win2.size() * sizeof(float2));
-    hst.t.off_rstart = append(mr.rstart.data(), mr.rstart.size() * sizeof(int));
-    hst.t.off_rlen = append(mr.rlen.data(), mr.rlen.size() * sizeof(int));
-    hst.t.off_rrow = append(mr.rrow.data(), mr.rrow.size() * sizeof(int));
-    hst.t.off_mw = append(mr.wdense.data(), mr.wdense.size() * sizeof(float));
-    const unsigned char *d = nullptr;
-    if ((rc = f512_upload(blob, allocs, &d))) return rc;
-    hst.t.cblob = d;
-    hst.t.cblob_bytes = (int)blob.size();
-  }
+  ConstBlob blob;
+  blob.append(win2);
+  hst.t.off_rstart = blob.append(mr.rstart);
+  hst.t.off_rlen = blob.append(mr.rlen);
+  hst.t.off_rrow = blob.append(mr.rrow);
+  hst.t.off_mw = blob.append(mr.wdense);
+  if (blob.upload(allocs, &hst.t.cblob, &hst.t.cblob_bytes)) return B200FEAT_ECUDA;
   hst.smem = fast256_smem_bytes(hst.t);
   if (hst.smem > 113 * 1024) return B200FEAT_EUNSUPPORTED;  // keep 2 CTAs per SM
   DevBatch none{};
@@ -445,9 +414,6 @@ static inline int fast256_prepare(DevPlan &p, const std::vector<float> &bank, st
 }
 
 static inline int fast256_launch(const DevPlan &p, const Fast256Host &hst, const DevBatch &b, int dt, int sm_count, cudaStream_t stream) {
-  int64_t blocks = b.num_tiles;
-  const int64_t cap = (int64_t)sm_count * 2;
-  if (blocks > cap) blocks = cap;
-  f256_dispatch(dt, p.L == 200 ? 200 : 0, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
+  f256_dispatch(dt, p.L == 200 ? 200 : 0, true, hst.smem, p, hst.t, b, dim3(persistent_grid(b.num_tiles, sm_count, 2)), stream);
   return (int)cudaGetLastError();
 }

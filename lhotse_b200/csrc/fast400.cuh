@@ -121,25 +121,11 @@ b200feat_fast400_kernel(const DevPlan p, const Fast400Tables ft, const DevBatch 
   float *S = reinterpret_cast<float *>(X);   // the same tile first holds the frame's raw samples
   float *P = pall + (size_t)qw * F400_PBUF;  // [slot][F400_PBINS]
 
-  const unsigned bar = f512_smem_u32(s_bar);
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) {  // constant tables: one TMA bulk copy
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(ft.cblob_bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(f512_smem_u32(s_const)), "l"(ft.cblob), "r"(ft.cblob_bytes), "r"(bar) : "memory");
-  }
+  const unsigned bar = smem_u32(s_bar);
+  blob_copy_start(bar, s_const, ft.cblob, ft.cblob_bytes);  // constant tables: one TMA bulk copy
   for (int i = tid; i < QW * F400_PBUF + F400_PTAIL; i += blockDim.x) pall[i] = 0.f;  // never NaN under zero weights
   const float inv_L = 1.0f / (float)L;
-  {
-    unsigned done = 0;
-    while (!done)
-      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                   : "=r"(done) : "r"(bar), "r"(0u) : "memory");
-  }
+  mbar_wait(bar, 0);
   __syncthreads();
 
   for (int64_t tg = blockIdx.x; tg < b.num_tiles; tg += gridDim.x) {
@@ -399,11 +385,7 @@ static inline bool fast400_supported(const DevPlan &p) {
 
 template <int DT>
 static int f400_go(bool launch, size_t smem, const DevPlan &p, const Fast400Tables &t, const DevBatch &b, dim3 grid, cudaStream_t stream) {
-  auto kern = b200feat_fast400_kernel<DT, F400_WARPS>;
-  if (!launch)
-    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
-  kern<<<grid, dim3(F400_WARPS * 32), smem, stream>>>(p, t, b);
-  return 0;
+  return configure_or_launch(b200feat_fast400_kernel<DT, F400_WARPS>, F400_WARPS * 32, launch, smem, p, t, b, grid, stream);
 }
 
 static inline int fast400_prepare(DevPlan &p, const std::vector<float> &bank, std::vector<void *> &allocs,
@@ -424,30 +406,12 @@ static inline int fast400_prepare(DevPlan &p, const std::vector<float> &bank, st
   const MelRounds mr = pack_mel_rounds(bank, p.K, p.M, p.use_mag ? 0.5f : 0.25f, 16, 4, F400_PBINS / 4 * 4);  // 16 filters per round, two per lane
   if (mr.max_reach > F400_PBINS) return B200FEAT_EUNSUPPORTED;
   hst.t.mel_rounds = mr.rounds;
-  int rc;
-  {
-    std::vector<unsigned char> blob;
-    auto append = [&](const void *src, size_t bytes) -> int {
-      const size_t off = blob.size();
-      blob.resize(off + ((bytes + 15) & ~(size_t)15), 0);
-      if (bytes) memcpy(blob.data() + off, src, bytes);
-      return (int)off;
-    };
-    append(win2.data(), win2.size() * sizeof(float2));
-    hst.t.off_tws = append(tws.data(), tws.size() * sizeof(float2));
-    std::vector<int> rdesc((size_t)std::max(mr.rounds, 1) * 16 * 4, 0);
-    for (int j = 0; j < mr.rounds; ++j)
-      for (int l = 0; l < 16; ++l) {
-        int *d = &rdesc[((size_t)j * 16 + l) * 4];
-        d[0] = mr.rstart[j * 16 + l]; d[1] = mr.rlen[j]; d[2] = mr.rrow[j] * 4 + l;  // float4 index: (row / 4) * 16 + column
-      }
-    hst.t.off_rdesc = append(rdesc.data(), rdesc.size() * sizeof(int));
-    hst.t.off_mw = append(mr.wdense.data(), mr.wdense.size() * sizeof(float));
-    const unsigned char *d = nullptr;
-    if ((rc = f512_upload(blob, allocs, &d))) return rc;
-    hst.t.cblob = d;
-    hst.t.cblob_bytes = (int)blob.size();
-  }
+  ConstBlob blob;
+  blob.append(win2);
+  hst.t.off_tws = blob.append(tws);
+  hst.t.off_rdesc = blob.append(mel_round_descs(mr));
+  hst.t.off_mw = blob.append(mr.wdense);
+  if (blob.upload(allocs, &hst.t.cblob, &hst.t.cblob_bytes)) return B200FEAT_ECUDA;
   hst.smem = fast400_smem_bytes(hst.t, F400_WARPS);
   if (hst.smem > 113 * 1024) return B200FEAT_EUNSUPPORTED;  // keep 2 CTAs per SM
   DevBatch none{};
@@ -459,10 +423,8 @@ static inline int fast400_prepare(DevPlan &p, const std::vector<float> &bank, st
 }
 
 static inline int fast400_launch(const DevPlan &p, const Fast400Host &hst, const DevBatch &b, int dt, int sm_count, cudaStream_t stream) {
-  int64_t blocks = b.num_tiles;
-  const int64_t cap = (int64_t)sm_count * 2;
-  if (blocks > cap) blocks = cap;
-  if (dt == B200FEAT_I16) f400_go<B200FEAT_I16>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
-  else f400_go<B200FEAT_F32>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
+  const dim3 grid(persistent_grid(b.num_tiles, sm_count, 2));
+  if (dt == B200FEAT_I16) f400_go<B200FEAT_I16>(true, hst.smem, p, hst.t, b, grid, stream);
+  else f400_go<B200FEAT_F32>(true, hst.smem, p, hst.t, b, grid, stream);
   return (int)cudaGetLastError();
 }

@@ -54,8 +54,6 @@ struct Fast512Tables {  // derived once per handle
   int mel_wrows;        // sum of the rounds' trip counts
 };
 
-__device__ __forceinline__ unsigned f512_smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-
 // (F512_HD: the pure arithmetic helpers also compile for the host, where scripts/micro/f2k_host_check.cu runs the FFT
 // stages of fast2048.cuh lane by lane against a float64 DFT)
 #define F512_HD __host__ __device__ __forceinline__
@@ -241,17 +239,8 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
   float *P = pall + (size_t)hw * PBUF;                        // [slot][PBINS]
 
   // ---- constant tables: one TMA bulk copy global -> shared, completion signalled on an mbarrier
-  const unsigned bar = f512_smem_u32(s_bar);
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(ft.cblob_bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(f512_smem_u32(s_const)), "l"(ft.cblob), "r"(ft.cblob_bytes), "r"(bar) : "memory");
-  }
+  const unsigned bar = smem_u32(s_bar);
+  blob_copy_start(bar, s_const, ft.cblob, ft.cblob_bytes);
   // P is read past a filter's support with zero weights: it must never hold NaN patterns
   for (int i = tid; i < HW * PBUF + F512_PTAIL; i += blockDim.x) pall[i] = 0.f;
 
@@ -266,12 +255,7 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
   for (int i = 0; i < 8; ++i) wsplit[i] = __ldg(ft.w512 + i * 16 + l);
   const int partner = (16 - l) & 15;
   const float inv_L = 1.0f / (float)L;
-  {  // every thread observes the completion of the bulk copy (phase 0 of the mbarrier) before touching the tables
-    unsigned done = 0;
-    while (!done)
-      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                   : "=r"(done) : "r"(bar), "r"(0u) : "memory");
-  }
+  mbar_wait(bar, 0);  // every thread observes the completion of the bulk copy before touching the tables
   __syncthreads();
 
   for (int64_t tg = blockIdx.x; tg < b.num_tiles; tg += gridDim.x) {
@@ -574,16 +558,11 @@ b200feat_fast512_kernel(const DevPlan p, const Fast512Tables ft, const DevBatch 
 // ---------------------------------------------------------------------------------------------- host
 // Launch shapes on the headline workload (kernel ms per launch of 2048 x 10 s cuts, scripts/variant_bench.py, H100 SXM with a
 // 400 W power limit, profiles/h100_launch_shapes.jsonl):
-//   {8 warps, 4 slots, twiddles in registers, 2 CTAs/SM}  1.796 / 1.767   <- variant 0, what ships
-//   {10, 2, shared, 2}  (20 warps/SM, 96 registers)       1.859
-// Only variants 0 and 2 stay instantiated; B200FEAT_FAST_VARIANT=2 selects the high-occupancy shape for A/B runs.
+//   {8 warps, 4 slots, twiddles in registers, 2 CTAs/SM}  1.796 / 1.767   <- shape 0, what ships
+//   {10, 2, shared, 2}  (20 warps/SM, 96 registers)       1.859           <- shape 2
+// B200FEAT_FAST_VARIANT=2 selects the high-occupancy shape for A/B runs; 0 and 1 select shape 0.
 struct Fast512Variant { int warps, slots, tws, minb; };
-static const Fast512Variant kFast512Variants[] = {
-    {8, 4, 0, 2},   // 0
-    {8, 4, 0, 2},   // 1 (alias of 0)
-    {10, 2, 1, 2},  // 2
-};
-#define F512_NUM_VARIANTS 3
+static inline Fast512Variant f512_variant(int v) { return v == 2 ? Fast512Variant{10, 2, 1, 2} : Fast512Variant{8, 4, 0, 2}; }
 #ifndef F512_DEFAULT_VARIANT
 #define F512_DEFAULT_VARIANT 0
 #endif
@@ -591,22 +570,12 @@ static const Fast512Variant kFast512Variants[] = {
 struct Fast512Host {
   Fast512Tables t;
   size_t smem;
-  int variant;
+  int variant;  // 0 or 2
 };
 
 static inline bool fast512_supported(const DevPlan &p) {
   return p.N == 512 && p.packed && p.L >= 2 && p.L <= 512 && p.C <= 128 &&
          4 * ((p.M + 3) & ~3) <= 2 * F512_XBUF;  // log-mel staging reuses the transpose tile
-}
-
-template <typename T>
-static int f512_upload(const std::vector<T> &h, std::vector<void *> &allocs, const T **out) {
-  void *d = nullptr;
-  if (cudaMalloc(&d, h.size() * sizeof(T)) != cudaSuccess) return B200FEAT_ECUDA;
-  allocs.push_back(d);
-  if (cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return B200FEAT_ECUDA;
-  *out = reinterpret_cast<const T *>(d);
-  return 0;
 }
 
 // one instantiation per (dtype, compile-time L, variant, plain log-mel or not); `launch` == false only raises the
@@ -618,11 +587,7 @@ static int f512_go(bool launch, size_t smem, const DevPlan &p, const Fast512Tabl
   constexpr int S = V == 2 ? 2 : 4;
   constexpr int TW = V == 2 ? 1 : 0;
   constexpr int MB = 2;
-  auto kern = b200feat_fast512_kernel<DT, LCT, W, S, TW, MB, PLAIN>;
-  if (!launch)
-    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess ? 0 : B200FEAT_ECUDA;
-  kern<<<grid, dim3(W * 32), smem, stream>>>(p, t, b);
-  return 0;
+  return configure_or_launch(b200feat_fast512_kernel<DT, LCT, W, S, TW, MB, PLAIN>, W * 32, launch, smem, p, t, b, grid, stream);
 }
 
 template <int DT, int LCT, bool PLAIN>
@@ -653,12 +618,9 @@ static inline bool fast512_plain(const DevPlan &p, const DevBatch &b) {
 static inline int fast512_prepare(DevPlan &p, const std::vector<float> &bank, std::vector<void *> &allocs,
                                   int *frames_per_tile, const std::vector<float> &window, Fast512Host *out) {
   Fast512Host hst;
-  hst.variant = F512_DEFAULT_VARIANT;
-  if (const char *e = getenv("B200FEAT_FAST_VARIANT")) {
-    const int v = atoi(e);
-    if (v >= 0 && v < F512_NUM_VARIANTS) hst.variant = v;
-  }
-  const Fast512Variant var = kFast512Variants[hst.variant];
+  const int forced = launch_shape_override("B200FEAT_FAST_VARIANT", 3);
+  hst.variant = (forced >= 0 ? forced : F512_DEFAULT_VARIANT) == 2 ? 2 : 0;
+  const Fast512Variant var = f512_variant(hst.variant);
   std::vector<float2> win2(256), tw1(256), w512(128);
   for (int n1 = 0; n1 < 16; ++n1)
     for (int l = 0; l < 16; ++l) {
@@ -675,41 +637,19 @@ static inline int fast512_prepare(DevPlan &p, const std::vector<float> &bank, st
       const double a = -2.0 * M_PI * (double)(l + 16 * i) / 512.0;
       w512[i * 16 + l] = make_float2((float)cos(a), (float)sin(a));
     }
-  int rc;
-  if ((rc = f512_upload(tw1, allocs, &hst.t.tw1))) return rc;
-  if ((rc = f512_upload(w512, allocs, &hst.t.w512))) return rc;
+  if (upload_table(tw1, allocs, &hst.t.tw1) || upload_table(w512, allocs, &hst.t.w512)) return B200FEAT_ECUDA;
   // mel bank re-packed for the epilogue (pack_mel_rounds, common.cuh); the kernel stores |2X|^2 (or |2X|), so the
   // exact power-of-two factor 1/4 (1/2) rides on the weights
   const MelRounds mr = pack_mel_rounds(bank, p.K, p.M, p.use_mag ? 0.5f : 0.25f, 16, 4, 260);  // 4-aligned filter starts: 128-bit mel loads
   if (mr.max_reach > 260) return B200FEAT_EUNSUPPORTED;  // zero-weight over-reads must stay inside the frame's own P row
-  const int rounds = mr.rounds;
-  const std::vector<int> &rstart = mr.rstart, &rlen = mr.rlen, &rrow = mr.rrow;
-  const std::vector<float> &wdense = mr.wdense;
-  hst.t.mel_rounds = rounds;
-  hst.t.mel_wrows = rounds ? (int)(wdense.size() / 16) : 0;
-  {  // one 16-byte-aligned blob for the TMA bulk copy
-    std::vector<unsigned char> blob;
-    auto append = [&](const void *src, size_t bytes) -> int {
-      const size_t off = blob.size();
-      blob.resize(off + ((bytes + 15) & ~(size_t)15), 0);
-      memcpy(blob.data() + off, src, bytes);
-      return (int)off;
-    };
-    append(win2.data(), win2.size() * sizeof(float2));
-    hst.t.off_tw1 = var.tws ? append(tw1.data(), tw1.size() * sizeof(float2)) : 0;
-    std::vector<int> rdesc((size_t)std::max(rounds, 1) * 16 * 4, 0);  // per (round, lane): {first bin, trips, weight idx, 0}
-    for (int j = 0; j < rounds; ++j)
-      for (int l = 0; l < 16; ++l) {
-        int *d = &rdesc[((size_t)j * 16 + l) * 4];
-        d[0] = rstart[j * 16 + l]; d[1] = rlen[j]; d[2] = rrow[j] * 4 + l;  // float4 index of the lane's first weights
-      }
-    hst.t.off_rdesc = append(rdesc.data(), rdesc.size() * sizeof(int));
-    hst.t.off_mw = append(wdense.data(), wdense.size() * sizeof(float));
-    const unsigned char *d = nullptr;
-    if ((rc = f512_upload(blob, allocs, &d))) return rc;  // cudaMalloc returns >= 256-byte aligned storage
-    hst.t.cblob = d;
-    hst.t.cblob_bytes = (int)blob.size();
-  }
+  hst.t.mel_rounds = mr.rounds;
+  hst.t.mel_wrows = mr.rounds ? (int)(mr.wdense.size() / 16) : 0;
+  ConstBlob blob;
+  blob.append(win2);
+  hst.t.off_tw1 = var.tws ? blob.append(tw1) : 0;
+  hst.t.off_rdesc = blob.append(mel_round_descs(mr));
+  hst.t.off_mw = blob.append(mr.wdense);
+  if (blob.upload(allocs, &hst.t.cblob, &hst.t.cblob_bytes)) return B200FEAT_ECUDA;
   hst.smem = fast512_smem_bytes(p, hst.t, var.warps, var.slots, var.tws);
   if (hst.smem > (size_t)(227 * 1024 / var.minb) - 1024) return B200FEAT_EUNSUPPORTED;  // keep MINB CTAs per SM
   DevBatch none{};
@@ -725,12 +665,9 @@ static inline int fast512_prepare(DevPlan &p, const std::vector<float> &bank, st
 
 static inline int fast512_launch(const DevPlan &p, const Fast512Host &hst, const DevBatch &b, int dt, int sm_count,
                                  cudaStream_t stream) {
-  const Fast512Variant var = kFast512Variants[hst.variant];
-  int64_t blocks = b.num_tiles;
-  const int64_t cap = (int64_t)sm_count * var.minb;
-  if (blocks > cap) blocks = cap;
+  const dim3 grid(persistent_grid(b.num_tiles, sm_count, f512_variant(hst.variant).minb));
   const int L = p.L == 400 ? 400 : 0;
-  if (fast512_plain(p, b)) f512_dispatch<true>(hst.variant, dt, L, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
-  else f512_dispatch<false>(hst.variant, dt, L, true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream);
+  if (fast512_plain(p, b)) f512_dispatch<true>(hst.variant, dt, L, true, hst.smem, p, hst.t, b, grid, stream);
+  else f512_dispatch<false>(hst.variant, dt, L, true, hst.smem, p, hst.t, b, grid, stream);
   return (int)cudaGetLastError();
 }

@@ -56,7 +56,6 @@ struct Tc512Tables {
   const float *c16;       // [16][16]: cos / -sin of 2 pi n2 (1 + 2 k2) / 32 at [2 k2 + part][n2] (the k1 = 16 column)
 };
 
-__device__ __forceinline__ uint32_t tc_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // tf32 (10 explicit mantissa bits) nearest to x, in an fp32 container.  hi = rna(x) and lo = rna(x - hi) leave a
 // representation error of 2^-24 |x| (masking the low bits instead would leave 2^-22: the tensor core truncates whatever it is
 // given), which keeps bins 70 dB under a frame's peak within the fp32 reference's tolerance.
@@ -104,12 +103,6 @@ template <int N>
 __device__ __forceinline__ void tc_pin(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-__device__ __forceinline__ void tc_wait(uint32_t bar, uint32_t parity) {
-  unsigned done = 0;
-  while (!done)
-    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
 }
 
 template <int DT>
@@ -163,32 +156,23 @@ __global__ void __launch_bounds__(TC_THREADS, 2)
 b200feat_tc512_kernel(const DevPlan p, const Tc512Tables tt, const DevBatch b) {
   extern __shared__ unsigned char tc_smem_raw[];
   // the swizzled B images need a 1024-byte-aligned base (the launch reserves the slack)
-  unsigned char *sC = tc_smem_raw + ((1024u - (tc_smem_u32(tc_smem_raw) & 1023u)) & 1023u);
+  unsigned char *sC = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int f = warp;                            // this warp's frame in every tile (warpgroup warp / 4 owns frames 4 (warp / 4) ..)
   const int g = lane >> 2, tq = lane & 3;        // fragment row (and row + 8) / fragment column (and column + 4)
-  const uint32_t bar0 = tc_smem_u32(sC + tt.cblob_bytes);
+  const uint32_t bar0 = smem_u32(sC + tt.cblob_bytes);
   float *V = reinterpret_cast<float *>(sC + tt.cblob_bytes + 16 + (size_t)warp * tt.warp_bytes);  // [32 n1][TC_VS]
   float *Yp = V + 32 * TC_VS;                    // [16 k1][TC_YS]: (Re, Im) Y'[n2][k1] at 2 n2
   float *Pf = Yp + 16 * TC_YS;                   // [TC_PP]
   float *Y16 = Pf + TC_PP;                       // [16]
   float *E = Y16 + 16;                           // [Mpad]
 
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) {  // constant tables: one TMA bulk copy
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar0), "r"(tt.cblob_bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(tc_smem_u32(sC)), "l"(tt.cblob), "r"(tt.cblob_bytes), "r"(bar0) : "memory");
-  }
-  tc_wait(bar0, 0);
+  blob_copy_start(bar0, sC, tt.cblob, tt.cblob_bytes);  // constant tables: one TMA bulk copy
+  mbar_wait(bar0, 0);
   const int64_t tile_begin = b.tile_base + b.num_tiles * (int64_t)blockIdx.x / gridDim.x;
   const int64_t my_tiles = b.tile_base + b.num_tiles * (int64_t)(blockIdx.x + 1) / gridDim.x - tile_begin;
 
-  const uint32_t cb = tc_smem_u32(sC);
+  const uint32_t cb = smem_u32(sC);
   const float2 *s_tw = reinterpret_cast<const float2 *>(sC + tt.off_tw);  // [k1 - 1][n2]: W512^(n2 k1), k1 = 1..16
   const int4 *s_md = reinterpret_cast<const int4 *>(sC + tt.off_md);      // [unit][slot] {first bin, float4 groups, weight index, filter}
   const float4 *s_mw4 = reinterpret_cast<const float4 *>(sC + tt.off_mw);
@@ -435,19 +419,9 @@ static inline float tc_hi_host(float x) {  // cvt.rna.tf32.f32: round to nearest
   return r;
 }
 
-template <typename T>
-static int tc_upload(const std::vector<T> &h, std::vector<void *> &allocs, const T **out) {
-  void *d = nullptr;
-  if (cudaMalloc(&d, h.size() * sizeof(T)) != cudaSuccess) return B200FEAT_ECUDA;
-  allocs.push_back(d);
-  if (cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return B200FEAT_ECUDA;
-  *out = reinterpret_cast<const T *>(d);
-  return 0;
-}
-
 // host images of the constant tables
 struct Tc512Image {
-  std::vector<unsigned char> blob;
+  ConstBlob blob;
   std::vector<float> win4, c16;
   int off_tw = 0, off_md = 0, off_mw = 0, fpu = 0, Mpad = 0;
 };
@@ -497,12 +471,10 @@ static inline int tc512_build_image(const DevPlan &p, const std::vector<float> &
       const int m = u + 16 * j;
       d[3] = -1;
       if (m >= p.M) continue;
-      int f0 = -1, f1 = -1;
-      for (int k = 0; k < p.K; ++k)
-        if (bank[(size_t)k * p.M + m] != 0.f) { if (f0 < 0) f0 = k; f1 = k; }
+      int f0, f1;
       d[3] = m;
       d[2] = (int)(mw.size() / 4);
-      if (f0 < 0) { d[0] = 0; d[1] = 0; continue; }
+      if (!filter_support(bank.data(), p.K, p.M, m, &f0, &f1)) { d[0] = 0; d[1] = 0; continue; }
       const int s0 = f0 & ~3;
       const int g = (f1 - s0) / 4 + 1;
       d[0] = s0; d[1] = g;
@@ -512,17 +484,11 @@ static inline int tc512_build_image(const DevPlan &p, const std::vector<float> &
       }
     }
   if (mw.empty()) mw.assign(4, 0.f);
-  img->blob.clear();
-  auto append = [&](const void *src, size_t bytes) -> int {
-    const size_t off = img->blob.size();
-    img->blob.resize(off + ((bytes + 15) & ~(size_t)15), 0);
-    memcpy(img->blob.data() + off, src, bytes);
-    return (int)off;
-  };
-  append(img4.data(), img4.size() * 4);
-  img->off_tw = append(tw.data(), tw.size() * sizeof(float2));
-  img->off_md = append(md.data(), md.size() * 4);
-  img->off_mw = append(mw.data(), mw.size() * 4);
+  img->blob = ConstBlob();
+  img->blob.append(img4);
+  img->off_tw = img->blob.append(tw);
+  img->off_md = img->blob.append(md);
+  img->off_mw = img->blob.append(mw);
   img->fpu = fpu;
   img->Mpad = (p.M + 3) & ~3;
   img->win4.assign(512, 0.f);
@@ -546,13 +512,9 @@ template <int DT>
 static int tc512_go(bool launch, size_t smem, const DevPlan &p, const Tc512Tables &t, const DevBatch &b, dim3 grid, cudaStream_t stream,
                     int *ctas_per_sm) {
   auto kern = b200feat_tc512_kernel<DT>;
-  if (!launch) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return B200FEAT_ECUDA;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, kern, TC_THREADS, smem) != cudaSuccess || *ctas_per_sm < 1)
-      return B200FEAT_ECUDA;
-    return 0;
-  }
-  kern<<<grid, dim3(TC_THREADS), smem, stream>>>(p, t, b);
+  if (configure_or_launch(kern, TC_THREADS, launch, smem, p, t, b, grid, stream)) return B200FEAT_ECUDA;
+  if (!launch && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, kern, TC_THREADS, smem) != cudaSuccess || *ctas_per_sm < 1))
+    return B200FEAT_ECUDA;
   return 0;
 }
 
@@ -561,15 +523,10 @@ static inline int tc512_prepare(DevPlan &p, const std::vector<float> &bank, std:
   Tc512Image img;
   tc512_build_image(p, bank, window, &img);
   Tc512Host hst;
-  int rc;
-  const unsigned char *d = nullptr;
-  if ((rc = tc_upload(img.blob, allocs, &d))) return rc;
-  hst.t.cblob = d;
-  hst.t.cblob_bytes = (int)img.blob.size();
+  if (img.blob.upload(allocs, &hst.t.cblob, &hst.t.cblob_bytes)) return B200FEAT_ECUDA;
   hst.t.off_tw = img.off_tw; hst.t.off_md = img.off_md; hst.t.off_mw = img.off_mw; hst.t.fpu = img.fpu; hst.t.Mpad = img.Mpad;
   hst.t.warp_bytes = tc512_warp_bytes(img.Mpad);
-  if ((rc = tc_upload(img.win4, allocs, &hst.t.win4))) return rc;
-  if ((rc = tc_upload(img.c16, allocs, &hst.t.c16))) return rc;
+  if (upload_table(img.win4, allocs, &hst.t.win4) || upload_table(img.c16, allocs, &hst.t.c16)) return B200FEAT_ECUDA;
   hst.smem = tc512_smem_bytes(hst.t);
   if (hst.smem > (size_t)227 * 1024) return B200FEAT_EUNSUPPORTED;
   DevBatch none{};
@@ -583,10 +540,9 @@ static inline int tc512_prepare(DevPlan &p, const std::vector<float> &bank, std:
 }
 
 static inline int tc512_launch(const DevPlan &p, const Tc512Host &hst, const DevBatch &b, int dt, int sm_count, cudaStream_t stream) {
-  int64_t blocks = b.num_tiles;
-  const int64_t cap = (int64_t)sm_count * hst.ctas_per_sm;  // persistent: every resident CTA walks a contiguous tile range
-  if (blocks > cap) blocks = cap;
-  if (dt == B200FEAT_I16) tc512_go<B200FEAT_I16>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream, nullptr);
-  else tc512_go<B200FEAT_F32>(true, hst.smem, p, hst.t, b, dim3((unsigned)blocks), stream, nullptr);
+  // persistent: every resident CTA walks a contiguous tile range
+  const dim3 grid(persistent_grid(b.num_tiles, sm_count, hst.ctas_per_sm));
+  if (dt == B200FEAT_I16) tc512_go<B200FEAT_I16>(true, hst.smem, p, hst.t, b, grid, stream, nullptr);
+  else tc512_go<B200FEAT_F32>(true, hst.smem, p, hst.t, b, grid, stream, nullptr);
   return (int)cudaGetLastError();
 }
