@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import threading
-from concurrent.futures import ThreadPoolExecutor
+from concurrent.futures import Future, ThreadPoolExecutor
 from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -196,6 +196,13 @@ class Engine:
         if rc != 0:
             raise B200FeatError(rc, self.lib.b200feat_last_error(self._h).decode())
 
+    def _check_cuts(self, rc: int):
+        """`_check` for the calls that frame the caller's cuts: B200FEAT_ESHORT (-5, a cut too short to frame) is an input
+        error and raises ValueError, as the reference does."""
+        if rc == -5:
+            raise ValueError(self.lib.b200feat_last_error(self._h).decode())
+        self._check(rc)
+
     # ------------------------------------------------------------------ integer contract
     def num_frames(self, num_samples: int) -> int:
         t = int(self.lib.b200feat_num_frames(self._h, int(num_samples)))
@@ -211,16 +218,12 @@ class Engine:
         ns = np.ascontiguousarray(num_samples, dtype=np.int64)
         off = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.int64)
         words = int(self.lib.b200feat_plan_words(self._h, _ptr(ns), B, out_mode))
-        if words == -5:
-            raise ValueError(self.lib.b200feat_last_error(self._h).decode())
         if words < 0:
-            self._check(words)
+            self._check_cuts(words)
         meta = np.empty(words, dtype=np.int64)
         tot = BatchTotals()
-        rc = self.lib.b200feat_plan_batch(self._h, _ptr(ns), _ptr(off), B, align, out_mode, _ptr(meta), words, C.byref(tot))
-        if rc == -5:
-            raise ValueError(self.lib.b200feat_last_error(self._h).decode())
-        self._check(rc)
+        self._check_cuts(self.lib.b200feat_plan_batch(self._h, _ptr(ns), _ptr(off), B, align, out_mode, _ptr(meta), words,
+                                                      C.byref(tot)))
         return meta[: tot.meta_words], tot
 
     # ------------------------------------------------------------------ device-resident path
@@ -280,11 +283,7 @@ class Engine:
         off = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.int64)
         assert (int(ns.sum()) if off is None else int(off[-1] + ns[-1])) <= numel
         B = len(ns)
-        p = self.plan
-        if p.snip_edges and p.feature not in ("whisper-fbank", "librosa-fbank"):
-            Ts = np.where(ns < p.L, 0, 1 + (ns - p.L) // p.S)
-        else:
-            Ts = (ns + p.S // 2) // p.S
+        Ts = self.plan.num_frames(ns)
         tmax = int(Ts.max())
         rows = B * tmax if out_mode == OUT_PADDED else int(Ts.sum())
         shape = (B, tmax, self.feature_dim) if out_mode == OUT_PADDED else (rows, self.feature_dim)
@@ -293,66 +292,24 @@ class Engine:
             # host allocator makes repeated allocations of the same size cheap
             out = torch.empty(shape, dtype=torch.float32, pin_memory=True).numpy()
         optr = out.data_ptr() if isinstance(out, torch.Tensor) else out.ctypes.data
-        rc = self.lib.b200feat_extract_host_at(self._h, sptr, dt, _ptr(ns), _ptr(off), B, optr, out_mode, float(pad_value))
-        if rc == -5:
-            raise ValueError(self.lib.b200feat_last_error(self._h).decode())
-        self._check(rc)
+        self._check_cuts(self.lib.b200feat_extract_host_at(self._h, sptr, dt, _ptr(ns), _ptr(off), B, optr, out_mode,
+                                                           float(pad_value)))
         return out, np.concatenate(([0], np.cumsum(Ts))).astype(np.int64)
 
-    def extract_host_list(self, arrays: Sequence[np.ndarray], dtype=np.float32, sub_bytes: int = 64 << 20):
+    def extract_host_list(self, arrays: Sequence[np.ndarray], dtype=np.float32):
         """A LIST of separately allocated host waveforms -> packed (sum T_i, F) features in pinned host memory + row prefix.
         One C call (`b200feat_extract_host_ptrs`): the library gathers the cuts into its pinned staging slots with its own
         thread pool (non-temporal stores) and overlaps that with the H2D / kernel / D2H pipeline; the GIL is released
-        throughout.  `B200FEAT_PY_GATHER=1` selects the round-1 route (Python staging threads) for A/B measurements."""
-        if os.environ.get("B200FEAT_PY_GATHER") != "1":
-            want = np.dtype(dtype)
-            arrs = [np.ascontiguousarray(a, dtype=want).reshape(-1) for a in arrays]
-            B = len(arrs)
-            ns = np.asarray([a.shape[0] for a in arrs], dtype=np.int64)
-            p = self.plan
-            if p.snip_edges and p.feature not in ("whisper-fbank", "librosa-fbank"):
-                Ts = np.where(ns < p.L, 0, 1 + (ns - p.L) // p.S)
-            else:
-                Ts = (ns + p.S // 2) // p.S
-            prefix = np.concatenate(([0], np.cumsum(Ts))).astype(np.int64)
-            out = torch.empty((int(prefix[-1]), self.feature_dim), dtype=torch.float32, pin_memory=torch.cuda.is_available()).numpy()
-            ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
-            rc = self.lib.b200feat_extract_host_ptrs(self._h, ptrs, DT_I16 if want == np.int16 else DT_F32, _ptr(ns), B, out.ctypes.data,
-                                                     OUT_PACKED, 0.0)
-            if rc == -5:
-                raise ValueError(self.lib.b200feat_last_error(self._h).decode())
-            self._check(rc)
-            return out, prefix
-        lens = [int(a.shape[0]) for a in arrays]
-        B = len(lens)
-        p = self.plan
-        ns = np.asarray(lens, dtype=np.int64)
-        if p.snip_edges and p.feature not in ("whisper-fbank", "librosa-fbank"):
-            Ts = np.where(ns < p.L, 0, 1 + (ns - p.L) // p.S)
-        else:
-            Ts = (ns + p.S // 2) // p.S
-        prefix = np.concatenate(([0], np.cumsum(Ts))).astype(np.int64)
-        pin = torch.cuda.is_available()
-        out = torch.empty((int(prefix[-1]), self.feature_dim), dtype=torch.float32, pin_memory=pin).numpy()
-        esz = 2 if np.dtype(dtype) == np.int16 else 4
-        groups = _groups(lens, sub_bytes, esz, ramp=True)
-        tdt = torch.int16 if esz == 2 else torch.float32
-        cap = max(_aligned_offsets(lens[b0:b1], 4)[1] for b0, b1 in groups)
-        bufs = [torch.empty(cap, dtype=tdt, pin_memory=pin) for _ in range(min(2, len(groups)))]
-        stager = (lambda j: stage_host(arrays[groups[j][0]: groups[j][1]], dtype=dtype, out=bufs[j % 2]))
-        cur, nxt = stager(0), None
-        side = ThreadPoolExecutor(max_workers=1) if len(groups) > 1 else None  # drives the staging of j + 1 (fans out to the pool)
-        try:
-            for j, (b0, b1) in enumerate(groups):
-                if side is not None and j + 1 < len(groups):
-                    nxt = side.submit(stager, j + 1)
-                buf, glens, goffs = cur
-                self.extract_host(buf, glens, out=out[prefix[b0]: prefix[b1]], offsets=goffs)
-                if nxt is not None:
-                    cur, nxt = nxt.result(), None
-        finally:
-            if side is not None:
-                side.shutdown(wait=True)
+        throughout."""
+        want = np.dtype(dtype)
+        arrs = [np.ascontiguousarray(a, dtype=want).reshape(-1) for a in arrays]
+        B = len(arrs)
+        ns = np.asarray([a.shape[0] for a in arrs], dtype=np.int64)
+        prefix = np.concatenate(([0], np.cumsum(self.plan.num_frames(ns)))).astype(np.int64)
+        out = torch.empty((int(prefix[-1]), self.feature_dim), dtype=torch.float32, pin_memory=torch.cuda.is_available()).numpy()
+        ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
+        self._check_cuts(self.lib.b200feat_extract_host_ptrs(self._h, ptrs, DT_I16 if want == np.int16 else DT_F32, _ptr(ns), B,
+                                                             out.ctypes.data, OUT_PACKED, 0.0))
         return out, prefix
 
     def set_output_affine(self, scale: Optional[np.ndarray], shift: Optional[np.ndarray]) -> None:
@@ -401,13 +358,12 @@ def _copy_pool() -> Optional[ThreadPoolExecutor]:
     return _POOL
 
 
-def _groups(lens: Sequence[int], target_bytes: int, esz: int, ramp: bool = False) -> List[Tuple[int, int]]:
-    """Consecutive index ranges [b0, b1) of roughly `target_bytes` each; with `ramp` the first two groups are 1/4 and 1/2
-    of that (a software pipeline starts sooner on a small first stage)."""
+def _groups(lens: Sequence[int], target_bytes: int, esz: int) -> List[Tuple[int, int]]:
+    """Consecutive index ranges [b0, b1) of roughly `target_bytes` each."""
     out, b0, acc = [], 0, 0
     for i, n in enumerate(lens):
         acc += n * esz
-        if acc >= (target_bytes >> max(0, 2 - len(out)) if ramp else target_bytes):
+        if acc >= target_bytes:
             out.append((b0, i + 1))
             b0, acc = i + 1, 0
     if b0 < len(lens):
@@ -424,6 +380,30 @@ def _aligned_offsets(lens: Sequence[int], align: int) -> Tuple[List[int], int]:
     return offs, cur
 
 
+def _zero_gaps(view: np.ndarray, lens: Sequence[int], offs: Sequence[int], b0: int = 0, b1: Optional[int] = None) -> None:
+    """Zero-fills the alignment gap in front of each cut b0 <= i < b1: defined bytes only cross PCIe."""
+    for i in range(max(b0, 1), len(lens) if b1 is None else b1):
+        view[offs[i - 1] + lens[i - 1]: offs[i]] = 0
+
+
+def _gather(view: np.ndarray, arrays: Sequence[np.ndarray], lens: List[int], offs: List[int],
+            split: int) -> List[Tuple[Tuple[int, int], Future]]:
+    """Copies arrays[i] to view[offs[i]: offs[i] + lens[i]] and zero-fills the gaps.  Below 8 MB (or with one staging
+    thread) the calling thread does it all and this returns [].  Above, the staging pool copies groups of consecutive cuts,
+    each about 1 / (split * STAGING_THREADS) of the batch, and this returns [((b0, b1), future)] in batch order."""
+    def copy(b0, b1):
+        _zero_gaps(view, lens, offs, b0, b1)
+        for i in range(b0, b1):
+            view[offs[i]: offs[i] + lens[i]] = arrays[i]
+
+    pool, esz = _copy_pool(), view.itemsize
+    total = offs[-1] + lens[-1] if lens else 0
+    if pool is None or total * esz < (8 << 20):
+        copy(0, len(lens))
+        return []
+    return [(g, pool.submit(copy, *g)) for g in _groups(lens, max(4 << 20, total * esz // (split * STAGING_THREADS)), esz)]
+
+
 def pack_device(tensors: List[torch.Tensor], device: torch.device, align: int = 4,
                 dtype: torch.dtype = torch.float32) -> Tuple[torch.Tensor, List[int], List[int]]:
     """Packs 1-D waveforms into one ragged device buffer (each start aligned to `align` elements).
@@ -432,64 +412,31 @@ def pack_device(tensors: List[torch.Tensor], device: torch.device, align: int = 
     copied device-to-device."""
     lens = [int(t.numel()) for t in tensors]
     offs, total = _aligned_offsets(lens, align)
-    if all(not t.is_cuda for t in tensors):
-        cuda = torch.cuda.is_available()
-        stage = torch.empty(total, dtype=dtype, pin_memory=cuda)
-        pool = _copy_pool()
-        esz = stage.element_size()
-
-        view = stage.numpy()
-
-        def gather(b0, b1):
-            for i in range(b0, b1):
-                if i > 0:
-                    view[offs[i - 1] + lens[i - 1]: offs[i]] = 0  # alignment gap: defined bytes only
-                t = tensors[i]
-                if t.requires_grad or not t.is_contiguous():
-                    stage[offs[i]: offs[i] + lens[i]].copy_(t.detach().reshape(-1))
-                else:  # a numpy view of the tensor: plain memcpy (3x torch's CPU copy_ on this path), GIL released
-                    view[offs[i]: offs[i] + lens[i]] = t.numpy().reshape(-1)
-
-        if pool is None or total * esz < (8 << 20) or not cuda:
-            gather(0, len(tensors))
-            return stage.to(device, non_blocking=True), lens, offs
-        dev = torch.empty(total, dtype=dtype, device=device)
-        groups = _groups(lens, max(4 << 20, total * esz // (4 * STAGING_THREADS)), esz)
-        futs = [pool.submit(gather, b0, b1) for b0, b1 in groups]
-        for (b0, b1), f in zip(groups, futs):
-            f.result()
-            e0, e1 = offs[b0], offs[b1 - 1] + lens[b1 - 1]
-            dev[e0:e1].copy_(stage[e0:e1], non_blocking=True)
-        return dev, lens, offs
-    buf = torch.empty(total, dtype=dtype, device=device)
-    for t, o, n in zip(tensors, offs, lens):
-        buf[o:o + n].copy_(t.reshape(-1), non_blocking=True)
-    return buf, lens, offs
+    if any(t.is_cuda for t in tensors):
+        buf = torch.empty(total, dtype=dtype, device=device)
+        for t, o, n in zip(tensors, offs, lens):
+            buf[o:o + n].copy_(t.reshape(-1), non_blocking=True)
+        return buf, lens, offs
+    stage = torch.empty(total, dtype=dtype, pin_memory=torch.cuda.is_available())
+    # numpy views of the tensors: a plain memcpy (3x torch's CPU copy_ on this path) that releases the GIL
+    groups = _gather(stage.numpy(), [t.detach().numpy().reshape(-1) for t in tensors], lens, offs, split=4)
+    if not groups:
+        return stage.to(device, non_blocking=True), lens, offs
+    dev = torch.empty(total, dtype=dtype, device=device)
+    for (b0, b1), f in groups:
+        f.result()
+        e0, e1 = offs[b0], offs[b1 - 1] + lens[b1 - 1]
+        dev[e0:e1].copy_(stage[e0:e1], non_blocking=True)
+    return dev, lens, offs
 
 
-def stage_host(arrays: Sequence[np.ndarray], dtype=np.float32, align: int = 4,
-               out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
-    """Copies 1-D host waveforms into ONE pinned buffer (`out`, or a fresh one), each start aligned to `align` elements
-    (gaps are zero-filled so that no uninitialised memory crosses PCIe), using the staging threads.
-    Returns (buffer, lengths, offsets) for `Engine.extract_host(offsets=)`."""
+def stage_host(arrays: Sequence[np.ndarray], dtype=np.float32, align: int = 4) -> Tuple[torch.Tensor, List[int], List[int]]:
+    """Copies 1-D host waveforms into ONE pinned buffer, each start aligned to `align` elements (gaps zero-filled), using
+    the staging threads.  Returns (buffer, lengths, offsets) for `Engine.extract_host(offsets=)`."""
     lens = [int(a.shape[0]) for a in arrays]
-    offs, cur = _aligned_offsets(lens, align)
-    tdt = torch.int16 if np.dtype(dtype) == np.int16 else torch.float32
-    stage = out if out is not None else torch.empty(max(cur, 1), dtype=tdt, pin_memory=torch.cuda.is_available())
-    assert stage.dtype == tdt and stage.numel() >= cur
-    view = stage.numpy()
-
-    def gather(b0, b1):
-        for i in range(b0, b1):
-            if i > 0:
-                view[offs[i - 1] + lens[i - 1]: offs[i]] = 0
-            view[offs[i]: offs[i] + lens[i]] = arrays[i]
-
-    pool = _copy_pool()
-    esz = 2 if tdt == torch.int16 else 4
-    if pool is None or cur * esz < (8 << 20):
-        gather(0, len(arrays))
-    else:
-        for f in [pool.submit(gather, b0, b1) for b0, b1 in _groups(lens, max(4 << 20, cur * esz // (2 * STAGING_THREADS)), esz)]:
-            f.result()
-    return stage[:max(cur, 1)], lens, offs
+    offs, total = _aligned_offsets(lens, align)
+    stage = torch.empty(max(total, 1), dtype=torch.int16 if np.dtype(dtype) == np.int16 else torch.float32,
+                        pin_memory=torch.cuda.is_available())
+    for _, f in _gather(stage.numpy(), arrays, lens, offs, split=2):
+        f.result()
+    return stage, lens, offs

@@ -27,13 +27,13 @@ from __future__ import annotations
 import dataclasses
 import warnings
 from dataclasses import asdict, dataclass
-from typing import Any, Dict, List, Optional, Sequence, Union
+from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 
 from .base import FeatureExtractor, register_extractor
-from .engine import OUT_PADDED, Engine, pack_device, stage_host
+from .engine import OUT_PADDED, Engine, pack_device
 from .plan import EPSILON, LOG_EPSILON, FeaturePlan, build_plan
 
 Seconds = float
@@ -167,6 +167,22 @@ def _first_channel_1d(x: ArrayLike) -> ArrayLike:
     raise ValueError(f"expected a (n,) or (C, n) waveform, got shape {tuple(x.shape)}")
 
 
+def _kernel_input(items: Sequence[ArrayLike]) -> Tuple[List[ArrayLike], bool]:
+    """A batch as the kernels take it: every item (numpy array or tensor) flattened to 1-D, and `(items, pcm16)`.  An
+    all-int16 batch stays int16 (the kernels widen it to x / 32768 on load); any other batch becomes float32, its int16
+    items multiplied by 1/32768 here, so that an int16 item means the same waveform in either kind of batch."""
+    flat = [x.reshape(-1) if isinstance(x, torch.Tensor) else np.asarray(x).reshape(-1) for x in items]
+    if all(x.dtype in (torch.int16, np.int16) for x in flat):
+        return flat, True
+    return [_to_float32(x) for x in flat], False
+
+
+def _to_float32(x: ArrayLike) -> ArrayLike:
+    if isinstance(x, torch.Tensor):
+        return x.to(torch.float32) * (1.0 / 32768.0) if x.dtype == torch.int16 else x.to(torch.float32)
+    return x.astype(np.float32) * np.float32(1.0 / 32768.0) if x.dtype == np.int16 else x.astype(np.float32, copy=False)
+
+
 class _B200Extractor(FeatureExtractor):
     feature_kind: str = None
     _returns_cpu_tensor = False  # Spectrogram/LogSpectrogram `.cpu()` their tensor outputs (:343, :453)
@@ -185,10 +201,13 @@ class _B200Extractor(FeatureExtractor):
             self._plan = build_plan(self.feature_kind, self.config)
         return self._plan
 
+    def _new_engine(self, plan: FeaturePlan) -> Engine:
+        return Engine(plan, device=self.config.device, kernel=getattr(self.config, "kernel", "auto"))
+
     @property
     def engine(self) -> Engine:
         if self._engine is None:
-            self._engine = Engine(self.plan, device=self.config.device, kernel=getattr(self.config, "kernel", "auto"))
+            self._engine = self._new_engine(self.plan)
         return self._engine
 
     def use_engine(self, engine: Engine) -> "_B200Extractor":
@@ -240,24 +259,45 @@ class _B200Extractor(FeatureExtractor):
 
     def extract(self, samples: ArrayLike, sampling_rate: int) -> ArrayLike:
         self._check_sr(sampling_rate)
-        is_numpy = not isinstance(samples, torch.Tensor)
-        x = _first_channel_1d(samples)
-        if is_numpy and self.config.dither != 0.0:  # noise is generated on the device: take the tensor route
-            feats = self.extract(torch.from_numpy(np.ascontiguousarray(x)), sampling_rate)
+        (x,), _ = _kernel_input([_first_channel_1d(samples)])
+        if isinstance(x, torch.Tensor):
+            feats, _ = self._extract_on_device(x.contiguous(), [x.numel()], [0])
+            return feats.cpu() if self._returns_cpu_tensor else feats
+        if self.config.dither != 0.0:  # noise is generated on the device: take the tensor route
+            feats, _ = self._extract_on_device(torch.from_numpy(np.ascontiguousarray(x)), [x.size], [0])
             return feats.cpu().numpy()
-        if is_numpy:
-            x = np.ascontiguousarray(x)
-            if x.dtype not in (np.float32, np.int16):
-                x = x.astype(np.float32)
-            feats, _ = self.engine.extract_host(x, [x.shape[0]])
-            return feats
-        x = x.contiguous()
-        if x.dtype not in (torch.float32, torch.int16):
-            x = x.to(torch.float32)
-        dev = self.engine.device
-        xd = self._dithered(x.to(dev, non_blocking=True))
-        feats, _ = self.engine.extract_device(xd, [xd.numel()], offsets=[0])
-        return feats.cpu() if self._returns_cpu_tensor else feats
+        feats, _ = self.engine.extract_host(x, [x.shape[0]])
+        return feats
+
+    def _extract_on_device(self, buf: torch.Tensor, lens: Sequence[int], offsets: Sequence[int],
+                           engine: Optional[Engine] = None, ring=None, **kw):
+        """Moves a staged 1-D batch to the engine's device (then marks `ring`'s copy in flight), adds the dither there and
+        runs the kernels: (features, row prefix) of `Engine.extract_device`."""
+        eng = engine or self.engine
+        buf = buf.to(eng.device, non_blocking=True)
+        if ring is not None:
+            ring.mark_in_flight(eng.device)
+        return eng.extract_device(self._dithered(buf), list(lens), offsets=list(offsets), **kw)
+
+    def _extract_list_on_device(self, samples: Sequence[ArrayLike], engine: Optional[Engine] = None, **kw):
+        """A list of waveforms (numpy arrays or tensors, on the host or the device), packed into one device buffer."""
+        eng = engine or self.engine
+        flat, pcm16 = _kernel_input(samples)
+        tensors = [torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x for x in flat]
+        buf, lens, offs = pack_device(tensors, eng.device, dtype=torch.int16 if pcm16 else torch.float32)
+        return self._extract_on_device(buf, lens, offs, eng, **kw)
+
+    def _extract_rows(self, samples: torch.Tensor, lengths: Optional[ArrayLike] = None):
+        """A (B, n) tensor: its rows are the ragged buffer already (offset i * n; `lengths`: the samples of each row that
+        belong to its cut), no packing.  Returns (features, per-row list of features)."""
+        B, n = samples.shape
+        lens = [n] * B
+        if lengths is not None:
+            lens = [int(l) for l in lengths]
+            assert len(lens) == B and max(lens) <= n
+        (buf,), _ = _kernel_input([samples])
+        out, prefix = self._extract_on_device(buf, lens, [i * n for i in range(B)])
+        return out, [out[prefix[i]: prefix[i + 1]] for i in range(B)]
 
     def extract_batch(
         self,
@@ -267,83 +307,40 @@ class _B200Extractor(FeatureExtractor):
     ) -> Union[ArrayLike, List[np.ndarray], List[torch.Tensor]]:
         """Container rules of `_extract_batch` (extractors.py:485-554)."""
         self._check_sr(sampling_rate)
-        eng = self.engine
-        input_is_list = False
+        input_is_list = isinstance(samples, (list, tuple))
+        input_is_torch = isinstance(samples, torch.Tensor)
         if lengths is not None:
-            assert isinstance(
-                samples, torch.Tensor
-            ), "If `lengths` is provided, `samples` must be a batched and padded torch.Tensor."
+            assert input_is_torch, "If `lengths` is provided, `samples` must be a batched and padded torch.Tensor."
             assert samples.dim() == 2
-            lens = [int(l) for l in lengths]
-            B, nmax = samples.shape
-            assert len(lens) == B and max(lens) <= nmax
-            buf = samples.contiguous()
-            if buf.dtype not in (torch.float32, torch.int16):
-                buf = buf.to(torch.float32)
-            buf = self._dithered(buf.to(eng.device, non_blocking=True).reshape(-1))
-            out, prefix = eng.extract_device(buf, lens, offsets=[i * nmax for i in range(B)])
-            result = [out[prefix[i]: prefix[i + 1]] for i in range(B)]
-            input_is_torch = True
-        elif isinstance(samples, torch.Tensor) and samples.ndim == 2:
-            # (B, n) tensor: the rows are the ragged buffer already (offset i*n) — no packing, no copies
-            B, nmax = samples.shape
-            buf = samples.contiguous()
-            if buf.dtype not in (torch.float32, torch.int16):
-                buf = buf.to(torch.float32)
-            buf = self._dithered(buf.to(eng.device, non_blocking=True).reshape(-1))
-            lens = [nmax] * B
-            out, prefix = eng.extract_device(buf, lens, offsets=[i * nmax for i in range(B)])
-            result = [out[prefix[i]: prefix[i + 1]] for i in range(B)]
-            input_is_torch = True
+            out, result = self._extract_rows(samples, lengths)
+        elif input_is_torch and samples.ndim == 2:
+            out, result = self._extract_rows(samples)
         elif isinstance(samples, np.ndarray) and samples.ndim == 2 and self.config.dither == 0.0:
             # (B, n) array: handed to the C ABI host path as is (rows are back to back)
             B, nmax = samples.shape
             arr = np.ascontiguousarray(samples)
             if arr.dtype not in (np.float32, np.int16):
                 arr = arr.astype(np.float32)
-            lens = [nmax] * B
             if arr.nbytes >= (16 << 20) and not torch.from_numpy(arr).is_pinned():
-                # pageable memory: the driver would bounce it through its own staging on ONE thread; gather the rows into
-                # pinned memory with the staging threads instead, double-buffered against the transfer
-                out, prefix = eng.extract_host_list(list(arr), dtype=arr.dtype)
+                # pageable memory: the driver would bounce it through its own staging on ONE thread; the library's gather
+                # threads copy the rows into its pinned staging instead, overlapped with the transfer
+                out, prefix = self.engine.extract_host_list(list(arr), dtype=arr.dtype)
             else:
-                out, prefix = eng.extract_host(arr.reshape(-1), lens)
+                out, prefix = self.engine.extract_host(arr.reshape(-1), [nmax] * B)
             result = [out[prefix[i]: prefix[i + 1]] for i in range(B)]
-            input_is_torch = False
         else:
-            if isinstance(samples, (list, tuple)):
-                input_is_list = True
-                items = list(samples)
-            elif samples.ndim > 1:
-                items = list(samples)
-            else:
-                items = [samples.reshape(1, -1)]
+            items = list(samples) if input_is_list or samples.ndim > 1 else [samples]
             input_is_torch = any(isinstance(x, torch.Tensor) for x in items)
-            if input_is_torch:
-                flat = [(torch.from_numpy(x) if isinstance(x, np.ndarray) else x).squeeze() for x in items]
-                dt = torch.int16 if all(t.dtype == torch.int16 for t in flat) else torch.float32
-                if dt == torch.float32:  # a mixed list: PCM items get the x / 32768 an all-int16 batch gets inside the kernel
-                    flat = [t.to(torch.float32) * (1.0 / 32768.0) if t.dtype == torch.int16 else t for t in flat]
-                buf, lens, offs = pack_device(flat, eng.device, dtype=dt)
-                out, prefix = eng.extract_device(self._dithered(buf), lens, offsets=offs)
-            elif self.config.dither != 0.0:  # numpy inputs with dither: device route, numpy results
-                flat = [torch.from_numpy(np.ascontiguousarray(np.asarray(x).squeeze())) for x in items]
-                dt = torch.int16 if all(t.dtype == torch.int16 for t in flat) else torch.float32
-                if dt == torch.float32:
-                    flat = [t.to(torch.float32) * (1.0 / 32768.0) if t.dtype == torch.int16 else t for t in flat]
-                buf, lens, offs = pack_device(flat, eng.device, dtype=dt)
-                out, prefix = eng.extract_device(self._dithered(buf), lens, offsets=offs)
-                out = out.cpu().numpy()
+            if input_is_torch or self.config.dither != 0.0:  # numpy inputs with dither: device route (noise), numpy results
+                out, prefix = self._extract_list_on_device(items)
+                if not input_is_torch:
+                    out = out.cpu().numpy()
             else:
-                flat = [np.asarray(x).squeeze() for x in items]
-                dt = np.int16 if all(a.dtype == np.int16 for a in flat) else np.float32
-                if dt == np.float32:  # mixed list: same x / 32768 as the all-int16 route
-                    flat = [a.astype(np.float32) * np.float32(1.0 / 32768.0) if a.dtype == np.int16 else a for a in flat]
-                # pinned staging with every cut on a 4-element boundary (vector-load path of the kernels), gathered by the
-                # staging threads and double-buffered against the H2D / kernel / D2H pipeline of the C call
-                lens = [int(a.shape[0]) for a in flat]
-                out, prefix = eng.extract_host_list(flat, dtype=dt)
-            result = [out[prefix[i]: prefix[i + 1]] for i in range(len(lens))]
+                # the library gathers the cuts into pinned staging, every cut on a 16-byte boundary (vector-load path of
+                # the kernels), overlapped with the H2D / kernel / D2H pipeline of the C call
+                flat, pcm16 = _kernel_input(items)
+                out, prefix = self.engine.extract_host_list(flat, dtype=np.int16 if pcm16 else np.float32)
+            result = [out[prefix[i]: prefix[i + 1]] for i in range(len(items))]
         if self._returns_cpu_tensor and input_is_torch:
             result = [r.cpu() for r in result]
 
@@ -366,8 +363,7 @@ class _B200Extractor(FeatureExtractor):
             if self.plan.snip_edges:
                 self._stream_eng = self.engine
             else:
-                plan = build_plan(self.feature_kind, dataclasses.replace(self.config, snip_edges=True))
-                self._stream_eng = Engine(plan, device=self.config.device, kernel=getattr(self.config, "kernel", "auto"))
+                self._stream_eng = self._new_engine(build_plan(self.feature_kind, dataclasses.replace(self.config, snip_edges=True)))
         return self._stream_eng
 
     def online_inference(self, samples: torch.Tensor, context: Optional[torch.Tensor] = None):
@@ -407,7 +403,7 @@ class _B200Extractor(FeatureExtractor):
     def affine_engine(self, scale, shift) -> Engine:
         """A second handle of the same plan whose kernels apply `v * scale[c] + shift[c]` in their epilogue (fused GlobalMVN,
         signal_transforms.py:16-58).  Pass it as `engine=` to the padded / packed batch entry points."""
-        eng = Engine(self.plan, device=self.config.device, kernel=getattr(self.config, "kernel", "auto"))
+        eng = self._new_engine(self.plan)
         eng.set_output_affine(scale, shift)
         return eng
 
@@ -417,24 +413,14 @@ class _B200Extractor(FeatureExtractor):
         `extract_batch` + `collate_matrices(padding_value=LOG_EPSILON)` (collation.py:506-533,
         input_strategies.py:441-462) in one launch, staying on the device."""
         self._check_sr(sampling_rate)
-        eng = engine or self.engine
-        flat = [(torch.from_numpy(x) if isinstance(x, np.ndarray) else x).squeeze() for x in samples]
-        buf, lens, offs = pack_device(flat, eng.device)
-        out, prefix = eng.extract_device(self._dithered(buf), lens, offsets=offs, out_mode=OUT_PADDED, pad_value=padding_value)
-        feat_lens = torch.from_numpy(np.diff(prefix)).to(torch.int64)
-        return out, feat_lens
+        out, prefix = self._extract_list_on_device(samples, engine, out_mode=OUT_PADDED, pad_value=padding_value)
+        return out, torch.from_numpy(np.diff(prefix)).to(torch.int64)
 
     def extract_batch_packed(self, samples: Sequence[ArrayLike], sampling_rate: int):
         """Ragged list -> (packed (sum T_i, F) tensor on the device, int64 row prefix [B + 1]): the kernels' native output
         layout, for callers that move the whole batch at once (lhotse_b200.storage, SURVEY.md §8f-3)."""
         self._check_sr(sampling_rate)
-        eng = self.engine
-        flat = [(torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x).squeeze() for x in samples]
-        dt = torch.int16 if all(t.dtype == torch.int16 for t in flat) else torch.float32
-        if dt == torch.float32:
-            flat = [t.to(torch.float32) * (1.0 / 32768.0) if t.dtype == torch.int16 else t for t in flat]
-        buf, lens, offs = pack_device(flat, eng.device, dtype=dt)
-        out, prefix = eng.extract_device(self._dithered(buf), lens, offsets=offs)
+        out, prefix = self._extract_list_on_device(samples)
         return out, np.asarray(prefix, dtype=np.int64)
 
     def extract_staged_packed(self, staged: torch.Tensor, lens: Sequence[int], offsets: Sequence[int], sampling_rate: int,
@@ -442,11 +428,7 @@ class _B200Extractor(FeatureExtractor):
         """`extract_batch_packed` for a batch already staged in ONE host buffer (the PCM16 ring; pass it as `ring` so that its
         next `stage()` waits for this asynchronous copy)."""
         self._check_sr(sampling_rate)
-        eng = self.engine
-        buf = staged.to(eng.device, non_blocking=True)
-        if ring is not None:
-            ring.mark_in_flight(eng.device)
-        out, prefix = eng.extract_device(self._dithered(buf), list(lens), offsets=list(offsets))
+        out, prefix = self._extract_on_device(staged, lens, offsets, ring=ring)
         return out, np.asarray(prefix, dtype=np.int64)
 
     def extract_staged_padded(self, staged: torch.Tensor, lens: Sequence[int], offsets: Sequence[int], sampling_rate: int,
@@ -454,13 +436,8 @@ class _B200Extractor(FeatureExtractor):
         """`extract_batch_padded` for a batch that already sits in ONE (pinned) host buffer — e.g. the int16 PCM ring of
         `lhotse_b200.pcm_staging` (SURVEY.md §8f-2): one H2D copy of the raw bytes, one launch, features stay on the device."""
         self._check_sr(sampling_rate)
-        eng = engine or self.engine
         assert staged.dim() == 1 and staged.dtype in (torch.int16, torch.float32)
-        buf = staged.to(eng.device, non_blocking=True)
-        if ring is not None:
-            ring.mark_in_flight(eng.device)
-        out, prefix = eng.extract_device(self._dithered(buf), list(lens), offsets=list(offsets), out_mode=OUT_PADDED,
-                                         pad_value=padding_value)
+        out, prefix = self._extract_on_device(staged, lens, offsets, engine, ring, out_mode=OUT_PADDED, pad_value=padding_value)
         return out, torch.from_numpy(np.diff(prefix)).to(torch.int64)
 
 

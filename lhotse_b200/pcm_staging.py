@@ -27,6 +27,8 @@ from typing import List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
+from .engine import _aligned_offsets, _zero_gaps
+
 _WAVE_FORMAT_PCM = 0x0001
 _WAVE_FORMAT_EXTENSIBLE = 0xFFFE
 _KSDATAFORMAT_SUBTYPE_PCM = bytes.fromhex("0100000000001000800000aa00389b71")
@@ -255,16 +257,11 @@ class PcmStagingRing:
             self._in_flight.synchronize()
             self._in_flight = None
         lens = [int(r.num_samples) for r in requests]
-        offs, total = [], 0
-        for n in lens:
-            total = (total + self.ALIGN - 1) // self.ALIGN * self.ALIGN
-            offs.append(total)
-            total += n
+        offs, total = _aligned_offsets(lens, self.ALIGN)
         if total > self._buf.numel():
             self._buf = torch.empty(max(total, 2 * self._buf.numel()), dtype=torch.int16, pin_memory=self._pin)
         view = self._buf.numpy()
-        for i in range(1, len(lens)):  # alignment gaps: defined bytes only
-            view[offs[i - 1] + lens[i - 1]: offs[i]] = 0
+        _zero_gaps(view, lens, offs)
         srs = set()
 
         def one(i):

@@ -12,7 +12,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
-from typing import Any, Optional
+from typing import Any, Optional, Union
 
 import numpy as np
 import torch
@@ -269,10 +269,12 @@ class FeaturePlan:
             return self.num_ceps
         return self.K
 
-    def num_frames(self, n: int) -> int:
-        """layers.py:747-753 (the in-layer twin of utils.py:424-434); whisper-fbank: whisper_fbank.py:73-80."""
+    def num_frames(self, n: Union[int, np.ndarray]) -> Union[int, np.ndarray]:
+        """layers.py:747-753 (the in-layer twin of utils.py:424-434); whisper-fbank: whisper_fbank.py:73-80.
+        `n` is a sample count or an integer array of them (element-wise)."""
         if self.snip_edges and self.feature not in ("whisper-fbank", "librosa-fbank"):
-            return 0 if n < self.L else 1 + (n - self.L) // self.S
+            t = np.where(n < self.L, 0, 1 + (n - self.L) // self.S)
+            return t if isinstance(n, np.ndarray) else int(t)
         return (n + self.S // 2) // self.S
 
     def tables_blob(self) -> np.ndarray:

@@ -55,13 +55,6 @@ def main():
         finally:
             E.STAGING_THREADS = keep
 
-    def py_gather(fn):
-        os.environ["B200FEAT_PY_GATHER"] = "1"
-        try:
-            return fn()
-        finally:
-            os.environ.pop("B200FEAT_PY_GATHER", None)
-
     print(json.dumps({"staging_threads": E.STAGING_THREADS, "cpu_count": os.cpu_count()}), flush=True)
     pageable = arr.copy()
     eng = ext.engine
@@ -71,7 +64,6 @@ def main():
                      ("list of numpy arrays, single-thread staging then C call (before)", legacy_numpy),
                      ("list of CPU torch tensors -> padded device tensor, single-thread staging (before)", legacy_torch),
                      ("list of numpy arrays (C-side gather: b200feat_extract_host_ptrs)", lambda: ext.extract_batch(lst, SR)),
-                     ("list of numpy arrays (round-1 route: Python staging threads)", lambda: py_gather(lambda: ext.extract_batch(lst, SR))),
                      ("list of CPU torch tensors -> device features", lambda: ext.extract_batch(tl, SR)),
                      ("list of CPU torch tensors -> padded device tensor", lambda: ext.extract_batch_padded(tl, SR))):
         t = timeit(fn)

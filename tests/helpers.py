@@ -140,7 +140,7 @@ class OracleEngine:
             return res, prefix
         return np.concatenate(outs, axis=0), prefix
 
-    def extract_host_list(self, arrays, dtype=np.float32, sub_bytes=0):
+    def extract_host_list(self, arrays, dtype=np.float32):
         outs, prefix = self._run([np.asarray(a) for a in arrays])
         return np.concatenate(outs, axis=0), prefix
 

@@ -104,9 +104,19 @@ def test_frame_count_contract_through_the_c_abi_without_a_gpu():
                 assert got == plan.num_frames(n)
                 if not snip:
                     assert got == O.num_frames_api(n, cfg.frame_shift, cfg.sampling_rate)
+        # the vectorised form (extract_host / extract_host_list size their outputs with it) agrees element by element
+        arr = np.asarray(ns, dtype=np.int64)
+        got = np.asarray([desc_num_frames(plan, n) for n in ns])
+        vec = plan.num_frames(arr)
+        assert isinstance(vec, np.ndarray) and vec.shape == arr.shape
+        assert np.array_equal(vec[got >= 0], got[got >= 0])
+        assert vec.tolist() == [plan.num_frames(n) for n in ns]
     wplan = lb.build_plan("whisper-fbank", lb.B200WhisperFbankConfig())
     lplan = lb.build_plan("librosa-fbank", lb.B200LibrosaFbankConfig())
     for n in ns:
         assert desc_num_frames(wplan, n) == (W.num_rows(n) if n > 200 else -5)      # torch reflect padding needs n > n_fft / 2
         assert desc_num_frames(lplan, n) == (LO.num_rows(n, 256) if n > 512 else -5)
+    for plan in (wplan, lplan):
+        got = np.asarray([desc_num_frames(plan, n) for n in ns])
+        assert np.array_equal(plan.num_frames(np.asarray(ns, dtype=np.int64))[got >= 0], got[got >= 0])
     assert desc_num_frames(wplan, -1) == -1

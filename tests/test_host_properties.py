@@ -24,14 +24,13 @@ def test_aligned_offsets_are_aligned_increasing_and_tight(lens, align):
         assert o0 + n0 <= o1 < o0 + n0 + align  # no overlap, never more than align - 1 elements of gap
 
 
-@given(lens=lens_st, target=st.integers(min_value=1, max_value=40000), ramp=st.booleans())
+@given(lens=lens_st, target=st.integers(min_value=1, max_value=40000))
 @settings(max_examples=60, deadline=None, derandomize=True)
-def test_groups_partition_the_batch_in_order(lens, target, ramp):
-    g = _groups(lens, target, 4, ramp=ramp)
+def test_groups_partition_the_batch_in_order(lens, target):
+    g = _groups(lens, target, 4)
     assert g[0][0] == 0 and g[-1][1] == len(lens) and all(a[1] == b[0] for a, b in zip(g, g[1:])) and all(b0 < b1 for b0, b1 in g)
-    for k, (b0, b1) in enumerate(g[:-1]):  # every closed group reached its target; dropping its last cut would not
-        want = (target >> max(0, 2 - k)) if ramp else target
-        assert 4 * sum(lens[b0:b1]) >= want and (want == 0 or want > 4 * sum(lens[b0:b1 - 1]))  # (a ramped target can be 0)
+    for b0, b1 in g[:-1]:  # every closed group reached its target; dropping its last cut would not
+        assert 4 * sum(lens[b0:b1]) >= target > 4 * sum(lens[b0:b1 - 1])
 
 
 @given(lens=lens_st, i16=st.booleans(), seed=st.integers(0, 2**31 - 1))

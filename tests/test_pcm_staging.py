@@ -238,60 +238,10 @@ def test_gpu_packed_batch_to_archive_roundtrip(tmp_path):
     assert np.array_equal(pa, pb) and torch.equal(a, b)
 
 
-def test_extract_host_list_pipeline_logic_with_a_recording_engine(monkeypatch):
-    """CPU-only check of the Python staging route of `Engine.extract_host_list` (`B200FEAT_PY_GATHER=1`; the default route is
-    one C call, `b200feat_extract_host_ptrs`, exercised by the `-m gpu` ragged-list tests): sub-batching, double buffering, row
-    prefix, aligned offsets.  The C call
-    is replaced by a recorder that 'extracts' one row per 160 samples holding the cut's first sample, so every row of the
-    result says which cut and which staging buffer content produced it."""
-    import lhotse_b200.engine as E
-    from lhotse_b200.plan import build_plan
-    import lhotse_b200 as lb
-
-    monkeypatch.setenv("B200FEAT_PY_GATHER", "1")
-    eng = E.Engine.__new__(E.Engine)
-    eng.plan = build_plan("fbank", lb.B200FbankConfig())
-    eng.feature_dim = 3
-    calls = []
-
-    def fake_extract_host(samples, num_samples, out_mode=0, pad_value=0.0, out=None, offsets=None):
-        buf = samples.numpy() if isinstance(samples, torch.Tensor) else samples
-        assert offsets is not None and all(o % 4 == 0 for o in offsets)
-        row = 0
-        for n, o in zip(num_samples, offsets):
-            T = (n + 80) // 160
-            out[row: row + T, 0] = buf[o]            # first sample of the cut as staged
-            out[row: row + T, 1] = buf[o + n - 1]    # last sample
-            out[row: row + T, 2] = n
-            row += T
-        assert row == out.shape[0]
-        calls.append((len(num_samples), int(sum(num_samples))))
-        return out, None
-
-    eng.extract_host = fake_extract_host
-    rs = np.random.RandomState(0)
-    lens = [int(v) for v in rs.randint(161, 5000, size=137)]
-    xs = [np.full(n, i + 1, dtype=np.float32) for i, n in enumerate(lens)]
-    for x in xs:
-        x[-1] = -x[0]
-    out, prefix = eng.extract_host_list(xs, sub_bytes=64 << 10)   # 64 KB sub-batches -> many groups, both buffers reused
-    assert len(calls) > 4 and sum(c[0] for c in calls) == len(xs) and sum(c[1] for c in calls) == sum(lens)
-    assert calls[0][1] * 4 <= (64 << 10) // 4 + 5000 * 4           # the ramp: a small first stage
-    Ts = [(n + 80) // 160 for n in lens]
-    assert prefix.tolist() == np.concatenate(([0], np.cumsum(Ts))).tolist() and out.shape == (sum(Ts), 3)
-    for i, (n, T) in enumerate(zip(lens, Ts)):
-        blk = out[prefix[i]: prefix[i + 1]]
-        assert np.all(blk[:, 0] == i + 1) and np.all(blk[:, 1] == -(i + 1)) and np.all(blk[:, 2] == n)
-    # int16 input keeps its dtype through the staging buffers
-    calls.clear()
-    out16, _ = eng.extract_host_list([x.astype(np.int16) for x in xs[:9]], dtype=np.int16, sub_bytes=8 << 10)
-    assert np.all(out16[: Ts[0], 0] == 1) and len(calls) >= 2
-
-
 @pytest.mark.gpu
 def test_gpu_large_list_routes_take_the_staged_pipelines_and_match():
-    """Lists big enough for the multi-group paths (threads + double buffering in `extract_host_list`, group-wise H2D in
-    `pack_device`) give the same bits as the plain routes."""
+    """Lists and arrays big enough for the staged routes (the library's gather threads behind `extract_host_list`, the
+    pageable (B, n) route, group-wise H2D in `pack_device`) give the same bits as the plain routes."""
     import lhotse_b200 as lb
     import lhotse_b200.engine as E
 
@@ -301,9 +251,9 @@ def test_gpu_large_list_routes_take_the_staged_pipelines_and_match():
     ext = lb.B200Fbank()
     want = ext.extract_batch(torch.from_numpy(arr).pin_memory().numpy(), 16000)   # (B, n) pinned: direct C call
     lst = [arr[i].copy() for i in range(B)]
-    out, prefix = ext.engine.extract_host_list(lst, sub_bytes=4 << 20)             # 4 MB sub-batches: ~8 groups
+    out, prefix = ext.engine.extract_host_list(lst)                                 # 30 MB: gathered by the library
     assert np.array_equal(out.reshape(want.shape), want)
-    assert np.array_equal(np.asarray(ext.extract_batch(lst, 16000)), want)          # default sub-batch size
+    assert np.array_equal(np.asarray(ext.extract_batch(lst, 16000)), want)
     assert np.array_equal(np.asarray(ext.extract_batch(arr, 16000)), want)          # pageable (B, n): staged route
     tens = [torch.from_numpy(a) for a in lst]                                       # 30 MB: group-wise H2D in pack_device
     got = ext.extract_batch(tens, 16000)
