@@ -241,6 +241,64 @@ int b200feat_set_output_affine(b200feat_handle *h, const float *scale, const flo
 
 int b200feat_get_stats(const b200feat_handle *h, b200feat_stats *out);
 
+/*
+ * FLAC (RFC 9639) on the GPU: 16-bit streams, 1-8 channels, every subframe type, both Rice methods, fixed and variable
+ * blocking.  The host indexes a file once (pure host work, no device); the device decodes one frame per job into an int16
+ * ragged buffer that b200feat_extract takes as B200FEAT_I16.
+ */
+typedef struct b200feat_flac_stream {
+  int32_t struct_size;       /* sizeof(b200feat_flac_stream) — ABI guard */
+  int32_t sample_rate, channels, bits_per_sample;
+  int32_t min_block_size, max_block_size;
+  int32_t variable_blocking; /* 1: frame headers carry the first sample number, 0: the frame number */
+  int32_t reserved;
+  int64_t total_samples;     /* per channel; 0 = unknown */
+  int64_t audio_offset;      /* byte offset of the first frame */
+  uint8_t md5[16];           /* MD5 of the interleaved little-endian samples */
+} b200feat_flac_stream;
+
+typedef struct b200feat_flac_frame {
+  int64_t byte_offset, first_sample;
+  int32_t block_size, byte_length; /* the last frame runs to the end of the file */
+} b200feat_flac_frame;
+
+/* Parses STREAMINFO and finds every frame of a whole file held in memory.  A sync candidate is a frame only when its
+ * reserved bits are zero, its CRC-8 holds, its frame / first-sample number is the next one expected, and its block size and
+ * channel count agree with STREAMINFO.  Returns the frame count (frames beyond `capacity` are counted, not written) or a
+ * negative B200FEAT_E* code. */
+int64_t b200feat_flac_index(const uint8_t *file, int64_t nbytes, b200feat_flac_stream *info, b200feat_flac_frame *frames,
+                            int64_t capacity);
+
+/* One job = one FLAC frame of one cut: samples [skip, skip + count) of channel `want_channel` go to
+ * out_dev[dst_elem, dst_elem + count).  A job of a multi-channel stream gets `count` int32 of scratch at element
+ * `scratch_elem` (decorrelated stereo needs the other channel at the same index); -1 for mono. */
+typedef struct b200feat_flac_job {
+  int64_t src_byte;       /* first byte of the frame in bytes_dev */
+  int64_t dst_elem;
+  int64_t scratch_elem;
+  int64_t coded_number;   /* frame number (fixed blocking) or first sample number (variable blocking) the header must carry */
+  int32_t byte_length, block_size, channels, want_channel, skip, count, variable_blocking, reserved;
+} b200feat_flac_job;
+
+/* per-job status written by b200feat_flac_decode */
+#define B200FEAT_FLAC_OK 0
+#define B200FEAT_FLAC_EJOB 1       /* the job itself is inconsistent (window, channel, scratch, lengths) */
+#define B200FEAT_FLAC_EHEADER 2    /* sync, reserved bits, CRC-8, or a header that disagrees with the job */
+#define B200FEAT_FLAC_ECRC 3       /* CRC-16 of the frame */
+#define B200FEAT_FLAC_ERESERVED 4  /* reserved subframe type or residual method, non-zero subframe pad bit */
+#define B200FEAT_FLAC_EPRECISION 5 /* LPC coefficient precision code 1111 */
+#define B200FEAT_FLAC_ESHIFT 6     /* negative LPC shift */
+#define B200FEAT_FLAC_EPARTITION 7 /* partition order / predictor order that does not fit the block */
+#define B200FEAT_FLAC_ERANGE 8     /* a sample outside its subframe's width or outside int16, wasted bits >= width */
+#define B200FEAT_FLAC_ETRUNCATED 9 /* the subframes run past the frame's bytes */
+#define B200FEAT_FLAC_ELENGTH 10   /* the subframes end before the frame's CRC-16 */
+
+/* Device-resident and asynchronous on `stream`: decodes `njobs` jobs out of bytes_dev into out_dev (`out_elems` int16) and
+ * writes status_dev[j] (B200FEAT_FLAC_*).  Malformed frames yield a status, never an access outside the job's byte range or
+ * output window. */
+int b200feat_flac_decode(const uint8_t *bytes_dev, const b200feat_flac_job *jobs_dev, int32_t njobs, int16_t *out_dev,
+                         int64_t out_elems, int32_t *status_dev, void *scratch_dev, int64_t scratch_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -23,6 +23,7 @@
 #include "fast2048.cuh"
 #include "fast1024.cuh"
 #include "fast400.cuh"
+#include "flac.cuh"
 
 namespace {
 
@@ -841,6 +842,24 @@ int b200feat_set_output_affine(b200feat_handle *h, const float *scale, const flo
 int b200feat_get_stats(const b200feat_handle *h, b200feat_stats *out) {
   if (!h || !out) return B200FEAT_EINVAL;
   *out = h->stats;
+  return B200FEAT_OK;
+}
+
+int64_t b200feat_flac_index(const uint8_t *file, int64_t nbytes, b200feat_flac_stream *info, b200feat_flac_frame *frames,
+                            int64_t capacity) {
+  const int64_t r = flac_index(file, nbytes, info, frames, capacity);
+  if (r < 0) fail(nullptr, (int)r, "flac_index: not a FLAC stream with a valid STREAMINFO block (or bad arguments)");
+  return r;
+}
+
+int b200feat_flac_decode(const uint8_t *bytes_dev, const b200feat_flac_job *jobs_dev, int32_t njobs, int16_t *out_dev,
+                         int64_t out_elems, int32_t *status_dev, void *scratch_dev, int64_t scratch_bytes, void *stream) {
+  if (njobs < 0 || (njobs > 0 && (!bytes_dev || !jobs_dev || !out_dev || !status_dev)) || out_elems < 0 || scratch_bytes < 0)
+    return fail(nullptr, B200FEAT_EINVAL, "flac_decode: bad arguments");
+  if (njobs == 0) return B200FEAT_OK;
+  flac_decode_kernel<<<(njobs + FLAC_THREADS - 1) / FLAC_THREADS, FLAC_THREADS, 0, (cudaStream_t)stream>>>(
+      bytes_dev, jobs_dev, njobs, out_dev, out_elems, status_dev, (int32_t *)scratch_dev, scratch_dev ? scratch_bytes / 4 : 0);
+  CU_TRY(nullptr, cudaGetLastError());
   return B200FEAT_OK;
 }
 

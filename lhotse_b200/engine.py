@@ -57,12 +57,29 @@ class Stats(C.Structure):
                 ("samples", C.c_int64), ("kernel_launches", C.c_int64)]
 
 
+class FlacStreamInfo(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("sample_rate", C.c_int32), ("channels", C.c_int32), ("bits_per_sample", C.c_int32),
+                ("min_block_size", C.c_int32), ("max_block_size", C.c_int32), ("variable_blocking", C.c_int32),
+                ("reserved", C.c_int32), ("total_samples", C.c_int64), ("audio_offset", C.c_int64), ("md5", C.c_uint8 * 16)]
+
+
+# b200feat_flac_frame / b200feat_flac_job as numpy record layouts (the job table is built with vector operations)
+FLAC_FRAME_DTYPE = np.dtype([("byte_offset", "<i8"), ("first_sample", "<i8"), ("block_size", "<i4"), ("byte_length", "<i4")])
+FLAC_JOB_DTYPE = np.dtype([("src_byte", "<i8"), ("dst_elem", "<i8"), ("scratch_elem", "<i8"), ("coded_number", "<i8"),
+                           ("byte_length", "<i4"), ("block_size", "<i4"), ("channels", "<i4"), ("want_channel", "<i4"),
+                           ("skip", "<i4"), ("count", "<i4"), ("variable_blocking", "<i4"), ("reserved", "<i4")])
+FLAC_STATUS = {1: "inconsistent job", 2: "bad frame header", 3: "CRC-16 mismatch", 4: "reserved code", 5: "invalid LPC precision",
+               6: "negative LPC shift", 7: "partition order does not fit the block", 8: "sample out of range",
+               9: "frame truncated", 10: "frame shorter than its byte range"}
+
+
 EXPORTS = [
     "b200feat_version", "b200feat_global_error", "b200feat_create", "b200feat_destroy",
     "b200feat_last_error", "b200feat_num_frames", "b200feat_feature_dim", "b200feat_kernel_kind",
     "b200feat_meta_words", "b200feat_plan_words", "b200feat_plan_batch", "b200feat_extract", "b200feat_extract_host",
     "b200feat_extract_host_at", "b200feat_desc_num_frames",
     "b200feat_get_table", "b200feat_get_stats", "b200feat_set_output_affine", "b200feat_extract_host_ptrs",
+    "b200feat_flac_index", "b200feat_flac_decode",
 ]
 
 
@@ -122,6 +139,10 @@ def load_library():
         lib.b200feat_extract_host_ptrs.argtypes = [vp, vp, i32, vp, i32, vp, i32, C.c_float]
         lib.b200feat_set_output_affine.restype = C.c_int
         lib.b200feat_set_output_affine.argtypes = [vp, vp, vp]
+        lib.b200feat_flac_index.restype = i64
+        lib.b200feat_flac_index.argtypes = [vp, i64, C.POINTER(FlacStreamInfo), vp, i64]
+        lib.b200feat_flac_decode.restype = C.c_int
+        lib.b200feat_flac_decode.argtypes = [vp, vp, i32, vp, i64, vp, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -151,6 +172,38 @@ def desc_num_frames(plan: FeaturePlan, num_samples: int) -> int:
     """Rows the kernels produce for a cut of `num_samples` under `plan` — the C library's own integer contract, callable
     without a GPU (negative: B200FEAT_ESHORT -5 when the cut cannot be framed)."""
     return int(load_library().b200feat_desc_num_frames(C.byref(plan_desc(plan)), int(num_samples)))
+
+
+def flac_index(data) -> Tuple[FlacStreamInfo, np.ndarray]:
+    """`b200feat_flac_index` over a whole FLAC file in memory (bytes or a uint8 array): (STREAMINFO, frame table as a
+    FLAC_FRAME_DTYPE array).  Pure host work (no device); ctypes releases the GIL for the scan.  Raises ValueError when the
+    data is not a native FLAC stream."""
+    lib = load_library()
+    buf = np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
+    info = FlacStreamInfo()
+    info.struct_size = C.sizeof(FlacStreamInfo)
+    cap = max(16, buf.size // 1024)
+    while True:
+        frames = np.empty(cap, dtype=FLAC_FRAME_DTYPE)
+        n = int(lib.b200feat_flac_index(buf.ctypes.data, buf.size, C.byref(info), frames.ctypes.data, cap))
+        if n < 0:
+            raise ValueError(lib.b200feat_global_error().decode())
+        if n <= cap:
+            return info, frames[:n]
+        cap = n
+
+
+def flac_decode(bytes_dev: torch.Tensor, jobs_dev: torch.Tensor, njobs: int, out: torch.Tensor, status: torch.Tensor,
+                scratch: Optional[torch.Tensor]) -> None:
+    """Launches `b200feat_flac_decode` on the current stream of `out`'s device (asynchronous; `status` holds the per-job
+    B200FEAT_FLAC_* codes once it has run)."""
+    lib = load_library()
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    rc = lib.b200feat_flac_decode(bytes_dev.data_ptr(), jobs_dev.data_ptr(), int(njobs), out.data_ptr(), out.numel(),
+                                  status.data_ptr(), None if scratch is None else scratch.data_ptr(),
+                                  0 if scratch is None else scratch.numel() * 4, stream)
+    if rc != 0:
+        raise B200FeatError(rc, lib.b200feat_global_error().decode())
 
 
 def _ptr(a: Optional[np.ndarray]):

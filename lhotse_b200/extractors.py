@@ -34,6 +34,7 @@ import torch
 
 from .base import FeatureExtractor, register_extractor
 from .engine import OUT_PADDED, Engine, pack_device
+from .pcm_staging import FlacBatch, decode_staged
 from .plan import EPSILON, LOG_EPSILON, FeaturePlan, build_plan
 
 Seconds = float
@@ -272,11 +273,15 @@ class _B200Extractor(FeatureExtractor):
     def _extract_on_device(self, buf: torch.Tensor, lens: Sequence[int], offsets: Sequence[int],
                            engine: Optional[Engine] = None, ring=None, **kw):
         """Moves a staged 1-D batch to the engine's device (then marks `ring`'s copy in flight), adds the dither there and
-        runs the kernels: (features, row prefix) of `Engine.extract_device`."""
+        runs the kernels: (features, row prefix) of `Engine.extract_device`.  A staged FLAC batch (`pcm_staging.FlacBatch`)
+        crosses compressed and is decoded on the device into the int16 ragged buffer first, on the same stream."""
         eng = engine or self.engine
-        buf = buf.to(eng.device, non_blocking=True)
-        if ring is not None:
-            ring.mark_in_flight(eng.device)
+        if isinstance(buf, FlacBatch):
+            buf, lens, offsets = decode_staged(buf, eng.device, ring)
+        else:
+            buf = buf.to(eng.device, non_blocking=True)
+            if ring is not None:
+                ring.mark_in_flight(eng.device)
         return eng.extract_device(self._dithered(buf), list(lens), offsets=list(offsets), **kw)
 
     def _extract_list_on_device(self, samples: Sequence[ArrayLike], engine: Optional[Engine] = None, **kw):
@@ -425,8 +430,8 @@ class _B200Extractor(FeatureExtractor):
 
     def extract_staged_packed(self, staged: torch.Tensor, lens: Sequence[int], offsets: Sequence[int], sampling_rate: int,
                               ring=None):
-        """`extract_batch_packed` for a batch already staged in ONE host buffer (the PCM16 ring; pass it as `ring` so that its
-        next `stage()` waits for this asynchronous copy)."""
+        """`extract_batch_packed` for a batch already staged in ONE host buffer (the PCM16 ring, or a FLAC ring's batch; pass
+        the ring as `ring` so that its next `stage()` waits for this asynchronous copy)."""
         self._check_sr(sampling_rate)
         out, prefix = self._extract_on_device(staged, lens, offsets, ring=ring)
         return out, np.asarray(prefix, dtype=np.int64)
@@ -436,7 +441,7 @@ class _B200Extractor(FeatureExtractor):
         """`extract_batch_padded` for a batch that already sits in ONE (pinned) host buffer — e.g. the int16 PCM ring of
         `lhotse_b200.pcm_staging` (SURVEY.md §8f-2): one H2D copy of the raw bytes, one launch, features stay on the device."""
         self._check_sr(sampling_rate)
-        assert staged.dim() == 1 and staged.dtype in (torch.int16, torch.float32)
+        assert isinstance(staged, FlacBatch) or (staged.dim() == 1 and staged.dtype in (torch.int16, torch.float32))
         out, prefix = self._extract_on_device(staged, lens, offsets, engine, ring, out_mode=OUT_PADDED, pad_value=padding_value)
         return out, torch.from_numpy(np.diff(prefix)).to(torch.int64)
 

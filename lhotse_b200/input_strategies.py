@@ -49,10 +49,13 @@ class FusedOnTheFlyFeatures:
         self.features_on_device = features_on_device
         # §8f-2: when every cut of the batch is a plain slice of a 16-bit PCM WAV file (and nothing has to see the float
         # waveform: no wave_transforms, no return_audio), the PCM bytes go file -> pinned int16 ring -> GPU, and are
-        # widened inside the kernel (bit-identical to the float route)
+        # widened inside the kernel (bit-identical to the float route).  When every cut is a slice of a 16-bit FLAC file, the
+        # compressed frames go file -> pinned byte ring -> GPU and are decoded there into the same int16 buffer ("flac").
+        # `pcm16_fast_path=False` turns both staged routes off.
         self.pcm16_fast_path = pcm16_fast_path and hasattr(extractor, "extract_staged_padded")
         self._ring = None
-        self.last_batch_route = None  # "pcm16" | "float" (introspection for tests / logs)
+        self._flac_ring = None
+        self.last_batch_route = None  # "pcm16" | "flac" | "float" (introspection for tests / logs)
         self._executor_type = executor_type
         self._executor = None
         # §8f-1: GlobalMVN (lhotse/dataset/signal_transforms.py:16-58) fused into the kernels' epilogue.  `global_mvn` is a
@@ -82,9 +85,10 @@ class FusedOnTheFlyFeatures:
         return self._executor
 
     def _try_pcm16(self, cuts, recording_field):
+        """(route, (features, lengths)) of a staged route, or None: the float route takes the batch."""
         if not self.pcm16_fast_path or self.wave_transforms or self.return_audio or recording_field is not None:
             return None
-        from .pcm_staging import PcmStagingRing, pcm16_request_for_cut
+        from .pcm_staging import pcm16_request_for_cut
 
         if len({c.sampling_rate for c in cuts}) != 1:
             return None  # mixed sampling rates: grouped by the float route
@@ -92,8 +96,36 @@ class FusedOnTheFlyFeatures:
         for c in cuts:
             r = pcm16_request_for_cut(c)
             if r is None:
-                return None
+                return self._try_flac(cuts)
             reqs.append(r)
+        return "pcm16", self._stage_pcm16(cuts, reqs)
+
+    def _try_flac(self, cuts):
+        from .pcm_staging import FlacStagingRing, flac_request_for_cut
+
+        reqs = []
+        for c in cuts:
+            r = flac_request_for_cut(c)
+            if r is None:
+                return None  # not every cut is a FLAC slice (e.g. a WAV / FLAC mix): the float route
+            reqs.append(r)
+        if self._flac_ring is None:
+            self._flac_ring = FlacStagingRing()
+        try:  # a frame that does not decode raises ValueError from the decode, before any feature is handed back
+            staged, lens, offs, sr = self._flac_ring.stage(reqs, executor=self._get_executor())
+            if sr != cuts[0].sampling_rate:
+                return None
+            out = self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON, ring=self._flac_ring,
+                                                       **({"engine": self._mvn_engine} if self._mvn_engine is not None else {}))
+        except (OSError, ValueError):
+            if self.fault_tolerant:
+                return None  # the float route knows how to skip broken cuts
+            raise
+        return "flac", out
+
+    def _stage_pcm16(self, cuts, reqs):
+        from .pcm_staging import PcmStagingRing
+
         if self._ring is None:
             self._ring = PcmStagingRing()
         try:
@@ -111,9 +143,8 @@ class FusedOnTheFlyFeatures:
         from lhotse.dataset.collation import collate_vectors, read_audio_from_cuts
 
         fast = self._try_pcm16(cuts, recording_field)
-        if fast is not None:
-            self.last_batch_route = "pcm16"
-            feats, feat_lens = fast
+        if fast is not None and fast[1] is not None:
+            self.last_batch_route, (feats, feat_lens) = fast
             if not self.features_on_device:
                 feats = feats.cpu()
             return (feats, feat_lens) + ((cuts,) if self.fault_tolerant else ())

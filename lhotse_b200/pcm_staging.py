@@ -12,6 +12,8 @@ ragged buffer (no float copy on the host), cross PCIe as 2 bytes per sample and 
   * `PcmStagingRing`             grow-only pinned int16 buffer; `stage(requests)` fills it back to back
   * `pcm16_request_for_cut(cut)` the (path, first sample, sample count, channel) of a lhotse MonoCut when it is eligible
                                  (one "file" source, .wav, no augmentation transforms); None otherwise
+  * `FlacStream`, `FlacStagingRing`, `flac_request_for_cut`, `decode_flac`: the same for 16-bit FLAC files, whose frames
+                                 cross PCIe compressed and are decoded by the sm_90a kernel of csrc/flac.cuh
 Everything here is host-side I/O; the arithmetic stays in the CUDA kernels.
 """
 from __future__ import annotations
@@ -102,13 +104,53 @@ class _FdCache:
 
 
 _FDS = _FdCache()
-_HEADERS: "OrderedDict[str, Tuple[Tuple[int, int], object]]" = OrderedDict()  # path -> ((size, mtime_ns), WavPcm16 | exception)
+_HEADERS: "OrderedDict[Tuple[str, str], Tuple[Tuple[int, int], object]]" = OrderedDict()  # (kind, path) -> ((size, mtime_ns), header | exception)
 _HEADERS_LOCK = threading.Lock()
 
 
 def _stamp(path: str) -> Tuple[int, int]:
     st = os.stat(path)
     return (st.st_size, st.st_mtime_ns)
+
+
+def _open_cached(kind, path: str, refusal):
+    """`kind.open(path)`, remembered in `_HEADERS` under (kind, path) while the file's size and mtime stay the same; a
+    `refusal` (the file is not of this kind) is remembered and raised again."""
+    path = str(path)
+    stamp = _stamp(path)
+    key = (kind.__name__, path)
+    with _HEADERS_LOCK:
+        ent = _HEADERS.get(key)
+        if ent is not None and ent[0] == stamp:
+            _HEADERS.move_to_end(key)
+            if isinstance(ent[1], Exception):
+                raise ent[1]
+            return ent[1]
+    try:
+        h = kind.open(path)
+    except refusal as e:
+        h = e
+    with _HEADERS_LOCK:
+        _HEADERS[key] = (stamp, h)
+        while len(_HEADERS) > 65536:
+            _HEADERS.popitem(last=False)
+    if isinstance(h, Exception):
+        raise h
+    return h
+
+
+def _pread(path: str, stamp: Tuple[int, int], view: memoryview, pos: int) -> None:
+    """Fills `view` with the file's bytes from `pos` on through the shared descriptor cache."""
+    ent = _FDS.acquire(path, stamp)  # shared descriptor, held for the duration of the read; preadv carries its own offset
+    try:
+        got = 0
+        while got < len(view):
+            k = os.preadv(ent.fd, [view[got:]], pos + got)
+            if not k:
+                raise IOError(f"{path}: short read")
+            got += k
+    finally:
+        _FDS.release(ent)
 
 
 @dataclass(frozen=True)
@@ -124,26 +166,7 @@ class WavPcm16:
     def open_cached(path: str) -> "WavPcm16":
         """`open` with the parsed header remembered per path for as long as the file's size and mtime stay the same (one
         `stat` per call instead of open + parse + close); a file that is not 16-bit PCM is remembered too."""
-        path = str(path)
-        stamp = _stamp(path)
-        with _HEADERS_LOCK:
-            ent = _HEADERS.get(path)
-            if ent is not None and ent[0] == stamp:
-                _HEADERS.move_to_end(path)
-                if isinstance(ent[1], Exception):
-                    raise ent[1]
-                return ent[1]
-        try:
-            h = WavPcm16.open(path)
-        except NotPcm16Wav as e:
-            h = e
-        with _HEADERS_LOCK:
-            _HEADERS[path] = (stamp, h)
-            while len(_HEADERS) > 65536:
-                _HEADERS.popitem(last=False)
-        if isinstance(h, Exception):
-            raise h
-        return h
+        return _open_cached(WavPcm16, path, NotPcm16Wav)
 
     @staticmethod
     def open(path: str) -> "WavPcm16":
@@ -200,19 +223,27 @@ class WavPcm16:
         else:
             raw = np.empty(self.channels * n, dtype="<i2")
             view = memoryview(raw).cast("B")
-        ent = _FDS.acquire(self.path, self.stamp)  # shared descriptor, held for the duration of the read; preadv carries its own offset
-        try:
-            got = 0
-            while got < len(view):
-                k = os.preadv(ent.fd, [view[got:]], pos + got)
-                if not k:
-                    raise IOError(f"{self.path}: short read")
-                got += k
-        finally:
-            _FDS.release(ent)
+        _pread(self.path, self.stamp, view, pos)
         if self.channels != 1:
             dst[:] = raw.reshape(n, self.channels)[:, channel]
         return n
+
+
+def _for_each(n: int, one, executor) -> None:
+    """one(i) for i in [0, n), on `executor`'s threads when there is enough work: one task per worker over a contiguous share
+    of the batch (a task per cut costs more than the read it wraps)."""
+    workers = getattr(executor, "_max_workers", 1) if executor is not None else 1
+    if executor is None or workers <= 1 or n < 2 * workers:
+        for i in range(n):
+            one(i)
+        return
+    step = (n + workers - 1) // workers
+
+    def share(a):
+        for i in range(a, min(a + step, n)):
+            one(i)
+
+    list(executor.map(share, range(0, n, step)))
 
 
 @dataclass(frozen=True)
@@ -223,15 +254,12 @@ class PcmRequest:
     channel: int = 0
 
 
-class PcmStagingRing:
-    """Grow-only pinned int16 buffer holding one ragged batch, every cut starting on a 4-sample boundary (the kernels'
-    vector-load path; `b200feat_extract_host_at` / `b200feat_plan_batch` take the offsets).
-    `stage` returns (buffer view, lengths, offsets, sampling rate)."""
+class _PinnedRing:
+    """Grow-only pinned host buffers whose contents leave for the device with asynchronous copies: `mark_in_flight` after
+    such a copy, and the next `_wait_idle` (before the buffers are refilled) waits for it."""
 
-    def __init__(self, initial_samples: int = 1 << 22, pin_memory: Optional[bool] = None):
+    def __init__(self, pin_memory: Optional[bool] = None):
         self._pin = torch.cuda.is_available() if pin_memory is None else pin_memory
-        self._buf = torch.empty(int(initial_samples), dtype=torch.int16, pin_memory=self._pin)
-        self._headers = {}
         self._in_flight = None  # CUDA event recorded after the last asynchronous H2D copy out of the ring
 
     def mark_in_flight(self, device=None) -> None:
@@ -241,6 +269,25 @@ class PcmStagingRing:
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream(device))
             self._in_flight = ev
+
+    def _wait_idle(self) -> None:
+        if self._in_flight is not None:
+            self._in_flight.synchronize()
+            self._in_flight = None
+
+    def _grown(self, buf: torch.Tensor, n: int) -> torch.Tensor:
+        return buf if n <= buf.numel() else torch.empty(max(n, 2 * buf.numel()), dtype=buf.dtype, pin_memory=self._pin)
+
+
+class PcmStagingRing(_PinnedRing):
+    """Grow-only pinned int16 buffer holding one ragged batch, every cut starting on a 4-sample boundary (the kernels'
+    vector-load path; `b200feat_extract_host_at` / `b200feat_plan_batch` take the offsets).
+    `stage` returns (buffer view, lengths, offsets, sampling rate)."""
+
+    def __init__(self, initial_samples: int = 1 << 22, pin_memory: Optional[bool] = None):
+        super().__init__(pin_memory)
+        self._buf = torch.empty(int(initial_samples), dtype=torch.int16, pin_memory=self._pin)
+        self._headers = {}
 
     def _header(self, path: str) -> WavPcm16:
         h = self._headers.get(path)
@@ -253,13 +300,10 @@ class PcmStagingRing:
     ALIGN = 4
 
     def stage(self, requests: Sequence[PcmRequest], executor=None) -> Tuple[torch.Tensor, List[int], List[int], int]:
-        if self._in_flight is not None:
-            self._in_flight.synchronize()
-            self._in_flight = None
+        self._wait_idle()
         lens = [int(r.num_samples) for r in requests]
         offs, total = _aligned_offsets(lens, self.ALIGN)
-        if total > self._buf.numel():
-            self._buf = torch.empty(max(total, 2 * self._buf.numel()), dtype=torch.int16, pin_memory=self._pin)
+        self._buf = self._grown(self._buf, total)
         view = self._buf.numpy()
         _zero_gaps(view, lens, offs)
         srs = set()
@@ -270,18 +314,7 @@ class PcmStagingRing:
             srs.add(h.sampling_rate)
             h.read_into(view[offs[i]: offs[i] + lens[i]], r.first_sample, r.channel)
 
-        workers = getattr(executor, "_max_workers", 1) if executor is not None else 1
-        if executor is None or workers <= 1 or len(requests) < 2 * workers:
-            for i in range(len(requests)):
-                one(i)
-        else:  # one task per worker over a contiguous share of the batch (a task per cut costs more than the read it wraps)
-            step = (len(requests) + workers - 1) // workers
-
-            def share(a):
-                for i in range(a, min(a + step, len(requests))):
-                    one(i)
-
-            list(executor.map(share, range(0, len(requests), step)))
+        _for_each(len(requests), one, executor)
         if len(srs) != 1:
             raise ValueError(f"one sampling rate per batch expected, got {sorted(srs)}")
         return self._buf[:total], lens, offs, srs.pop()
@@ -312,3 +345,216 @@ def pcm16_request_for_cut(cut) -> Optional[PcmRequest]:
     if first + n > h.num_samples:
         return None
     return PcmRequest(path=h.path, first_sample=first, num_samples=n, channel=sources[0].channels.index(ch))
+
+
+# ---- FLAC ----------------------------------------------------------------------------------------------------------
+# The compressed frames go file -> pinned byte ring -> one H2D copy -> the sm_90a decode kernel (csrc/flac.cuh), which writes
+# the int16 samples straight into the ragged device buffer the feature kernels take as B200FEAT_I16.  A FLAC batch crosses
+# PCIe at about half the bytes of the same audio as PCM16.
+
+
+class NotFlac16(ValueError):
+    """The file is not a native FLAC stream of 16-bit samples that the frame index can walk."""
+
+
+@dataclass(frozen=True, eq=False)
+class FlacStream:
+    path: str
+    sampling_rate: int
+    channels: int
+    num_samples: int          # per channel (STREAMINFO total samples)
+    variable_blocking: bool
+    md5: bytes
+    frames: np.ndarray        # engine.FLAC_FRAME_DTYPE: byte offset, first sample, block size, byte length
+    stamp: Tuple[int, int] = (0, 0)
+
+    @staticmethod
+    def open_cached(path: str) -> "FlacStream":
+        """`open`, remembered in the same per-path cache as the WAV headers (keyed on the file's size and mtime)."""
+        return _open_cached(FlacStream, path, NotFlac16)
+
+    @staticmethod
+    def open(path: str) -> "FlacStream":
+        from .engine import flac_index
+
+        with open(path, "rb") as f:
+            data = f.read()
+            st = os.fstat(f.fileno())
+        try:
+            info, frames = flac_index(data)
+        except ValueError as e:
+            raise NotFlac16(f"{path}: {e}") from None
+        if info.bits_per_sample != 16:
+            raise NotFlac16(f"{path}: {info.bits_per_sample}-bit samples")
+        total = int(frames["block_size"].sum())
+        if not len(frames) or info.total_samples != total:
+            raise NotFlac16(f"{path}: the frames hold {total} samples, STREAMINFO says {info.total_samples}")
+        return FlacStream(path=str(path), sampling_rate=int(info.sample_rate), channels=int(info.channels), num_samples=total,
+                          variable_blocking=bool(info.variable_blocking), md5=bytes(info.md5), frames=frames,
+                          stamp=(st.st_size, st.st_mtime_ns))
+
+
+@dataclass(frozen=True)
+class FlacRequest:
+    path: str
+    first_sample: int
+    num_samples: int
+    channel: int = 0
+
+
+@dataclass
+class FlacBatch:
+    """One staged FLAC batch: the compressed frames in the ring's pinned bytes, the job table (engine.FLAC_JOB_DTYPE, one job
+    per frame of each cut) and where every cut's samples go in the int16 output."""
+    data: torch.Tensor        # pinned uint8 view, the frames of every cut back to back
+    jobs: torch.Tensor        # pinned uint8 view of the job records
+    njobs: int
+    job_cut: np.ndarray       # cut index of every job
+    lens: List[int]
+    offsets: List[int]
+    out_elems: int
+    scratch_elems: int
+    requests: Sequence[FlacRequest]
+
+
+class FlacStagingRing(_PinnedRing):
+    """Grow-only pinned byte buffers for one FLAC batch; `stage(requests)` reads each cut's frame range into it and builds the
+    job table with vector operations over the cached frame tables.  Returns (FlacBatch, lengths, offsets, sampling rate), the
+    rate None when the files have several."""
+
+    ALIGN = 4
+
+    def __init__(self, initial_bytes: int = 1 << 22, pin_memory: Optional[bool] = None):
+        super().__init__(pin_memory)
+        self._data = torch.empty(int(initial_bytes), dtype=torch.uint8, pin_memory=self._pin)
+        self._jobs = torch.empty(1 << 16, dtype=torch.uint8, pin_memory=self._pin)
+
+    def stage(self, requests: Sequence[FlacRequest], executor=None) -> Tuple[FlacBatch, List[int], List[int], int]:
+        from .engine import FLAC_JOB_DTYPE
+
+        self._wait_idle()
+        B = len(requests)
+        streams = [FlacStream.open_cached(r.path) for r in requests]
+        srs = {s.sampling_rate for s in streams}
+        lens = [int(r.num_samples) for r in requests]
+        offs, out_elems = _aligned_offsets(lens, self.ALIGN)
+        first = np.asarray([r.first_sample for r in requests], dtype=np.int64)
+        # per cut: the frames [f0, f1) that hold samples [first, first + n)
+        f0 = np.empty(B, dtype=np.int64)
+        f1 = np.empty(B, dtype=np.int64)
+        parts = []
+        for i, (r, s) in enumerate(zip(requests, streams)):
+            if r.first_sample < 0 or r.first_sample + r.num_samples > s.num_samples or not (0 <= r.channel < s.channels):
+                raise ValueError(f"{r.path}: samples [{r.first_sample}, {r.first_sample + r.num_samples}) of channel {r.channel} "
+                                 f"outside 0..{s.num_samples} x {s.channels}")
+            fs = s.frames["first_sample"]
+            f0[i] = np.searchsorted(fs, r.first_sample, "right") - 1
+            f1[i] = max(int(f0[i]), int(np.searchsorted(fs, r.first_sample + r.num_samples, "left"))) if r.num_samples else f0[i]
+            parts.append(s.frames[f0[i]: f1[i]])
+        frames = np.concatenate(parts) if parts else np.empty(0, dtype=streams[0].frames.dtype)
+        nfr = f1 - f0
+        J = int(nfr.sum())
+        cut = np.repeat(np.arange(B), nfr)
+        start = np.concatenate(([0], np.cumsum(nfr)[:-1])).astype(np.int64)
+        index = f0[cut] + (np.arange(J) - start[cut])  # frame number within its stream
+        # the bytes of each cut's frames, back to back
+        lo = np.asarray([p["byte_offset"][0] if len(p) else 0 for p in parts], dtype=np.int64)
+        hi = np.asarray([p["byte_offset"][-1] + p["byte_length"][-1] if len(p) else 0 for p in parts], dtype=np.int64)
+        base = np.concatenate(([0], np.cumsum(hi - lo)[:-1])).astype(np.int64)
+        nbytes = int((hi - lo).sum())
+        self._data = self._grown(self._data, max(nbytes, 1))
+        data = self._data.numpy()
+
+        def one(i):
+            if hi[i] > lo[i]:
+                s = streams[i]
+                _pread(s.path, s.stamp, memoryview(data[base[i]: base[i] + hi[i] - lo[i]]), int(lo[i]))
+
+        _for_each(B, one, executor)
+        self._jobs = self._grown(self._jobs, max(J, 1) * FLAC_JOB_DTYPE.itemsize)
+        jobs = self._jobs.numpy()[: J * FLAC_JOB_DTYPE.itemsize].view(FLAC_JOB_DTYPE)
+        fsample = frames["first_sample"]
+        block = frames["block_size"].astype(np.int64)
+        a, n = first[cut], np.asarray(lens, dtype=np.int64)[cut]
+        skip = np.maximum(0, a - fsample)
+        count = np.minimum(block, a + n - fsample) - skip
+        chans = np.asarray([s.channels for s in streams], dtype=np.int32)[cut]
+        variable = np.asarray([s.variable_blocking for s in streams], dtype=np.int32)[cut]
+        multi = chans > 1
+        scr = np.cumsum(np.where(multi, count, 0))
+        jobs["src_byte"] = base[cut] + frames["byte_offset"] - lo[cut]
+        jobs["dst_elem"] = np.asarray(offs, dtype=np.int64)[cut] + fsample + skip - a
+        jobs["scratch_elem"] = np.where(multi, scr - count, -1)
+        jobs["coded_number"] = np.where(variable == 1, fsample, index)
+        jobs["byte_length"] = frames["byte_length"]
+        jobs["block_size"] = block
+        jobs["channels"] = chans
+        jobs["want_channel"] = np.asarray([r.channel for r in requests], dtype=np.int32)[cut]
+        jobs["skip"] = skip
+        jobs["count"] = count
+        jobs["variable_blocking"] = variable
+        jobs["reserved"] = 0
+        batch = FlacBatch(data=self._data[:nbytes], jobs=self._jobs[: J * FLAC_JOB_DTYPE.itemsize], njobs=J, job_cut=cut,
+                          lens=lens, offsets=offs, out_elems=out_elems, scratch_elems=int(scr[-1]) if J else 0,
+                          requests=list(requests))
+        return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)  # None: several rates (decodable, not one extraction)
+
+
+def decode_staged(batch: FlacBatch, device, ring: Optional[_PinnedRing] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
+    """The device half of the FLAC route on the current stream: H2D of the frames and the job table (then `ring`'s copy is
+    marked in flight), the decode kernel, and one small D2H of the status words.  Returns (int16 samples on `device`, lengths,
+    offsets); a frame that does not decode raises ValueError naming the file and the cut's sample range."""
+    from .engine import FLAC_STATUS, flac_decode
+
+    device = torch.device(device)
+    out = torch.zeros(max(batch.out_elems, 1), dtype=torch.int16, device=device)
+    if batch.njobs:
+        data = batch.data.to(device, non_blocking=True)
+        jobs = batch.jobs.to(device, non_blocking=True)
+        if ring is not None:
+            ring.mark_in_flight(device)
+        status = torch.empty(batch.njobs, dtype=torch.int32, device=device)
+        scratch = torch.empty(batch.scratch_elems, dtype=torch.int32, device=device) if batch.scratch_elems else None
+        flac_decode(data, jobs, batch.njobs, out, status, scratch)
+        bad = torch.nonzero(status).flatten().cpu().numpy()
+        if bad.size:
+            j = int(bad[0])
+            st = int(status[j].item())
+            r = batch.requests[int(batch.job_cut[j])]
+            raise ValueError(f"{r.path}: samples [{r.first_sample}, {r.first_sample + r.num_samples}) of channel {r.channel}: "
+                             f"FLAC decode failed ({FLAC_STATUS.get(st, st)}; {bad.size} bad frame(s) in the batch)")
+    return out, batch.lens, batch.offsets
+
+
+def decode_flac(requests: Sequence[FlacRequest], device="cuda", executor=None,
+                ring: Optional[FlacStagingRing] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
+    """Decodes the sample ranges of 16-bit FLAC files on the GPU: (int16 device tensor holding every cut at its offset, on
+    4-sample boundaries, lengths, offsets) — the ragged layout `Engine.extract_device` takes."""
+    ring = ring or FlacStagingRing()
+    batch, _, _, _ = ring.stage(requests, executor=executor)
+    return decode_staged(batch, device, ring)
+
+
+def flac_request_for_cut(cut) -> Optional[FlacRequest]:
+    """`pcm16_request_for_cut` for a slice of one 16-bit FLAC file: same eligibility (a MonoCut over a single-source "file"
+    recording with no transforms) and the same seconds -> samples arithmetic.  None when not eligible."""
+    rec = getattr(cut, "recording", None)
+    if rec is None or getattr(cut, "tracks", None) is not None or getattr(rec, "transforms", None):
+        return None
+    sources = getattr(rec, "sources", None) or []
+    if len(sources) != 1 or sources[0].type != "file" or not str(sources[0].source).lower().endswith(".flac"):
+        return None
+    ch = cut.channel
+    if not isinstance(ch, int) or ch not in sources[0].channels:
+        return None
+    try:
+        s = FlacStream.open_cached(str(sources[0].source))
+    except (NotFlac16, OSError):
+        return None
+    if s.sampling_rate != cut.sampling_rate or s.channels != len(sources[0].channels):
+        return None
+    first = int(math.floor(round(cut.start * s.sampling_rate, 8) + 0.5))
+    n = int(cut.num_samples)
+    if first + n > s.num_samples:
+        return None
+    return FlacRequest(path=s.path, first_sample=first, num_samples=n, channel=sources[0].channels.index(ch))

@@ -247,7 +247,7 @@ def compute_and_store_features_fused(
     from lhotse.qa import validate_features
     from lhotse.utils import fastcopy
 
-    from .pcm_staging import PcmStagingRing, pcm16_request_for_cut
+    from .pcm_staging import FlacStagingRing, PcmStagingRing, flac_request_for_cut, pcm16_request_for_cut
 
     register_with_lhotse()
     frame_shift = extractor.frame_shift
@@ -293,6 +293,7 @@ def compute_and_store_features_fused(
 
     failure = []  # first exception of a helper thread, re-raised by the caller
     rings = queue.Queue()
+    flac_rings = queue.Queue()  # the same hand-back protocol for batches of 16-bit FLAC slices (decoded on the GPU)
     stop = threading.Event()
     cuda_index = None  # the GPU this call works on, resolved in the calling thread ("cuda" without an index = its current device)
     try:
@@ -317,14 +318,18 @@ def compute_and_store_features_fused(
             assert all(c.sampling_rate == sr for c in batch_cuts)
             item = None
             if use_ring:
+                kind, free = "pcm", rings
                 reqs = [pcm16_request_for_cut(c) for c in batch_cuts]
+                if not all(r is not None for r in reqs):
+                    kind, free = "flac", flac_rings
+                    reqs = [flac_request_for_cut(c) for c in batch_cuts]
                 if all(r is not None for r in reqs):
-                    ring = rings.get()  # handed back by stage 2 once the batch's host-to-device copy has completed
+                    ring = free.get()  # handed back by stage 2 once the batch's host-to-device copy has completed
                     staged, lens, offs, fsr = ring.stage(reqs, executor=pool)
                     if fsr == sr:
-                        item = ("pcm", batch_cuts, sr, ring, staged, lens, offs)
+                        item = (kind, batch_cuts, sr, ring, staged, lens, offs)
                     else:
-                        rings.put(ring)
+                        free.put(ring)
             if item is None:
                 audios, batch_cuts = read_audio_from_cuts(batch_cuts, executor=pool)
                 if not batch_cuts:
@@ -333,7 +338,7 @@ def compute_and_store_features_fused(
             yield item
 
     def _extract(item):  # stage 2: the GPU
-        if item[0] == "pcm":
+        if item[0] in ("pcm", "flac"):
             _, batch_cuts, sr, ring, staged, lens, offs = item
             packed, prefix = extractor.extract_staged_packed(staged, lens, offs, sr, ring=ring)
         else:
@@ -348,7 +353,7 @@ def compute_and_store_features_fused(
                 packed = host
             packed = packed.numpy()
         if ring is not None:
-            rings.put(ring)  # the blocking copy above ordered the batch's H2D copy before this point
+            (rings if item[0] == "pcm" else flac_rings).put(ring)  # the blocking copy above ordered the batch's H2D copy before this point
         return batch_cuts, packed, prefix
 
     def _store(batch_cuts, packed, prefix):  # stage 3: archive append, then the manifest
@@ -361,6 +366,7 @@ def compute_and_store_features_fused(
         if use_ring:
             for _ in range(2 if pipelined else 1):
                 rings.put(PcmStagingRing())
+                flac_rings.put(FlacStagingRing(initial_bytes=1 << 16))
         if not pipelined:  # stage 1 and 2 in the calling thread, stage 3 one batch behind in a saver thread
             with ThreadPoolExecutor(max_workers=1) as saver:
                 futures = [saver.submit(_store, *_extract(item)) for item in _staged_batches()]
@@ -417,6 +423,8 @@ def compute_and_store_features_fused(
                         pass
                     if use_ring and rings.empty():
                         rings.put(PcmStagingRing(initial_samples=16, pin_memory=False))
+                    if use_ring and flac_rings.empty():
+                        flac_rings.put(FlacStagingRing(initial_bytes=16, pin_memory=False))
                 t_read.join()
     if pool is not None:
         pool.shutdown()
