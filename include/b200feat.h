@@ -299,6 +299,51 @@ typedef struct b200feat_flac_job {
 int b200feat_flac_decode(const uint8_t *bytes_dev, const b200feat_flac_job *jobs_dev, int32_t njobs, int16_t *out_dev,
                          int64_t out_elems, int32_t *status_dev, void *scratch_dev, int64_t scratch_bytes, void *stream);
 
+/*
+ * Audio-domain mixing of mono int16 tracks on the GPU: what lhotse's MixedCut.load_audio() computes under NumPy >= 2, bit
+ * for bit (DESIGN.md §3.1h).  The tracks are samples of two int16 device buffers (e.g. a PCM16 batch and a FLAC decode);
+ * every cut's mix is written as float32 into a ragged output buffer that b200feat_extract takes as B200FEAT_F32.
+ */
+#define B200FEAT_MIX_ROLE_MIXED 0   /* the track is part of the mix (the cut's first such track is the mixer's base) */
+#define B200FEAT_MIX_ROLE_ENERGY 1  /* a muted SNR reference: its energy sets the gains, its samples are not mixed */
+#define B200FEAT_MIX_F32 0          /* cut mode: a float32 mix */
+#define B200FEAT_MIX_SCALED_FIRST 1 /* cut mode: the first track carries an SNR against another reference; when both energies
+                                       are positive it is scaled in float64 and the whole mix is float64 */
+
+typedef struct b200feat_mix_track {
+  int32_t struct_size;   /* sizeof(b200feat_mix_track) — ABI guard, in every record */
+  int32_t source;        /* 0: src0, 1: src1, -1: padding (zeros) */
+  int64_t src_elem;      /* first sample of the track in its source buffer */
+  int64_t num_samples;   /* track length */
+  int64_t mix_offset;    /* first sample of the track in the mix */
+  double snr_factor;     /* 10 ** (-snr / 10) as the host evaluates it; NaN: the track has no SNR */
+  int32_t cut;           /* index of the cut the track belongs to */
+  int32_t role;          /* B200FEAT_MIX_ROLE_* */
+} b200feat_mix_track;
+
+typedef struct b200feat_mix_cut {
+  int32_t struct_size;   /* sizeof(b200feat_mix_cut) */
+  int32_t mode;          /* B200FEAT_MIX_F32 | B200FEAT_MIX_SCALED_FIRST */
+  int64_t out_elem;      /* first output element of the cut */
+  int64_t mix_len;       /* max(offset + length) over the mixed tracks */
+  int64_t target_len;    /* the cut's length: the mix is trimmed, or reflect-padded by at most mix_len - 1 samples */
+  int32_t first_track;   /* the cut's tracks are [first_track, first_track + num_tracks) of the track table, in track order */
+  int32_t num_tracks;
+  int32_t ref_track;     /* the SNR reference, relative to first_track */
+  int32_t reserved;
+} b200feat_mix_cut;
+
+/* Device scratch b200feat_mix needs for `ntracks` tracks and `ncuts` cuts. */
+int64_t b200feat_mix_work_bytes(int32_t ntracks, int32_t ncuts);
+
+/* Checks the host tables (every track inside its source buffer, every cut inside the output, source and reference indices),
+ * copies them to `work_dev` and launches the energy and mix kernels, asynchronously on `stream`.  The tables may be pinned:
+ * they are read by the copy on `stream`, so they must stay unchanged until it has run.  Errors are reported through `h`
+ * (b200feat_last_error) when it is not NULL, and through b200feat_global_error. */
+int b200feat_mix(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
+                 const b200feat_mix_track *tracks, int32_t ntracks, const b200feat_mix_cut *cuts, int32_t ncuts,
+                 float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -24,6 +24,7 @@
 #include "fast1024.cuh"
 #include "fast400.cuh"
 #include "flac.cuh"
+#include "mix.cuh"
 
 namespace {
 
@@ -860,6 +861,83 @@ int b200feat_flac_decode(const uint8_t *bytes_dev, const b200feat_flac_job *jobs
   flac_decode_kernel<<<(njobs + FLAC_THREADS - 1) / FLAC_THREADS, FLAC_THREADS, 0, (cudaStream_t)stream>>>(
       bytes_dev, jobs_dev, njobs, out_dev, out_elems, status_dev, (int32_t *)scratch_dev, scratch_dev ? scratch_bytes / 4 : 0);
   CU_TRY(nullptr, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+int64_t b200feat_mix_work_bytes(int32_t ntracks, int32_t ncuts) {
+  if (ntracks < 0 || ncuts < 0) return 0;
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  return up((int64_t)ntracks * (int64_t)sizeof(b200feat_mix_track)) + up((int64_t)ncuts * (int64_t)sizeof(b200feat_mix_cut)) +
+         up((int64_t)ntracks * 8) + up((int64_t)ntracks * 4) + up((int64_t)ncuts * 8);
+}
+
+int b200feat_mix(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
+                 const b200feat_mix_track *tracks, int32_t ntracks, const b200feat_mix_cut *cuts, int32_t ncuts,
+                 float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream) {
+  if (ntracks < 0 || ncuts < 0 || (ncuts > 0 && (!tracks || !cuts || !out_dev || !work_dev)) || out_elems < 0 || src0_elems < 0 ||
+      src1_elems < 0)
+    return fail(h, B200FEAT_EINVAL, "mix: bad arguments");
+  if (ncuts == 0) return B200FEAT_OK;
+  if (ncuts > 65535) return fail(h, B200FEAT_EINVAL, "mix: more than 65535 cuts in one call");
+  if (work_bytes < b200feat_mix_work_bytes(ntracks, ncuts)) return fail(h, B200FEAT_EINVAL, "mix: work buffer too small");
+  const int16_t *src[2] = {src0_dev, src1_dev};
+  const int64_t src_elems[2] = {src0_elems, src1_elems};
+  auto where = [](const char *what, int64_t i) { return std::string("mix: ") + what + " " + std::to_string(i) + ": "; };
+  for (int32_t t = 0; t < ntracks; ++t) {
+    const b200feat_mix_track &tr = tracks[t];
+    if (tr.struct_size != (int32_t)sizeof(b200feat_mix_track))
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "b200feat_mix_track size mismatch (ABI)");
+    if (tr.source < -1 || tr.source > 1) return fail(h, B200FEAT_EINVAL, where("track", t) + "source must be 0, 1 or -1 (padding)");
+    if (tr.num_samples < 0 || tr.num_samples > ((int64_t)1 << 40) || tr.mix_offset < 0 || tr.mix_offset > ((int64_t)1 << 40))
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "bad length or mix offset");
+    if (tr.source >= 0 && (!src[tr.source] || tr.src_elem < 0 || tr.src_elem + tr.num_samples > src_elems[tr.source]))
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "samples outside its source buffer");
+    if (tr.role != B200FEAT_MIX_ROLE_MIXED && tr.role != B200FEAT_MIX_ROLE_ENERGY)
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "bad role");
+    if (tr.cut < 0 || tr.cut >= ncuts) return fail(h, B200FEAT_EINVAL, where("track", t) + "cut index out of range");
+  }
+  for (int32_t c = 0; c < ncuts; ++c) {
+    const b200feat_mix_cut &cu = cuts[c];
+    if (cu.struct_size != (int32_t)sizeof(b200feat_mix_cut))
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "b200feat_mix_cut size mismatch (ABI)");
+    if (cu.mode != B200FEAT_MIX_F32 && cu.mode != B200FEAT_MIX_SCALED_FIRST) return fail(h, B200FEAT_EINVAL, where("cut", c) + "bad mode");
+    if (cu.num_tracks < 1 || cu.first_track < 0 || (int64_t)cu.first_track + cu.num_tracks > ntracks)
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "tracks outside the track table");
+    if (cu.ref_track < 0 || cu.ref_track >= cu.num_tracks) return fail(h, B200FEAT_EINVAL, where("cut", c) + "reference index outside the cut's tracks");
+    if (cu.out_elem < 0 || cu.target_len < 0 || cu.out_elem + cu.target_len > out_elems)
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "outside the output buffer");
+    int64_t len = 0;
+    for (int32_t k = 0; k < cu.num_tracks; ++k) {
+      const b200feat_mix_track &tr = tracks[cu.first_track + k];
+      if (tr.cut != c) return fail(h, B200FEAT_EINVAL, where("cut", c) + "a track of another cut inside its range");
+      if (k == 0 && tr.role != B200FEAT_MIX_ROLE_MIXED) return fail(h, B200FEAT_EINVAL, where("cut", c) + "the first track must be mixed");
+      if (tr.role == B200FEAT_MIX_ROLE_MIXED) len = std::max(len, tr.mix_offset + tr.num_samples);
+    }
+    if (len != cu.mix_len) return fail(h, B200FEAT_EINVAL, where("cut", c) + "mix_len is not the end of its last track");
+    if (cu.target_len > cu.mix_len && cu.target_len - cu.mix_len > cu.mix_len - 1)
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "reflect padding longer than the mix");
+  }
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  char *w = (char *)work_dev;
+  b200feat_mix_track *d_tracks = (b200feat_mix_track *)w;
+  w += up((int64_t)ntracks * (int64_t)sizeof(b200feat_mix_track));
+  b200feat_mix_cut *d_cuts = (b200feat_mix_cut *)w;
+  w += up((int64_t)ncuts * (int64_t)sizeof(b200feat_mix_cut));
+  double *energy = (double *)w;
+  w += up((int64_t)ntracks * 8);
+  float *gain32 = (float *)w;
+  w += up((int64_t)ntracks * 4);
+  double *scale64 = (double *)w;
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (ntracks) CU_TRY(h, cudaMemcpyAsync(d_tracks, tracks, (size_t)ntracks * sizeof(b200feat_mix_track), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_cuts, cuts, (size_t)ncuts * sizeof(b200feat_mix_cut), cudaMemcpyHostToDevice, st));
+  mix_energy_kernel<<<ncuts, MIX_THREADS, 0, st>>>(src0_dev, src1_dev, d_tracks, d_cuts, energy, gain32, scale64);
+  CU_TRY(h, cudaGetLastError());
+  int64_t longest = 1;
+  for (int32_t c = 0; c < ncuts; ++c) longest = std::max(longest, cuts[c].target_len);
+  const int64_t gx = std::min<int64_t>((longest + 4 * MIX_MIX_THREADS - 1) / (4 * MIX_MIX_THREADS), 1024);
+  mix_kernel<<<dim3((unsigned)gx, (unsigned)ncuts), MIX_MIX_THREADS, 0, st>>>(src0_dev, src1_dev, d_tracks, d_cuts, gain32, scale64, out_dev);
+  CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }
 

@@ -72,6 +72,14 @@ FLAC_STATUS = {1: "inconsistent job", 2: "bad frame header", 3: "CRC-16 mismatch
                6: "negative LPC shift", 7: "partition order does not fit the block", 8: "sample out of range",
                9: "frame truncated", 10: "frame shorter than its byte range"}
 
+# b200feat_mix_track / b200feat_mix_cut as numpy record layouts (the staged-mix tables are built with vector operations)
+MIX_TRACK_DTYPE = np.dtype([("struct_size", "<i4"), ("source", "<i4"), ("src_elem", "<i8"), ("num_samples", "<i8"),
+                            ("mix_offset", "<i8"), ("snr_factor", "<f8"), ("cut", "<i4"), ("role", "<i4")])
+MIX_CUT_DTYPE = np.dtype([("struct_size", "<i4"), ("mode", "<i4"), ("out_elem", "<i8"), ("mix_len", "<i8"), ("target_len", "<i8"),
+                          ("first_track", "<i4"), ("num_tracks", "<i4"), ("ref_track", "<i4"), ("reserved", "<i4")])
+MIX_ROLE_MIXED, MIX_ROLE_ENERGY = 0, 1
+MIX_F32, MIX_SCALED_FIRST = 0, 1
+
 
 EXPORTS = [
     "b200feat_version", "b200feat_global_error", "b200feat_create", "b200feat_destroy",
@@ -79,7 +87,7 @@ EXPORTS = [
     "b200feat_meta_words", "b200feat_plan_words", "b200feat_plan_batch", "b200feat_extract", "b200feat_extract_host",
     "b200feat_extract_host_at", "b200feat_desc_num_frames",
     "b200feat_get_table", "b200feat_get_stats", "b200feat_set_output_affine", "b200feat_extract_host_ptrs",
-    "b200feat_flac_index", "b200feat_flac_decode",
+    "b200feat_flac_index", "b200feat_flac_decode", "b200feat_mix_work_bytes", "b200feat_mix",
 ]
 
 
@@ -143,6 +151,10 @@ def load_library():
         lib.b200feat_flac_index.argtypes = [vp, i64, C.POINTER(FlacStreamInfo), vp, i64]
         lib.b200feat_flac_decode.restype = C.c_int
         lib.b200feat_flac_decode.argtypes = [vp, vp, i32, vp, i64, vp, vp, i64, vp]
+        lib.b200feat_mix_work_bytes.restype = i64
+        lib.b200feat_mix_work_bytes.argtypes = [i32, i32]
+        lib.b200feat_mix.restype = C.c_int
+        lib.b200feat_mix.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -204,6 +216,28 @@ def flac_decode(bytes_dev: torch.Tensor, jobs_dev: torch.Tensor, njobs: int, out
                                   0 if scratch is None else scratch.numel() * 4, stream)
     if rc != 0:
         raise B200FeatError(rc, lib.b200feat_global_error().decode())
+
+
+def mix(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], tracks: np.ndarray, cuts: np.ndarray, out: torch.Tensor,
+        handle=None) -> None:
+    """Launches `b200feat_mix` on the current stream of `out`'s device (asynchronous): the int16 device sources (None =
+    empty), the host track / cut tables (MIX_TRACK_DTYPE / MIX_CUT_DTYPE arrays, pinned or not: they are read by a copy on the
+    same stream, so a pinned table must not change until that copy has run) and the float32 output.  Raises B200FeatError
+    when the library refuses the tables."""
+    lib = load_library()
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    assert tracks.dtype == MIX_TRACK_DTYPE and cuts.dtype == MIX_CUT_DTYPE and out.dtype == torch.float32
+    work = torch.empty(max(int(lib.b200feat_mix_work_bytes(len(tracks), len(cuts))), 1), dtype=torch.uint8, device=out.device)
+
+    def src(t):
+        return (None, 0) if t is None or t.numel() == 0 else (t.data_ptr(), t.numel())
+
+    (p0, n0), (p1, n1) = src(src0), src(src1)
+    rc = lib.b200feat_mix(handle, p0, n0, p1, n1, tracks.ctypes.data, len(tracks), cuts.ctypes.data, len(cuts), out.data_ptr(),
+                          out.numel(), work.data_ptr(), work.numel(), stream)
+    if rc != 0:
+        msg = (lib.b200feat_last_error(handle) if handle is not None else lib.b200feat_global_error()).decode()
+        raise B200FeatError(rc, msg)
 
 
 def _ptr(a: Optional[np.ndarray]):

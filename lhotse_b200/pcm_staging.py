@@ -558,3 +558,239 @@ def flac_request_for_cut(cut) -> Optional[FlacRequest]:
     if first + n > s.num_samples:
         return None
     return FlacRequest(path=s.path, first_sample=first, num_samples=n, channel=sources[0].channels.index(ch))
+
+
+# ---- MixedCut ------------------------------------------------------------------------------------------------------
+# A MixedCut's tracks are staged as int16 by the two rings above (WAV tracks through PcmStagingRing, FLAC tracks through
+# FlacStagingRing), and the sm_90a kernels of csrc/mix.cuh compute the energies, the gains and the mix on the device, bit for
+# bit what MixedCut.load_audio() returns under NumPy >= 2 (DESIGN.md §3.1h).  The mixes land as float32 in the ragged layout
+# `Engine.extract_device` takes.
+
+
+@dataclass(frozen=True)
+class MixTrackRequest:
+    source: Optional[object]  # PcmRequest | FlacRequest; None = a PaddingCut (zeros)
+    num_samples: int
+    offset: int               # first sample in the mix
+    snr_factor: float         # 10 ** (-snr / 10) as Python evaluates it; NaN = no SNR
+    role: int = 0             # engine.MIX_ROLE_MIXED | engine.MIX_ROLE_ENERGY (a muted SNR reference)
+
+
+@dataclass(frozen=True)
+class MixRequest:
+    tracks: Tuple[MixTrackRequest, ...]  # the audible tracks in track order, then a muted SNR reference if there is one
+    ref: int                             # index of the SNR reference in `tracks`
+    mode: int                            # engine.MIX_F32 | engine.MIX_SCALED_FIRST
+    mix_len: int                         # max(offset + length) over the mixed tracks
+    num_samples: int                     # the cut's length: the mix is trimmed or reflect-padded to it
+
+
+def _numpy2() -> bool:
+    return int(np.__version__.split(".")[0]) >= 2
+
+
+def mix_request_for_cut(cut) -> Optional[MixRequest]:
+    """What `MixedCut.load_audio()` (lhotse/cut/mixed.py) amounts to for a MixedCut of mono 16-bit WAV / FLAC slices and
+    PaddingCuts: tracks, offsets, SNR factors, reference and length.  None when the cut is not eligible: not a MixedCut,
+    cut-level transforms, a track that `pcm16_request_for_cut` / `flac_request_for_cut` refuse (MultiCut, nested MixedCut,
+    recording transforms, other formats), a sampling rate other than the cut's, an empty track, a length outside lhotse's
+    duration-mismatch tolerance, or NumPy 1.x (whose promotion of np.float64 * float32 arrays differs)."""
+    if not _numpy2():
+        return None
+    try:
+        from lhotse.audio.utils import get_audio_duration_mismatch_tolerance
+        from lhotse.cut import MixedCut, MonoCut, PaddingCut
+        from lhotse.utils import compute_num_samples
+    except ImportError:
+        return None
+    from .engine import MIX_F32, MIX_ROLE_ENERGY, MIX_ROLE_MIXED, MIX_SCALED_FIRST
+
+    if not isinstance(cut, MixedCut) or getattr(cut, "transforms", None) or not cut.tracks:
+        return None
+    sr = cut.sampling_rate
+    tracks = list(cut.tracks)
+    if all(isinstance(t.cut, PaddingCut) for t in tracks):
+        return None  # no recording: load_audio() returns None
+    # _get_snr_reference_track / _get_audible_tracks
+    ref = next((t for t in tracks if getattr(t, "is_snr_reference", False)), None)
+    if ref is None:
+        ref = next((t for t in tracks if not isinstance(t.cut, PaddingCut) and t.snr is None), None)
+    if ref is None:
+        return None  # lhotse raises its own error on the float route
+    audible = [t for t in tracks if not t.mute] or tracks
+    chosen = audible + ([ref] if all(t is not ref for t in audible) else [])
+
+    def one(t, role):
+        c = t.cut
+        if c.sampling_rate != sr:
+            return None
+        if isinstance(c, PaddingCut):
+            src, n = None, compute_num_samples(c.duration, sr)
+        elif isinstance(c, MonoCut) and not isinstance(c, MixedCut):
+            src = pcm16_request_for_cut(c) or flac_request_for_cut(c)
+            if src is None:
+                return None
+            n = src.num_samples
+        else:
+            return None
+        if n <= 0:
+            return None
+        factor = float("nan") if t.snr is None else 10.0 ** (-t.snr / 10)
+        return MixTrackRequest(source=src, num_samples=int(n), offset=int(compute_num_samples(t.offset, sr)),
+                               snr_factor=factor, role=role)
+
+    reqs = []
+    for i, t in enumerate(chosen):
+        r = one(t, MIX_ROLE_MIXED if i < len(audible) else MIX_ROLE_ENERGY)
+        if r is None:
+            return None
+        reqs.append(r)
+    mix_len = max(r.offset + r.num_samples for r in reqs[: len(audible)])
+    target = int(cut.num_samples)
+    tol = compute_num_samples(get_audio_duration_mismatch_tolerance(), sr)
+    diff = mix_len - target
+    if diff != 0 and not (-tol < diff < tol and -diff <= mix_len - 1):
+        return None
+    first = audible[0]
+    mode = MIX_SCALED_FIRST if (ref is not first and first.snr is not None) else MIX_F32
+    return MixRequest(tracks=tuple(reqs), ref=next(i for i, t in enumerate(chosen) if t is ref), mode=mode, mix_len=mix_len,
+                      num_samples=target)
+
+
+def _plain_mix_request(cut) -> Optional[MixRequest]:
+    """A plain 16-bit WAV / FLAC slice as a mix of one track (the kernel writes x = q / 32768, what the float route reads)."""
+    from .engine import MIX_F32, MIX_ROLE_MIXED
+
+    if getattr(cut, "tracks", None) is not None:
+        return None
+    src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
+    if src is None or src.num_samples <= 0:
+        return None
+    return MixRequest(tracks=(MixTrackRequest(src, int(src.num_samples), 0, float("nan"), MIX_ROLE_MIXED),), ref=0,
+                      mode=MIX_F32, mix_len=int(src.num_samples), num_samples=int(src.num_samples))
+
+
+def mix_requests_for_batch(cuts) -> Optional[List[MixRequest]]:
+    """The "mix" route's requests for a batch: every cut a plain 16-bit WAV / FLAC slice or an eligible MixedCut, and at least
+    one MixedCut (batches of plain slices keep the "pcm16" / "flac" / "float" routes).  None otherwise."""
+    if not any(getattr(c, "tracks", None) is not None for c in cuts):
+        return None
+    reqs = []
+    for c in cuts:
+        r = mix_request_for_cut(c) if getattr(c, "tracks", None) is not None else _plain_mix_request(c)
+        if r is None:
+            return None
+        reqs.append(r)
+    return reqs
+
+
+@dataclass
+class MixBatch:
+    """One staged mix batch: the WAV tracks in the PCM ring's pinned int16 buffer, the FLAC tracks as a staged FlacBatch,
+    and the b200feat_mix track / cut tables (pinned numpy views) that place every cut's float32 mix in the output."""
+    pcm: Optional[torch.Tensor]
+    flac: Optional[FlacBatch]
+    tracks: np.ndarray        # engine.MIX_TRACK_DTYPE
+    cuts: np.ndarray          # engine.MIX_CUT_DTYPE
+    lens: List[int]
+    offsets: List[int]
+    out_elems: int
+
+
+class MixStagingRing(_PinnedRing):
+    """A PcmStagingRing, a FlacStagingRing and pinned table bytes for one mix batch; `stage(requests)` returns
+    (MixBatch, lengths, offsets, sampling rate), the rate None when the tracks' files have several."""
+
+    ALIGN = 4
+
+    def __init__(self, pin_memory: Optional[bool] = None):
+        super().__init__(pin_memory)
+        self.pcm = PcmStagingRing(initial_samples=1 << 20, pin_memory=self._pin)
+        self.flac = FlacStagingRing(initial_bytes=1 << 16, pin_memory=self._pin)
+        self._tables = torch.empty(1 << 16, dtype=torch.uint8, pin_memory=self._pin)
+
+    def mark_in_flight(self, device=None) -> None:
+        super().mark_in_flight(device)
+        self.pcm.mark_in_flight(device)
+        self.flac.mark_in_flight(device)
+
+    def stage(self, requests: Sequence[MixRequest], executor=None) -> Tuple[MixBatch, List[int], List[int], Optional[int]]:
+        from .engine import MIX_CUT_DTYPE, MIX_TRACK_DTYPE
+
+        self._wait_idle()
+        flat = [t for r in requests for t in r.tracks]
+        kind = np.asarray([-1 if t.source is None else (0 if isinstance(t.source, PcmRequest) else 1) for t in flat], dtype=np.int32)
+        wav = [t.source for t, k in zip(flat, kind) if k == 0]
+        flac = [t.source for t, k in zip(flat, kind) if k == 1]
+        srs = set()
+        pcm_buf, flac_batch = None, None
+        src_elem = np.zeros(len(flat), dtype=np.int64)
+        if wav:
+            pcm_buf, _, offs0, sr0 = self.pcm.stage(wav, executor=executor)
+            src_elem[kind == 0] = offs0
+            srs.add(sr0)
+        if flac:
+            flac_batch, _, offs1, sr1 = self.flac.stage(flac, executor=executor)
+            src_elem[kind == 1] = offs1
+            srs.add(sr1)
+        B, T = len(requests), len(flat)
+        lens = [int(r.num_samples) for r in requests]
+        offs, out_elems = _aligned_offsets(lens, self.ALIGN)
+        tb, cb = T * MIX_TRACK_DTYPE.itemsize, B * MIX_CUT_DTYPE.itemsize
+        self._tables = self._grown(self._tables, max(tb + cb, 1))
+        raw = self._tables.numpy()
+        tracks = raw[:tb].view(MIX_TRACK_DTYPE)
+        cuts = raw[tb: tb + cb].view(MIX_CUT_DTYPE)
+        ntr = np.asarray([len(r.tracks) for r in requests], dtype=np.int64)
+        tracks["struct_size"] = MIX_TRACK_DTYPE.itemsize
+        tracks["source"] = kind
+        tracks["src_elem"] = src_elem
+        tracks["num_samples"] = [t.num_samples for t in flat]
+        tracks["mix_offset"] = [t.offset for t in flat]
+        tracks["snr_factor"] = [t.snr_factor for t in flat]
+        tracks["cut"] = np.repeat(np.arange(B), ntr)
+        tracks["role"] = [t.role for t in flat]
+        cuts["struct_size"] = MIX_CUT_DTYPE.itemsize
+        cuts["mode"] = [r.mode for r in requests]
+        cuts["out_elem"] = offs
+        cuts["mix_len"] = [r.mix_len for r in requests]
+        cuts["target_len"] = lens
+        cuts["first_track"] = np.concatenate(([0], np.cumsum(ntr)[:-1])) if B else []
+        cuts["num_tracks"] = ntr
+        cuts["ref_track"] = [r.ref for r in requests]
+        cuts["reserved"] = 0
+        batch = MixBatch(pcm=pcm_buf, flac=flac_batch, tracks=tracks, cuts=cuts, lens=lens, offsets=offs, out_elems=out_elems)
+        return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
+
+
+def mix_staged(batch: MixBatch, device, ring: Optional[_PinnedRing] = None, handle=None) -> Tuple[torch.Tensor, List[int], List[int]]:
+    """The device half of the "mix" route on the current stream: H2D of the WAV tracks, the FLAC decode (if any), the table
+    copies, the energy and mix kernels; then `ring`'s copies are marked in flight.  Returns (float32 mixes on `device`,
+    lengths, offsets)."""
+    from .engine import mix
+
+    device = torch.device(device)
+    with torch.cuda.device(device):
+        src0 = batch.pcm.to(device, non_blocking=True) if batch.pcm is not None else None
+        src1 = decode_staged(batch.flac, device)[0] if batch.flac is not None else None
+        out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
+        mix(src0, src1, batch.tracks, batch.cuts, out, handle)
+        if ring is not None:
+            ring.mark_in_flight(device)
+    return out, batch.lens, batch.offsets
+
+
+def mix_cuts(cuts, device="cuda", executor=None,
+             ring: Optional[MixStagingRing] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
+    """Mixes MixedCuts (and plain 16-bit WAV / FLAC slices) on the GPU: (float32 device tensor holding every cut's samples at
+    its offset, on 4-sample boundaries, lengths, offsets), each cut bit-identical to float32(cut.load_audio()).  Raises
+    ValueError naming the first cut the route cannot take."""
+    reqs = []
+    for c in cuts:
+        r = mix_request_for_cut(c) if getattr(c, "tracks", None) is not None else _plain_mix_request(c)
+        if r is None:
+            raise ValueError(f"cut {getattr(c, 'id', c)!r} cannot be mixed on the GPU (see mix_request_for_cut)")
+        reqs.append(r)
+    ring = ring or MixStagingRing()
+    batch, _, _, _ = ring.stage(reqs, executor=executor)
+    return mix_staged(batch, device, ring)

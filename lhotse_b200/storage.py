@@ -247,7 +247,8 @@ def compute_and_store_features_fused(
     from lhotse.qa import validate_features
     from lhotse.utils import fastcopy
 
-    from .pcm_staging import FlacStagingRing, PcmStagingRing, flac_request_for_cut, pcm16_request_for_cut
+    from .pcm_staging import (FlacStagingRing, MixStagingRing, PcmStagingRing, flac_request_for_cut, mix_requests_for_batch,
+                              pcm16_request_for_cut)
 
     register_with_lhotse()
     frame_shift = extractor.frame_shift
@@ -294,6 +295,8 @@ def compute_and_store_features_fused(
     failure = []  # first exception of a helper thread, re-raised by the caller
     rings = queue.Queue()
     flac_rings = queue.Queue()  # the same hand-back protocol for batches of 16-bit FLAC slices (decoded on the GPU)
+    mix_rings = queue.Queue()  # ... and for batches with MixedCuts of such slices (mixed on the GPU)
+    free_rings = {"pcm": rings, "flac": flac_rings, "mix": mix_rings}
     stop = threading.Event()
     cuda_index = None  # the GPU this call works on, resolved in the calling thread ("cuda" without an index = its current device)
     try:
@@ -323,6 +326,9 @@ def compute_and_store_features_fused(
                 if not all(r is not None for r in reqs):
                     kind, free = "flac", flac_rings
                     reqs = [flac_request_for_cut(c) for c in batch_cuts]
+                if not all(r is not None for r in reqs):
+                    kind, free = "mix", mix_rings
+                    reqs = mix_requests_for_batch(batch_cuts) or [None]
                 if all(r is not None for r in reqs):
                     ring = free.get()  # handed back by stage 2 once the batch's host-to-device copy has completed
                     staged, lens, offs, fsr = ring.stage(reqs, executor=pool)
@@ -338,7 +344,7 @@ def compute_and_store_features_fused(
             yield item
 
     def _extract(item):  # stage 2: the GPU
-        if item[0] in ("pcm", "flac"):
+        if item[0] in free_rings:
             _, batch_cuts, sr, ring, staged, lens, offs = item
             packed, prefix = extractor.extract_staged_packed(staged, lens, offs, sr, ring=ring)
         else:
@@ -353,7 +359,7 @@ def compute_and_store_features_fused(
                 packed = host
             packed = packed.numpy()
         if ring is not None:
-            (rings if item[0] == "pcm" else flac_rings).put(ring)  # the blocking copy above ordered the batch's H2D copy before this point
+            free_rings[item[0]].put(ring)  # the blocking copy above ordered the batch's H2D copy before this point
         return batch_cuts, packed, prefix
 
     def _store(batch_cuts, packed, prefix):  # stage 3: archive append, then the manifest
@@ -367,6 +373,7 @@ def compute_and_store_features_fused(
             for _ in range(2 if pipelined else 1):
                 rings.put(PcmStagingRing())
                 flac_rings.put(FlacStagingRing(initial_bytes=1 << 16))
+                mix_rings.put(MixStagingRing())
         if not pipelined:  # stage 1 and 2 in the calling thread, stage 3 one batch behind in a saver thread
             with ThreadPoolExecutor(max_workers=1) as saver:
                 futures = [saver.submit(_store, *_extract(item)) for item in _staged_batches()]
@@ -425,6 +432,8 @@ def compute_and_store_features_fused(
                         rings.put(PcmStagingRing(initial_samples=16, pin_memory=False))
                     if use_ring and flac_rings.empty():
                         flac_rings.put(FlacStagingRing(initial_bytes=16, pin_memory=False))
+                    if use_ring and mix_rings.empty():
+                        mix_rings.put(MixStagingRing(pin_memory=False))
                 t_read.join()
     if pool is not None:
         pool.shutdown()
