@@ -344,6 +344,55 @@ int b200feat_mix(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems
                  const b200feat_mix_track *tracks, int32_t ntracks, const b200feat_mix_cut *cuts, int32_t ncuts,
                  float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
 
+/*
+ * Resampling and volume scaling of mono audio on the GPU: lhotse's Speed, Resample and Volume transforms as its CPU route
+ * computes them when torch runs the resampling conv1d through oneDNN, bit for bit (DESIGN.md §3.1i).  A cut's transform
+ * chain is a list of stages; stage 0 reads one of two int16 device buffers (e.g. a PCM16 batch and a FLAC decode), later
+ * stages read a float32 intermediate buffer, and the last stage writes the cut's float32 samples into a ragged output buffer
+ * that b200feat_extract takes as B200FEAT_F32.
+ */
+#define B200FEAT_RESAMPLE_SRC0 0    /* stage source: src0 (int16) */
+#define B200FEAT_RESAMPLE_SRC1 1    /* stage source: src1 (int16) */
+#define B200FEAT_RESAMPLE_MID 2     /* stage source: the float32 intermediate buffer */
+#define B200FEAT_RESAMPLE_TO_MID 0  /* stage target: the float32 intermediate buffer */
+#define B200FEAT_RESAMPLE_TO_OUT 1  /* stage target: the output buffer (the cut's final samples) */
+
+typedef struct b200feat_resample_stage {
+  int32_t struct_size;   /* sizeof(b200feat_resample_stage) — ABI guard, in every record */
+  int32_t table;         /* id from b200feat_resample_table; -1: no resampling (the scales only) */
+  int32_t source;        /* B200FEAT_RESAMPLE_SRC0 | _SRC1 | _MID */
+  int32_t target;        /* B200FEAT_RESAMPLE_TO_MID | _TO_OUT */
+  int32_t depth;         /* stages run in depth order (the records are sorted by it): depth d reads what depth d - 1 wrote */
+  float scale_in;        /* every input sample is multiplied by it on load (a Volume before the resampler; 1: none) */
+  float scale_out;       /* every output sample is multiplied by it before the store (a Volume after it; 1: none) */
+  int32_t reserved;
+  int64_t in_elem;       /* first input sample in the source buffer */
+  int64_t in_len;        /* L, at least 1 */
+  int64_t out_elem;      /* first output sample in the target buffer */
+  int64_t out_len;       /* for a table of the pair O -> N: min(ceil(f32(N * L / O)), N * (L / O + 1)), the quotient
+                            evaluated in double and rounded to float as lhotse's torch.as_tensor does; L without a table */
+  int64_t target_len;    /* samples written: out_len, or (target _TO_OUT only) fewer (trimmed) or at most out_len - 1 more
+                            (np.pad(mode="reflect")) */
+} b200feat_resample_stage;
+
+/* Registers the float32 table kernel[rows][taps] (rows = N, taps = 2 * width + O for the pair orig -> new reduced by their
+ * gcd to O -> N) on the current device and returns its id in *table_id.  Tables are kept per (device, orig, new) for the
+ * life of the process: when the pair is known on this device the stored table's id is returned and `kernel` is not read.
+ * B200FEAT_EINVAL for inconsistent sizes, or a table with taps + O > 8192 or more than 2^22 entries. */
+int b200feat_resample_table(b200feat_handle *h, int32_t orig, int32_t new_rate, const float *kernel, int32_t rows, int32_t taps,
+                            int32_t width, int32_t *table_id);
+
+/* Device scratch b200feat_resample needs for `nstages` stages. */
+int64_t b200feat_resample_work_bytes(int32_t nstages);
+
+/* Checks the host stage records (every read inside its source, every write inside its target, table ids of this device,
+ * out_len as above, reflect padding shorter than the stage output, depth order), copies them to `work_dev`
+ * and launches one kernel per depth, asynchronously on `stream`.  Errors are reported through `h` (b200feat_last_error) when
+ * it is not NULL, and through b200feat_global_error. */
+int b200feat_resample(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev,
+                      int64_t src1_elems, float *mid_dev, int64_t mid_elems, const b200feat_resample_stage *stages,
+                      int32_t nstages, float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -34,6 +34,7 @@ from .families import (  # noqa: F401
 from .engine import Engine, B200FeatError, load_library  # noqa: F401
 from .pcm_staging import FlacRequest, decode_flac, flac_request_for_cut  # noqa: F401
 from .pcm_staging import MixRequest, mix_cuts, mix_request_for_cut  # noqa: F401
+from .pcm_staging import TransformRequest, transform_cuts, transform_request_for_cut  # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -10,6 +10,7 @@
 #include <atomic>
 #include <condition_variable>
 #include <functional>
+#include <map>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -25,6 +26,7 @@
 #include "fast400.cuh"
 #include "flac.cuh"
 #include "mix.cuh"
+#include "resample.cuh"
 
 namespace {
 
@@ -938,6 +940,148 @@ int b200feat_mix(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems
   const int64_t gx = std::min<int64_t>((longest + 4 * MIX_MIX_THREADS - 1) / (4 * MIX_MIX_THREADS), 1024);
   mix_kernel<<<dim3((unsigned)gx, (unsigned)ncuts), MIX_MIX_THREADS, 0, st>>>(src0_dev, src1_dev, d_tracks, d_cuts, gain32, scale64, out_dev);
   CU_TRY(h, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Resampling tables, [K][N] on the device, kept per (device, orig, new) for the life of the process: a table is a pure
+// function of its pair, and a handle-free caller (lhotse_b200.transform_cuts) shares them with every extractor.
+struct RsTable {
+  int device;
+  int32_t orig, new_rate, N, O, K, width;
+  const float *dev;
+};
+std::mutex g_rs_mu;
+std::vector<RsTable> g_rs_tables;  // the id of a table is its index
+std::vector<void *> g_rs_allocs;
+
+}  // namespace
+
+extern "C" {
+
+int b200feat_resample_table(b200feat_handle *h, int32_t orig, int32_t new_rate, const float *kernel, int32_t rows, int32_t taps,
+                            int32_t width, int32_t *table_id) {
+  if (orig <= 0 || new_rate <= 0 || orig == new_rate || !table_id) return fail(h, B200FEAT_EINVAL, "resample_table: bad arguments");
+  int device = 0;
+  CU_TRY(h, cudaGetDevice(&device));
+  std::lock_guard<std::mutex> g(g_rs_mu);
+  for (size_t i = 0; i < g_rs_tables.size(); ++i) {
+    const RsTable &t = g_rs_tables[i];
+    if (t.device == device && t.orig == orig && t.new_rate == new_rate) {
+      *table_id = (int32_t)i;
+      return B200FEAT_OK;
+    }
+  }
+  int32_t a = orig, b = new_rate;
+  while (b) { const int32_t r = a % b; a = b; b = r; }
+  const int32_t O = orig / a, N = new_rate / a;
+  if (!kernel || rows != N || width <= 0 || taps != 2 * width + O)
+    return fail(h, B200FEAT_EINVAL, "resample_table: the table is not N x (2 * width + O) for the pair");
+  if ((int64_t)taps + O > RS_WIN_FLOATS || (int64_t)rows * taps > ((int64_t)1 << 22))
+    return fail(h, B200FEAT_EINVAL, "resample_table: table too large for the resampling kernel");
+  std::vector<float> tr((size_t)rows * taps);
+  for (int32_t p = 0; p < rows; ++p)
+    for (int32_t t = 0; t < taps; ++t) tr[(size_t)t * rows + p] = kernel[(size_t)p * taps + t];
+  const float *dev = nullptr;
+  CU_TRY(h, upload_table(tr, g_rs_allocs, &dev));
+  g_rs_tables.push_back(RsTable{device, orig, new_rate, N, O, taps, width, dev});
+  *table_id = (int32_t)(g_rs_tables.size() - 1);
+  return B200FEAT_OK;
+}
+
+int64_t b200feat_resample_work_bytes(int32_t nstages) {
+  if (nstages < 0) return 0;
+  return ((int64_t)nstages * (int64_t)sizeof(RsStage) + 255) / 256 * 256;
+}
+
+int b200feat_resample(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev,
+                      int64_t src1_elems, float *mid_dev, int64_t mid_elems, const b200feat_resample_stage *stages,
+                      int32_t nstages, float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream) {
+  if (nstages < 0 || (nstages > 0 && (!stages || !work_dev)) || src0_elems < 0 || src1_elems < 0 || mid_elems < 0 || out_elems < 0)
+    return fail(h, B200FEAT_EINVAL, "resample: bad arguments");
+  if (nstages == 0) return B200FEAT_OK;
+  if (work_bytes < b200feat_resample_work_bytes(nstages)) return fail(h, B200FEAT_EINVAL, "resample: work buffer too small");
+  int device = 0;
+  CU_TRY(h, cudaGetDevice(&device));
+  const void *src[3] = {src0_dev, src1_dev, mid_dev};
+  const int64_t src_elems[3] = {src0_elems, src1_elems, mid_elems};
+  float *dst[2] = {mid_dev, out_dev};
+  const int64_t dst_elems[2] = {mid_elems, out_elems};
+  auto where = [](int32_t i) { return std::string("resample: stage ") + std::to_string(i) + ": "; };
+  std::vector<RsStage> rs((size_t)nstages);
+  std::vector<int32_t> group_start;  // first record of every depth
+  std::vector<size_t> group_smem;
+  int64_t ctas = 0;
+  {
+    std::lock_guard<std::mutex> g(g_rs_mu);
+    for (int32_t i = 0; i < nstages; ++i) {
+      const b200feat_resample_stage &s = stages[i];
+      if (s.struct_size != (int32_t)sizeof(b200feat_resample_stage))
+        return fail(h, B200FEAT_EINVAL, where(i) + "b200feat_resample_stage size mismatch (ABI)");
+      if (s.source < 0 || s.source > 2 || s.target < 0 || s.target > 1) return fail(h, B200FEAT_EINVAL, where(i) + "bad source or target");
+      if (s.depth < 0 || (i > 0 && s.depth < stages[i - 1].depth)) return fail(h, B200FEAT_EINVAL, where(i) + "records not in depth order");
+      const RsTable *t = nullptr;
+      if (s.table != -1) {
+        if (s.table < 0 || s.table >= (int32_t)g_rs_tables.size() || g_rs_tables[s.table].device != device)
+          return fail(h, B200FEAT_EINVAL, where(i) + "unknown table id on this device");
+        t = &g_rs_tables[s.table];
+      }
+      if (s.in_len < 1 || s.in_len > ((int64_t)1 << 40) || s.in_elem < 0 || !src[s.source] || s.in_elem > src_elems[s.source] - s.in_len)
+        return fail(h, B200FEAT_EINVAL, where(i) + "input outside its source buffer");
+      // lhotse keeps torch.ceil(torch.as_tensor(N * L / O)) outputs: the double quotient as a float32 tensor, then its ceil,
+      // at most the N * (L / O + 1) the conv produces
+      const int64_t want = t ? std::min((int64_t)ceilf((float)((double)((int64_t)t->N * s.in_len) / (double)t->O)),
+                                        (int64_t)t->N * (s.in_len / t->O + 1))
+                             : s.in_len;
+      if (s.out_len != want) return fail(h, B200FEAT_EINVAL, where(i) + "out_len is not lhotse's ceil(f32(N * L / O))");
+      if (s.target_len < 0 || (s.target == B200FEAT_RESAMPLE_TO_MID && s.target_len != s.out_len) ||
+          (s.target_len > s.out_len && s.target_len - s.out_len > s.out_len - 1))
+        return fail(h, B200FEAT_EINVAL, where(i) + "bad target_len (reflect padding longer than the stage output?)");
+      if (s.out_elem < 0 || !dst[s.target] || s.out_elem > dst_elems[s.target] - s.target_len)
+        return fail(h, B200FEAT_EINVAL, where(i) + "output outside its target buffer");
+      if (i == 0 || s.depth != stages[i - 1].depth) {
+        group_start.push_back(i);
+        group_smem.push_back(0);
+        ctas = 0;
+      }
+      RsStage &r = rs[i];
+      r.tab = t ? t->dev : nullptr;
+      r.src16 = s.source == B200FEAT_RESAMPLE_MID ? nullptr : (const int16_t *)src[s.source] + s.in_elem;
+      r.src32 = s.source == B200FEAT_RESAMPLE_MID ? mid_dev + s.in_elem : nullptr;
+      r.dst = dst[s.target] + s.out_elem;
+      r.in_len = s.in_len;
+      r.out_len = s.out_len;
+      r.target_len = s.target_len;
+      r.N = t ? t->N : 1;
+      r.O = t ? t->O : 1;
+      r.K = t ? t->K : 1;
+      r.width = t ? t->width : 0;
+      r.chunk = rs_chunk_outputs(r.N, r.O, r.K);
+      r.tab_smem = t && (int64_t)r.N * r.K <= RS_SMEM_TAB_FLOATS;
+      r.scale_in = s.scale_in;
+      r.scale_out = s.scale_out;
+      r.cta_begin = ctas;
+      ctas += rs_stage_ctas(r);
+      if (ctas > 0x7fffffff) return fail(h, B200FEAT_EINVAL, where(i) + "too many CTAs in one depth");
+      if (t) group_smem.back() = std::max(group_smem.back(), sizeof(float) * (size_t)rs_smem_floats(r));
+    }
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  RsStage *d_rs = (RsStage *)work_dev;
+  // a pageable copy: the call returns once `rs` has been staged, so the vector may go when this function returns
+  CU_TRY(h, cudaMemcpyAsync(d_rs, rs.data(), rs.size() * sizeof(RsStage), cudaMemcpyHostToDevice, st));
+  group_start.push_back(nstages);
+  for (size_t gi = 0; gi + 1 < group_start.size(); ++gi) {
+    const int32_t a = group_start[gi], b = group_start[gi + 1];
+    const RsStage &last = rs[b - 1];
+    const int64_t n = last.cta_begin + rs_stage_ctas(last);
+    if (n == 0) continue;
+    resample_stage_kernel<<<(unsigned)n, RS_THREADS, group_smem[gi], st>>>(d_rs + a, b - a);
+    CU_TRY(h, cudaGetLastError());
+  }
   return B200FEAT_OK;
 }
 

@@ -80,6 +80,13 @@ MIX_CUT_DTYPE = np.dtype([("struct_size", "<i4"), ("mode", "<i4"), ("out_elem", 
 MIX_ROLE_MIXED, MIX_ROLE_ENERGY = 0, 1
 MIX_F32, MIX_SCALED_FIRST = 0, 1
 
+# b200feat_resample_stage as a numpy record layout (the transform route's stage table is built with vector operations)
+RESAMPLE_STAGE_DTYPE = np.dtype([("struct_size", "<i4"), ("table", "<i4"), ("source", "<i4"), ("target", "<i4"), ("depth", "<i4"),
+                                 ("scale_in", "<f4"), ("scale_out", "<f4"), ("reserved", "<i4"), ("in_elem", "<i8"),
+                                 ("in_len", "<i8"), ("out_elem", "<i8"), ("out_len", "<i8"), ("target_len", "<i8")])
+RESAMPLE_SRC0, RESAMPLE_SRC1, RESAMPLE_MID = 0, 1, 2
+RESAMPLE_TO_MID, RESAMPLE_TO_OUT = 0, 1
+
 
 EXPORTS = [
     "b200feat_version", "b200feat_global_error", "b200feat_create", "b200feat_destroy",
@@ -88,6 +95,7 @@ EXPORTS = [
     "b200feat_extract_host_at", "b200feat_desc_num_frames",
     "b200feat_get_table", "b200feat_get_stats", "b200feat_set_output_affine", "b200feat_extract_host_ptrs",
     "b200feat_flac_index", "b200feat_flac_decode", "b200feat_mix_work_bytes", "b200feat_mix",
+    "b200feat_resample_table", "b200feat_resample_work_bytes", "b200feat_resample",
 ]
 
 
@@ -155,6 +163,12 @@ def load_library():
         lib.b200feat_mix_work_bytes.argtypes = [i32, i32]
         lib.b200feat_mix.restype = C.c_int
         lib.b200feat_mix.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
+        lib.b200feat_resample_table.restype = C.c_int
+        lib.b200feat_resample_table.argtypes = [vp, i32, i32, vp, i32, i32, i32, C.POINTER(i32)]
+        lib.b200feat_resample_work_bytes.restype = i64
+        lib.b200feat_resample_work_bytes.argtypes = [i32]
+        lib.b200feat_resample.restype = C.c_int
+        lib.b200feat_resample.argtypes = [vp, vp, i64, vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -238,6 +252,46 @@ def mix(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], tracks: np.n
     if rc != 0:
         msg = (lib.b200feat_last_error(handle) if handle is not None else lib.b200feat_global_error()).decode()
         raise B200FeatError(rc, msg)
+
+
+def _raise(lib, rc: int, handle) -> None:
+    msg = (lib.b200feat_last_error(handle) if handle is not None else lib.b200feat_global_error()).decode()
+    raise B200FeatError(rc, msg)
+
+
+def resample_table(orig: int, new: int, kernel: np.ndarray, width: int, device, handle=None) -> int:
+    """The id of the rate pair's table on `device` (`b200feat_resample_table`): `kernel` is the float32 [N][K] table, read
+    only the first time the pair is seen on that device."""
+    lib = load_library()
+    kernel = np.ascontiguousarray(kernel, dtype=np.float32)
+    tid = C.c_int32(-1)
+    with torch.cuda.device(torch.device(device)):
+        rc = lib.b200feat_resample_table(handle, int(orig), int(new), kernel.ctypes.data, kernel.shape[0], kernel.shape[1],
+                                         int(width), C.byref(tid))
+    if rc != 0:
+        _raise(lib, rc, handle)
+    return int(tid.value)
+
+
+def resample(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], mid: Optional[torch.Tensor], stages: np.ndarray,
+             out: torch.Tensor, handle=None) -> None:
+    """Launches `b200feat_resample` on the current stream of `out`'s device (asynchronous): the int16 device sources and the
+    float32 intermediate buffer (None = empty), the host stage table (RESAMPLE_STAGE_DTYPE, sorted by depth) and the float32
+    output.  Raises B200FeatError when the library refuses the table."""
+    lib = load_library()
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    assert stages.dtype == RESAMPLE_STAGE_DTYPE and out.dtype == torch.float32
+    work = torch.empty(max(int(lib.b200feat_resample_work_bytes(len(stages))), 1), dtype=torch.uint8, device=out.device)
+
+    def src(t):
+        return (None, 0) if t is None or t.numel() == 0 else (t.data_ptr(), t.numel())
+
+    (p0, n0), (p1, n1), (pm, nm) = src(src0), src(src1), src(mid)
+    with torch.cuda.device(out.device):
+        rc = lib.b200feat_resample(handle, p0, n0, p1, n1, pm, nm, stages.ctypes.data, len(stages), out.data_ptr(), out.numel(),
+                                   work.data_ptr(), work.numel(), stream)
+    if rc != 0:
+        _raise(lib, rc, handle)
 
 
 def _ptr(a: Optional[np.ndarray]):

@@ -53,12 +53,15 @@ class FusedOnTheFlyFeatures:
         # compressed frames go file -> pinned byte ring -> GPU and are decoded there into the same int16 buffer ("flac").
         # When the batch holds MixedCuts of such slices (CutMix noise, padding, concatenation) and every other cut is a plain
         # slice, the tracks are staged as int16 by those rings and mixed on the GPU, bit-identical to lhotse ("mix").
+        # When the batch holds speed-perturbed, volume-perturbed or resampled cuts of such files (and no MixedCut), the
+        # source slices are staged as int16 and the transforms run on the GPU, bit-identical to lhotse ("transform").
         # `pcm16_fast_path=False` turns all staged routes off.
         self.pcm16_fast_path = pcm16_fast_path and hasattr(extractor, "extract_staged_padded")
         self._ring = None
         self._flac_ring = None
         self._mix_ring = None
-        self.last_batch_route = None  # "pcm16" | "flac" | "mix" | "float" (introspection for tests / logs)
+        self._transform_ring = None
+        self.last_batch_route = None  # "pcm16" | "flac" | "mix" | "transform" | "float" (introspection for tests / logs)
         self._executor_type = executor_type
         self._executor = None
         # §8f-1: GlobalMVN (lhotse/dataset/signal_transforms.py:16-58) fused into the kernels' epilogue.  `global_mvn` is a
@@ -97,6 +100,8 @@ class FusedOnTheFlyFeatures:
             return None  # mixed sampling rates: grouped by the float route
         if any(getattr(c, "tracks", None) is not None for c in cuts):
             return self._try_mix(cuts)
+        if any(getattr(getattr(c, "recording", None), "transforms", None) for c in cuts):
+            return self._try_transform(cuts)
         reqs = []
         for c in cuts:
             r = pcm16_request_for_cut(c)
@@ -147,6 +152,27 @@ class FusedOnTheFlyFeatures:
                 return None  # the float route knows how to skip broken cuts
             raise
         return "mix", out
+
+    def _try_transform(self, cuts):
+        from .pcm_staging import TransformStagingRing, transform_requests_for_batch
+
+        reqs = transform_requests_for_batch(cuts)
+        if reqs is None:
+            return None  # a cut the transform route cannot take: the float route
+        if self._transform_ring is None:
+            self._transform_ring = TransformStagingRing()
+        try:  # a FLAC frame that does not decode raises ValueError before any feature is handed back
+            staged, lens, offs, sr = self._transform_ring.stage(reqs, executor=self._get_executor())
+            if sr != cuts[0].sampling_rate:
+                return None
+            out = self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON,
+                                                       ring=self._transform_ring,
+                                                       **({"engine": self._mvn_engine} if self._mvn_engine is not None else {}))
+        except (OSError, ValueError):
+            if self.fault_tolerant:
+                return None  # the float route knows how to skip broken cuts
+            raise
+        return "transform", out
 
     def _stage_pcm16(self, cuts, reqs):
         from .pcm_staging import PcmStagingRing

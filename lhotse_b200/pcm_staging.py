@@ -14,6 +14,9 @@ ragged buffer (no float copy on the host), cross PCIe as 2 bytes per sample and 
                                  (one "file" source, .wav, no augmentation transforms); None otherwise
   * `FlacStream`, `FlacStagingRing`, `flac_request_for_cut`, `decode_flac`: the same for 16-bit FLAC files, whose frames
                                  cross PCIe compressed and are decoded by the sm_90a kernel of csrc/flac.cuh
+  * `mix_request_for_cut`, `MixStagingRing`, `mix_cuts`: MixedCuts of such slices, mixed by csrc/mix.cuh
+  * `transform_request_for_cut`, `TransformStagingRing`, `transform_cuts`: speed / volume perturbed and resampled slices, the
+                                 transforms run by csrc/resample.cuh
 Everything here is host-side I/O; the arithmetic stays in the CUDA kernels.
 """
 from __future__ import annotations
@@ -794,3 +797,398 @@ def mix_cuts(cuts, device="cuda", executor=None,
     ring = ring or MixStagingRing()
     batch, _, _, _ = ring.stage(reqs, executor=executor)
     return mix_staged(batch, device, ring)
+
+
+# ---- Speed / Volume / Resample transforms ---------------------------------------------------------------------------
+# A MonoCut whose recording carries a chain of Speed, Volume and Resample transforms (CutSet.perturb_speed / perturb_volume /
+# resample): its source slice is staged as int16 by the two rings above, and the sm_90a kernel of csrc/resample.cuh runs the
+# chain on the device, bit for bit what cut.load_audio() returns where torch sends lhotse's resampling conv1d to oneDNN
+# (DESIGN.md §3.1i).  The samples land as float32 in the ragged layout `Engine.extract_device` takes.
+
+ONEDNN_MIN_INPUT = 20481     # ATen runs this conv1d through oneDNN only when the padded input has more than 20480 elements
+_RESAMPLE_MAX_WINDOW = 8192  # K + O of a table the kernel takes (csrc/resample.cuh RS_WIN_FLOATS)
+_RESAMPLE_MAX_TABLE = 1 << 22
+
+
+def _resample_geometry(orig: int, new: int) -> Tuple[int, int, int, int]:
+    """(N, O, width, K) of lhotse's resampler for orig -> new (lowpass filter width 6, rolloff 0.99)."""
+    g = math.gcd(orig, new)
+    O, N = orig // g, new // g
+    width = math.ceil(6 * O / (min(O, N) * 0.99))
+    return N, O, width, 2 * width + O
+
+
+def resampled_len(N: int, L: int, O: int) -> int:
+    """Samples lhotse's resampler keeps of an input of L samples: `torch.ceil(torch.as_tensor(N * L / O))`, where the Python
+    float quotient becomes a float32 tensor (torch's default dtype; the route requires it), so a small fractional part is
+    rounded away once the quotient reaches a few tens of thousands; never more than the N * (L // O + 1) outputs the conv
+    produces."""
+    return min(int(math.ceil(np.float32(N * L / O))), N * (L // O + 1))
+
+
+_KERNELS: "dict[Tuple[int, int], Tuple[np.ndarray, int]]" = {}
+_KERNELS_LOCK = threading.Lock()
+
+
+def resample_kernel(orig: int, new: int) -> Tuple[np.ndarray, int]:
+    """(float32 table [N][K], width) of lhotse's Hann-windowed sinc resampler for orig -> new.  Output phase p, tap k sits at
+    time u = (-p / N + (k - width) / O) * min(O, N) * 0.99, clamped to +-6; its weight is sinc(pi u) * cos^2(pi u / 12) *
+    min(O, N) * 0.99 / O.  The table is evaluated in float64 with the torch operations lhotse uses, in the same order (the
+    phase offsets -p / N in torch's default float dtype), and rounded once."""
+    key = (int(orig), int(new))
+    with _KERNELS_LOCK:
+        hit = _KERNELS.get(key)
+    if hit is not None:
+        return hit
+    N, O, width, _ = _resample_geometry(*key)
+    lpw, base = 6, min(O, N) * 0.99
+    u = (torch.arange(0, -N, -1) / N)[:, None] + torch.arange(-width, width + O, dtype=torch.float64)[None, :] / O
+    u *= base
+    u = u.clamp_(-lpw, lpw)
+    hann = torch.cos(u * math.pi / lpw / 2) ** 2
+    u *= math.pi
+    w = torch.where(u == 0, torch.tensor(1.0).to(u), u.sin() / u)
+    w *= hann * (base / O)
+    hit = (w.to(torch.float32).numpy().copy(), width)
+    with _KERNELS_LOCK:
+        _KERNELS[key] = hit
+    return hit
+
+
+def _fma32(a: np.ndarray, b: np.ndarray, c: np.ndarray) -> np.ndarray:
+    """float32 fma(a, b, c), rounded once, for float32 arrays: a * b is exact in float64, the float64 sum's own rounding error
+    comes from TwoSum, and a sum that sits exactly between two float32 values is rounded toward that error's side."""
+    p = a.astype(np.float64) * b.astype(np.float64)
+    c64 = c.astype(np.float64)
+    s = p + c64
+    z = s - p
+    e = (p - (s - z)) + (c64 - z)  # p + c64 == s + e exactly
+    r = s.astype(np.float32)
+    d = s - r.astype(np.float64)
+    cand = (e != 0) & (d != 0)
+    if cand.any():
+        other = np.nextafter(r, np.where(d > 0, np.float32(np.inf), np.float32(-np.inf)))
+        tie = cand & ((r.astype(np.float64) + other.astype(np.float64)) * 0.5 == s)
+        r = np.where(tie & ((e > 0) == (d > 0)), other, r)
+    return r
+
+
+def resample_reference(x: np.ndarray, orig: int, new: int) -> np.ndarray:
+    """The resampling contract of DESIGN.md §3.1i in NumPy: the zero-padded segment, one float32 FMA chain per output over
+    the K taps in tap order from +0, `resampled_len` outputs kept.  What the kernel computes, on the host."""
+    table, width = resample_kernel(orig, new)
+    N, K = table.shape
+    O = K - 2 * width
+    L = int(x.shape[0])
+    xp = np.concatenate([np.zeros(width, np.float32), np.asarray(x, np.float32), np.zeros(width + O, np.float32)])
+    at = np.arange((xp.shape[0] - K) // O + 1) * O
+    acc = np.zeros((at.shape[0], N), np.float32)
+    for t in range(K):
+        acc = _fma32(xp[at + t][:, None], table[None, :, t], acc)
+    return acc.reshape(-1)[: resampled_len(N, L, O)]
+
+
+_PROBES: "dict[Tuple[int, int], bool]" = {}
+_PROBES_LOCK = threading.Lock()
+
+
+def resample_probe(orig: int, new: int) -> bool:
+    """Whether lhotse's own resampler for orig -> new, run here by torch, equals `resample_reference` bit for bit on a
+    seeded signal long enough for oneDNN (with a silent stretch, so signed zeros are compared too) and uses the same table.
+    Run once per pair and process: on a host whose oneDNN sums in another order the route declines instead of diverging."""
+    key = (int(orig), int(new))
+    with _PROBES_LOCK:
+        ok = _PROBES.get(key)
+        if ok is not None:
+            return ok
+        from lhotse.augmentation.torchaudio import get_or_create_resampler
+
+        rs = np.random.RandomState(key[0] * 7919 + key[1])
+        q = rs.randint(-32768, 32768, ONEDNN_MIN_INPUT + 3000).astype(np.int16)
+        q[4000:6000] = 0
+        x = q.astype(np.float32) / np.float32(32768)
+        resampler = get_or_create_resampler(*key)
+        with torch.no_grad():
+            got = resampler(torch.from_numpy(x)[None]).numpy()[0]
+        want = resample_reference(x, *key)
+        ok = bool(got.dtype == np.float32 and got.shape == want.shape and np.array_equal(got.view(np.int32), want.view(np.int32))
+                  and np.array_equal(resampler.kernel[:, 0, :].numpy(), resample_kernel(*key)[0]))
+        _PROBES[key] = ok
+        return ok
+
+
+@dataclass(frozen=True)
+class TransformRequest:
+    source: object             # PcmRequest | FlacRequest: the slice of the file the chain starts from
+    ops: Tuple[tuple, ...]     # in chain order: ("volume", float32 factor) | ("resample", orig, new)
+    num_samples: int           # the cut's length: the chain's output is trimmed or reflect-padded to it
+    sampling_rate: int         # the cut's (the recording's, after the chain)
+
+
+def _samples(seconds: float, sr: int) -> int:
+    return int(math.floor(round(seconds * sr, 8) + 0.5))  # lhotse's compute_num_samples
+
+
+def transform_request_for_cut(cut) -> Optional[TransformRequest]:
+    """What `cut.load_audio()` (audio/recording.py load_audio) amounts to for a MonoCut over a single-channel 16-bit WAV or
+    FLAC file whose recording carries a non-empty chain of Speed, Volume and Resample transforms: the source slice (the
+    transforms' own reverse_timestamps applied to the cut's range, a read to the end of the file when the cut's duration is
+    within 1 ms of the recording's), the chain, and the cut's length.  None when not eligible: another kind of cut or
+    transform, a Resample lhotse would not run through its torch resampler (sox backend, no torchaudio), a resampling stage
+    whose padded input is too short for oneDNN, oneDNN off, a rate pair whose probe fails, or a length outside lhotse's
+    duration-mismatch tolerance."""
+    try:
+        from lhotse.audio.resampling_backend import get_current_resampling_backend
+        from lhotse.audio.utils import get_audio_duration_mismatch_tolerance
+        from lhotse.augmentation import torchaudio as lta
+        from lhotse.augmentation.transform import AudioTransform
+        from lhotse.cut import MonoCut
+    except ImportError:
+        return None
+    rec = getattr(cut, "recording", None)
+    if not isinstance(cut, MonoCut) or getattr(cut, "tracks", None) is not None or rec is None or not rec.transforms:
+        return None
+    if getattr(rec, "has_video", False) or not (torch.backends.mkldnn.is_available() and torch.backends.mkldnn.enabled):
+        return None
+    if torch.get_default_dtype() != torch.float32:
+        return None  # lhotse's table phases and output lengths are evaluated in the default dtype
+    tfs = [t if isinstance(t, AudioTransform) else AudioTransform.from_dict(t) for t in rec.transforms]
+    if any(type(t) not in (lta.Speed, lta.Volume, lta.Resample) for t in tfs):
+        return None
+    sources = rec.sources or []
+    if len(sources) != 1 or sources[0].type != "file" or list(sources[0].channels) != [cut.channel]:
+        return None
+    path = str(sources[0].source)
+    try:
+        if path.lower().endswith(".wav"):
+            h, make = WavPcm16.open_cached(path), PcmRequest
+        elif path.lower().endswith(".flac"):
+            h, make = FlacStream.open_cached(path), FlacRequest
+        else:
+            return None
+    except (NotPcm16Wav, NotFlac16, OSError):
+        return None
+    if h.channels != 1:
+        return None
+    sr = rec.sampling_rate
+    offset, duration = cut.start, cut.duration
+    if math.isclose(duration, rec.duration, abs_tol=1e-3):
+        duration = None  # load_audio reads to the end of the file
+    for t in reversed(tfs):
+        offset, duration = t.reverse_timestamps(offset=offset, duration=duration, sampling_rate=sr)
+    first = _samples(offset, h.sampling_rate)
+    n = h.num_samples - first if duration is None else _samples(duration, h.sampling_rate)
+    if first < 0 or n <= 0 or first + n > h.num_samples:
+        return None
+    ops, L = [], n
+    for t in tfs:
+        if isinstance(t, lta.Volume):
+            if type(t.factor) not in (int, float) or not math.isfinite(np.float32(t.factor)):
+                return None  # a NumPy scalar factor would promote the samples to float64
+            ops.append(("volume", float(np.float32(t.factor))))
+            continue
+        if isinstance(t, lta.Speed):
+            a, b = round(sr * t.factor), sr
+        else:
+            if get_current_resampling_backend() != "default" or not lta.is_torchaudio_available():
+                return None  # sox, or scipy's resample_poly in float64
+            a, b = t.source_sampling_rate, t.target_sampling_rate
+        if a == b:
+            continue  # lhotse returns the samples unchanged
+        N, O, width, K = _resample_geometry(a, b)
+        if L + 2 * width + O < ONEDNN_MIN_INPUT or K + O > _RESAMPLE_MAX_WINDOW or N * K > _RESAMPLE_MAX_TABLE:
+            return None
+        if not resample_probe(a, b):
+            return None
+        ops.append(("resample", int(a), int(b)))
+        L = resampled_len(N, L, O)
+    target = _samples(cut.duration, sr)
+    diff = target - L
+    if abs(diff) > int(math.ceil(get_audio_duration_mismatch_tolerance() * sr)) or diff > L - 1:
+        return None
+    return TransformRequest(source=make(path=h.path, first_sample=first, num_samples=n), ops=tuple(ops), num_samples=target,
+                            sampling_rate=int(sr))
+
+
+def _has_transforms(cut) -> bool:
+    return bool(getattr(getattr(cut, "recording", None), "transforms", None))
+
+
+def transform_requests_for_batch(cuts) -> Optional[List[TransformRequest]]:
+    """The "transform" route's requests for a batch: no MixedCut, every cut a plain 16-bit WAV / FLAC slice or an eligible
+    transformed MonoCut, and at least one of the latter (batches of plain slices keep their routes).  None otherwise."""
+    if any(getattr(c, "tracks", None) is not None for c in cuts) or not any(_has_transforms(c) for c in cuts):
+        return None
+    reqs = [_transform_or_plain_request(c) for c in cuts]
+    return None if any(r is None for r in reqs) else reqs
+
+
+def _transform_or_plain_request(cut) -> Optional[TransformRequest]:
+    """transform_request_for_cut, or a plain 16-bit WAV / FLAC slice as an empty chain (a copy of x = q / 32768)."""
+    if _has_transforms(cut):
+        r = transform_request_for_cut(cut)
+    else:
+        src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
+        r = (TransformRequest(source=src, ops=(), num_samples=int(src.num_samples), sampling_rate=int(cut.sampling_rate))
+             if src is not None else None)
+    return r if r is not None and r.num_samples > 0 else None
+
+
+def _chain_stages(ops) -> List[Tuple[float, Optional[Tuple[int, int]], float]]:
+    """The chain as kernel stages (load scale, rate pair or None, store scale): each Volume goes into the load scale of a stage
+    that has not resampled yet, else into the store scale of a stage that has none yet, else it opens a new stage."""
+    stages = [[1.0, None, 1.0, False]]  # load scale, pair, store scale, store scale taken
+    for op in ops:
+        s = stages[-1]
+        if op[0] == "volume":
+            if s[1] is None and s[0] == 1.0 and not s[3]:
+                s[0] = op[1]
+            elif not s[3]:
+                s[2], s[3] = op[1], True
+            else:
+                stages.append([op[1], None, 1.0, False])
+        elif s[1] is None and not s[3]:
+            s[1] = (op[1], op[2])
+        else:
+            stages.append([1.0, (op[1], op[2]), 1.0, False])
+    return [(a, p, b) for a, p, b, _ in stages]
+
+
+@dataclass
+class TransformBatch:
+    """One staged transform batch: the WAV slices in the ring's pinned int16 buffer, the FLAC slices as a staged
+    FlacBatch, and the b200feat_resample stage table (a pinned numpy view, sorted by depth) with the rate pair of each stage."""
+    pcm: Optional[torch.Tensor]
+    flac: Optional[FlacBatch]
+    stages: np.ndarray        # engine.RESAMPLE_STAGE_DTYPE; `table` is filled per device by transform_staged
+    pair: np.ndarray          # index into `pairs` of every stage, -1: no resampling
+    pairs: List[Tuple[int, int]]
+    mid_elems: int
+    lens: List[int]
+    offsets: List[int]
+    out_elems: int
+
+
+class TransformStagingRing(_PinnedRing):
+    """A pinned int16 buffer for the WAV slices, a FlacStagingRing and pinned table bytes for one transform batch;
+    `stage(requests)` returns (TransformBatch, lengths, offsets, the cuts' sampling rate), the rate None when the cuts have
+    several."""
+
+    ALIGN = 4
+
+    def __init__(self, pin_memory: Optional[bool] = None):
+        super().__init__(pin_memory)
+        self._pcm = torch.empty(1 << 20, dtype=torch.int16, pin_memory=self._pin)
+        self.flac = FlacStagingRing(initial_bytes=1 << 16, pin_memory=self._pin)
+        self._tables = torch.empty(1 << 16, dtype=torch.uint8, pin_memory=self._pin)
+
+    def mark_in_flight(self, device=None) -> None:
+        super().mark_in_flight(device)
+        self.flac.mark_in_flight(device)
+
+    def _stage_wav(self, requests: Sequence[PcmRequest], executor) -> Tuple[torch.Tensor, List[int]]:
+        """The WAV slices back to back on 4-sample boundaries, as PcmStagingRing lays them out, but from files of any rate
+        (a Resample chain starts at its file's own rate): (pinned int16 view, offsets)."""
+        lens = [int(r.num_samples) for r in requests]
+        offs, total = _aligned_offsets(lens, self.ALIGN)
+        self._pcm = self._grown(self._pcm, total)
+        view = self._pcm.numpy()
+        _zero_gaps(view, lens, offs)
+
+        def one(i):
+            r = requests[i]
+            WavPcm16.open_cached(r.path).read_into(view[offs[i]: offs[i] + lens[i]], r.first_sample, r.channel)
+
+        _for_each(len(requests), one, executor)
+        return self._pcm[:total], offs
+
+    def stage(self, requests: Sequence[TransformRequest], executor=None) -> Tuple[TransformBatch, List[int], List[int], Optional[int]]:
+        from .engine import RESAMPLE_MID, RESAMPLE_STAGE_DTYPE, RESAMPLE_TO_MID, RESAMPLE_TO_OUT
+
+        self._wait_idle()
+        kind = np.asarray([0 if isinstance(r.source, PcmRequest) else 1 for r in requests], dtype=np.int32)
+        src_elem = np.zeros(len(requests), dtype=np.int64)
+        pcm_buf, flac_batch = None, None
+        if (kind == 0).any():
+            pcm_buf, offs0 = self._stage_wav([r.source for r, k in zip(requests, kind) if k == 0], executor)
+            src_elem[kind == 0] = offs0
+        if (kind == 1).any():
+            flac_batch, _, offs1, _ = self.flac.stage([r.source for r, k in zip(requests, kind) if k == 1], executor=executor)
+            src_elem[kind == 1] = offs1
+        srs = {r.sampling_rate for r in requests}
+        lens = [int(r.num_samples) for r in requests]
+        offs, out_elems = _aligned_offsets(lens, self.ALIGN)
+        pairs, pair_ix = [], {}
+        rows = []  # (depth, cut, table pair, source, in_elem, in_len, target, out_elem, out_len, target_len, scale_in, scale_out)
+        mid = 0
+        for i, r in enumerate(requests):
+            chain = _chain_stages(r.ops)
+            source, in_elem, L = int(kind[i]), int(src_elem[i]), int(r.source.num_samples)
+            for d, (s_in, pair, s_out) in enumerate(chain):
+                if pair is None:
+                    pi, n_out = -1, L
+                else:
+                    pi = pair_ix.setdefault(pair, len(pairs))
+                    if pi == len(pairs):
+                        pairs.append(pair)
+                    N, O, _, _ = _resample_geometry(*pair)
+                    n_out = resampled_len(N, L, O)
+                last = d == len(chain) - 1
+                out_elem = offs[i] if last else mid
+                rows.append((d, i, pi, source, in_elem, L, RESAMPLE_TO_OUT if last else RESAMPLE_TO_MID, out_elem, n_out,
+                             lens[i] if last else n_out, s_in, s_out))
+                if not last:
+                    mid += n_out
+                source, in_elem, L = RESAMPLE_MID, out_elem, n_out
+        rows.sort(key=lambda row: (row[0], row[1]))
+        nb = len(rows) * RESAMPLE_STAGE_DTYPE.itemsize
+        self._tables = self._grown(self._tables, max(nb, 1))
+        st = self._tables.numpy()[:nb].view(RESAMPLE_STAGE_DTYPE)
+        cols = list(zip(*rows)) if rows else [()] * 12
+        st["struct_size"] = RESAMPLE_STAGE_DTYPE.itemsize
+        st["table"] = -1
+        st["depth"], st["source"], st["in_elem"], st["in_len"] = cols[0], cols[3], cols[4], cols[5]
+        st["target"], st["out_elem"], st["out_len"], st["target_len"] = cols[6], cols[7], cols[8], cols[9]
+        st["scale_in"], st["scale_out"] = cols[10], cols[11]
+        st["reserved"] = 0
+        batch = TransformBatch(pcm=pcm_buf, flac=flac_batch, stages=st, pair=np.asarray(cols[2], dtype=np.int64), pairs=pairs,
+                               mid_elems=mid, lens=lens, offsets=offs, out_elems=out_elems)
+        return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
+
+
+def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] = None,
+                     handle=None) -> Tuple[torch.Tensor, List[int], List[int]]:
+    """The device half of the "transform" route on the current stream: the rate pairs' tables (built and uploaded once per
+    device), H2D of the WAV slices, the FLAC decode (if any), the resampling stages; then `ring`'s copies are marked in flight.
+    Returns (float32 samples on `device`, lengths, offsets)."""
+    from .engine import resample, resample_table
+
+    device = torch.device(device)
+    with torch.cuda.device(device):
+        ids = np.asarray([resample_table(a, b, *resample_kernel(a, b), device, handle) for a, b in batch.pairs] + [-1],
+                         dtype=np.int32)
+        batch.stages["table"] = ids[batch.pair]  # pair -1 picks the trailing -1
+        src0 = batch.pcm.to(device, non_blocking=True) if batch.pcm is not None else None
+        src1 = decode_staged(batch.flac, device)[0] if batch.flac is not None else None
+        mid = torch.empty(batch.mid_elems, dtype=torch.float32, device=device) if batch.mid_elems else None
+        out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
+        resample(src0, src1, mid, batch.stages, out, handle)
+        if ring is not None:
+            ring.mark_in_flight(device)
+    return out, batch.lens, batch.offsets
+
+
+def transform_cuts(cuts, device="cuda", executor=None,
+                   ring: Optional[TransformStagingRing] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
+    """Loads speed-perturbed, volume-perturbed and resampled cuts (and plain 16-bit WAV / FLAC slices) with the transforms run
+    on the GPU: (float32 device tensor holding every cut's samples at its offset, on 4-sample boundaries, lengths, offsets),
+    each cut bit-identical to float32(cut.load_audio()).  Raises ValueError naming the first cut the route cannot take."""
+    reqs = []
+    for c in cuts:
+        r = _transform_or_plain_request(c)
+        if r is None:
+            raise ValueError(f"cut {getattr(c, 'id', c)!r} cannot be loaded on the GPU (see transform_request_for_cut)")
+        reqs.append(r)
+    ring = ring or TransformStagingRing()
+    batch, _, _, _ = ring.stage(reqs, executor=executor)
+    return transform_staged(batch, device, ring)

@@ -247,8 +247,8 @@ def compute_and_store_features_fused(
     from lhotse.qa import validate_features
     from lhotse.utils import fastcopy
 
-    from .pcm_staging import (FlacStagingRing, MixStagingRing, PcmStagingRing, flac_request_for_cut, mix_requests_for_batch,
-                              pcm16_request_for_cut)
+    from .pcm_staging import (FlacStagingRing, MixStagingRing, PcmStagingRing, TransformStagingRing, flac_request_for_cut,
+                              mix_requests_for_batch, pcm16_request_for_cut, transform_requests_for_batch)
 
     register_with_lhotse()
     frame_shift = extractor.frame_shift
@@ -296,7 +296,8 @@ def compute_and_store_features_fused(
     rings = queue.Queue()
     flac_rings = queue.Queue()  # the same hand-back protocol for batches of 16-bit FLAC slices (decoded on the GPU)
     mix_rings = queue.Queue()  # ... and for batches with MixedCuts of such slices (mixed on the GPU)
-    free_rings = {"pcm": rings, "flac": flac_rings, "mix": mix_rings}
+    transform_rings = queue.Queue()  # ... and for batches with speed / volume / resample transforms (run on the GPU)
+    free_rings = {"pcm": rings, "flac": flac_rings, "mix": mix_rings, "transform": transform_rings}
     stop = threading.Event()
     cuda_index = None  # the GPU this call works on, resolved in the calling thread ("cuda" without an index = its current device)
     try:
@@ -329,6 +330,9 @@ def compute_and_store_features_fused(
                 if not all(r is not None for r in reqs):
                     kind, free = "mix", mix_rings
                     reqs = mix_requests_for_batch(batch_cuts) or [None]
+                if not all(r is not None for r in reqs):
+                    kind, free = "transform", transform_rings
+                    reqs = transform_requests_for_batch(batch_cuts) or [None]
                 if all(r is not None for r in reqs):
                     ring = free.get()  # handed back by stage 2 once the batch's host-to-device copy has completed
                     staged, lens, offs, fsr = ring.stage(reqs, executor=pool)
@@ -374,6 +378,7 @@ def compute_and_store_features_fused(
                 rings.put(PcmStagingRing())
                 flac_rings.put(FlacStagingRing(initial_bytes=1 << 16))
                 mix_rings.put(MixStagingRing())
+                transform_rings.put(TransformStagingRing())
         if not pipelined:  # stage 1 and 2 in the calling thread, stage 3 one batch behind in a saver thread
             with ThreadPoolExecutor(max_workers=1) as saver:
                 futures = [saver.submit(_store, *_extract(item)) for item in _staged_batches()]
@@ -434,6 +439,8 @@ def compute_and_store_features_fused(
                         flac_rings.put(FlacStagingRing(initial_bytes=16, pin_memory=False))
                     if use_ring and mix_rings.empty():
                         mix_rings.put(MixStagingRing(pin_memory=False))
+                    if use_ring and transform_rings.empty():
+                        transform_rings.put(TransformStagingRing(pin_memory=False))
                 t_read.join()
     if pool is not None:
         pool.shutdown()
