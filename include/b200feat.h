@@ -304,6 +304,7 @@ int b200feat_flac_decode(const uint8_t *bytes_dev, const b200feat_flac_job *jobs
  * for bit (DESIGN.md §3.1h).  The tracks are samples of two int16 device buffers (e.g. a PCM16 batch and a FLAC decode);
  * every cut's mix is written as float32 into a ragged output buffer that b200feat_extract takes as B200FEAT_F32.
  */
+#define B200FEAT_MIX_SRC_F32 2      /* b200feat_mix_track.source: the float32 track buffer of b200feat_mix_ex (read as is) */
 #define B200FEAT_MIX_ROLE_MIXED 0   /* the track is part of the mix (the cut's first such track is the mixer's base) */
 #define B200FEAT_MIX_ROLE_ENERGY 1  /* a muted SNR reference: its energy sets the gains, its samples are not mixed */
 #define B200FEAT_MIX_F32 0          /* cut mode: a float32 mix */
@@ -312,7 +313,7 @@ int b200feat_flac_decode(const uint8_t *bytes_dev, const b200feat_flac_job *jobs
 
 typedef struct b200feat_mix_track {
   int32_t struct_size;   /* sizeof(b200feat_mix_track) — ABI guard, in every record */
-  int32_t source;        /* 0: src0, 1: src1, -1: padding (zeros) */
+  int32_t source;        /* 0: src0, 1: src1, -1: padding (zeros), B200FEAT_MIX_SRC_F32: src2 (b200feat_mix_ex only) */
   int64_t src_elem;      /* first sample of the track in its source buffer */
   int64_t num_samples;   /* track length */
   int64_t mix_offset;    /* first sample of the track in the mix */
@@ -343,6 +344,14 @@ int64_t b200feat_mix_work_bytes(int32_t ntracks, int32_t ncuts);
 int b200feat_mix(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
                  const b200feat_mix_track *tracks, int32_t ntracks, const b200feat_mix_cut *cuts, int32_t ncuts,
                  float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
+
+/* b200feat_mix with a third, float32 source: tracks whose `source` is B200FEAT_MIX_SRC_F32 read `src2_dev` (for example
+ * perturbed tracks that b200feat_resample wrote), their samples taken as they are instead of q / 32768.  The same checks,
+ * plus: such a track lies inside src2 and src2 is present.  b200feat_mix is this call with no src2. */
+int b200feat_mix_ex(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
+                    const float *src2_dev, int64_t src2_elems, const b200feat_mix_track *tracks, int32_t ntracks,
+                    const b200feat_mix_cut *cuts, int32_t ncuts, float *out_dev, int64_t out_elems, void *work_dev,
+                    int64_t work_bytes, void *stream);
 
 /*
  * Resampling and volume scaling of mono audio on the GPU: lhotse's Speed, Resample and Volume transforms as its CPU route

@@ -876,23 +876,34 @@ int64_t b200feat_mix_work_bytes(int32_t ntracks, int32_t ncuts) {
 int b200feat_mix(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
                  const b200feat_mix_track *tracks, int32_t ntracks, const b200feat_mix_cut *cuts, int32_t ncuts,
                  float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream) {
+  return b200feat_mix_ex(h, src0_dev, src0_elems, src1_dev, src1_elems, nullptr, 0, tracks, ntracks, cuts, ncuts, out_dev,
+                         out_elems, work_dev, work_bytes, stream);
+}
+
+int b200feat_mix_ex(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
+                    const float *src2_dev, int64_t src2_elems, const b200feat_mix_track *tracks, int32_t ntracks,
+                    const b200feat_mix_cut *cuts, int32_t ncuts, float *out_dev, int64_t out_elems, void *work_dev,
+                    int64_t work_bytes, void *stream) {
   if (ntracks < 0 || ncuts < 0 || (ncuts > 0 && (!tracks || !cuts || !out_dev || !work_dev)) || out_elems < 0 || src0_elems < 0 ||
-      src1_elems < 0)
+      src1_elems < 0 || src2_elems < 0)
     return fail(h, B200FEAT_EINVAL, "mix: bad arguments");
   if (ncuts == 0) return B200FEAT_OK;
   if (ncuts > 65535) return fail(h, B200FEAT_EINVAL, "mix: more than 65535 cuts in one call");
   if (work_bytes < b200feat_mix_work_bytes(ntracks, ncuts)) return fail(h, B200FEAT_EINVAL, "mix: work buffer too small");
-  const int16_t *src[2] = {src0_dev, src1_dev};
-  const int64_t src_elems[2] = {src0_elems, src1_elems};
+  const void *src[3] = {src0_dev, src1_dev, src2_dev};
+  const int64_t src_elems[3] = {src0_elems, src1_elems, src2_elems};
   auto where = [](const char *what, int64_t i) { return std::string("mix: ") + what + " " + std::to_string(i) + ": "; };
   for (int32_t t = 0; t < ntracks; ++t) {
     const b200feat_mix_track &tr = tracks[t];
     if (tr.struct_size != (int32_t)sizeof(b200feat_mix_track))
       return fail(h, B200FEAT_EINVAL, where("track", t) + "b200feat_mix_track size mismatch (ABI)");
-    if (tr.source < -1 || tr.source > 1) return fail(h, B200FEAT_EINVAL, where("track", t) + "source must be 0, 1 or -1 (padding)");
+    if (tr.source < -1 || tr.source > B200FEAT_MIX_SRC_F32)
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "source must be 0, 1, 2 (float32) or -1 (padding)");
+    if (tr.source == B200FEAT_MIX_SRC_F32 && !src2_dev)
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "a float32 track without the float32 source (src2)");
     if (tr.num_samples < 0 || tr.num_samples > ((int64_t)1 << 40) || tr.mix_offset < 0 || tr.mix_offset > ((int64_t)1 << 40))
       return fail(h, B200FEAT_EINVAL, where("track", t) + "bad length or mix offset");
-    if (tr.source >= 0 && (!src[tr.source] || tr.src_elem < 0 || tr.src_elem + tr.num_samples > src_elems[tr.source]))
+    if (tr.source >= 0 && (!src[tr.source] || tr.src_elem < 0 || tr.src_elem > src_elems[tr.source] - tr.num_samples))
       return fail(h, B200FEAT_EINVAL, where("track", t) + "samples outside its source buffer");
     if (tr.role != B200FEAT_MIX_ROLE_MIXED && tr.role != B200FEAT_MIX_ROLE_ENERGY)
       return fail(h, B200FEAT_EINVAL, where("track", t) + "bad role");
@@ -933,12 +944,13 @@ int b200feat_mix(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems
   const cudaStream_t st = (cudaStream_t)stream;
   if (ntracks) CU_TRY(h, cudaMemcpyAsync(d_tracks, tracks, (size_t)ntracks * sizeof(b200feat_mix_track), cudaMemcpyHostToDevice, st));
   CU_TRY(h, cudaMemcpyAsync(d_cuts, cuts, (size_t)ncuts * sizeof(b200feat_mix_cut), cudaMemcpyHostToDevice, st));
-  mix_energy_kernel<<<ncuts, MIX_THREADS, 0, st>>>(src0_dev, src1_dev, d_tracks, d_cuts, energy, gain32, scale64);
+  mix_energy_kernel<<<ncuts, MIX_THREADS, 0, st>>>(src0_dev, src1_dev, src2_dev, d_tracks, d_cuts, energy, gain32, scale64);
   CU_TRY(h, cudaGetLastError());
   int64_t longest = 1;
   for (int32_t c = 0; c < ncuts; ++c) longest = std::max(longest, cuts[c].target_len);
   const int64_t gx = std::min<int64_t>((longest + 4 * MIX_MIX_THREADS - 1) / (4 * MIX_MIX_THREADS), 1024);
-  mix_kernel<<<dim3((unsigned)gx, (unsigned)ncuts), MIX_MIX_THREADS, 0, st>>>(src0_dev, src1_dev, d_tracks, d_cuts, gain32, scale64, out_dev);
+  mix_kernel<<<dim3((unsigned)gx, (unsigned)ncuts), MIX_MIX_THREADS, 0, st>>>(src0_dev, src1_dev, src2_dev, d_tracks, d_cuts, gain32, scale64,
+                                                                              out_dev);
   CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }

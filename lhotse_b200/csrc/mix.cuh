@@ -1,7 +1,9 @@
-// Audio-domain mixing of mono int16 tracks (lhotse MixedCut.load_audio) on the GPU, bit-identical to lhotse under NumPy >= 2.
+// Audio-domain mixing of mono tracks (lhotse MixedCut.load_audio) on the GPU, bit-identical to lhotse under NumPy >= 2.  A
+// track is int16 (x = q / 32768, sources 0 and 1) or float32 (x as it is, source 2: a perturbed track the resample kernel
+// wrote into a track buffer).
 //
 // The arithmetic contract is DESIGN.md §3.1h.  In short, per cut:
-//   energy   E = f32(S / n), S the float32 pairwise sum of f32(x)^2 in NumPy's order (x = q / 32768): n < 8 a sequential sum,
+//   energy   E = f32(S / n), S the float32 pairwise sum of f32(x)^2 in NumPy's order: n < 8 a sequential sum,
 //            n <= 128 eight strided accumulators combined ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)) then the tail, otherwise a split
 //            at n2 = n/2 - (n/2 mod 8) and the two halves recursively.  The tree depends on n only.
 //   gains    g = sqrt(E_ref * factor / E_track) in double (factor = 10 ** (-snr / 10), evaluated by the host); a further
@@ -53,10 +55,12 @@ MIX_HD double mix_ddiv_h(double a, double b) { volatile double r = a / b; return
 #define MIX_TOP_DEPTH 5    // one warp: lane l evaluates the subtree at depth 5 whose index is l
 #define MIX_STACK 40       // the pairwise tree of n <= 2^40 samples (b200feat_mix checks) is at most 35 deep
 
-// x = q / 32768 exactly as B200FEAT_I16 widens a sample
+// x = q / 32768 exactly as B200FEAT_I16 widens a sample; a float32 track sample (B200FEAT_MIX_SRC_F32) is x itself
 MIX_HD float mix_widen(int16_t q) { return (float)q * (1.0f / 32768.0f); }
+MIX_HD float mix_widen(float x) { return x; }
 
-MIX_HD float mix_sq(int16_t q) {
+template <typename T>
+MIX_HD float mix_sq(T q) {
   const float x = mix_widen(q);
   return MIX_FMUL(x, x);
 }
@@ -68,7 +72,8 @@ MIX_HD int64_t mix_split(int64_t n) {
 }
 
 // NumPy's pairwise_sum leaf (n <= 128) over the squares of q[0, n)
-MIX_HD float mix_leaf(const int16_t *q, int64_t n) {
+template <typename T>
+MIX_HD float mix_leaf(const T *q, int64_t n) {
   if (n < 8) {
     float r = 0.0f;
     for (int64_t i = 0; i < n; ++i) r = MIX_FADD(r, mix_sq(q[i]));
@@ -86,7 +91,8 @@ MIX_HD float mix_leaf(const int16_t *q, int64_t n) {
 
 // the pairwise sum of the squares of q[0, n), in NumPy's order, without recursion: a post-order walk with an explicit stack
 // of the open nodes' lengths and left-half sums; bit k of `right` says the walk is in the right half of open node k
-MIX_HD float mix_pairwise(const int16_t *q, int64_t n) {
+template <typename T>
+MIX_HD float mix_pairwise(const T *q, int64_t n) {
   int64_t len[MIX_STACK];
   float left[MIX_STACK];
   uint64_t right = 0;
@@ -148,7 +154,8 @@ MIX_HD void mix_combine(float *v, bool *present, float other, bool other_present
 MIX_HD double mix_energy_of_sum(float s, int64_t n) { return n > 0 ? (double)MIX_FDIV(s, (float)n) : 0.0; }
 
 // The whole energy on one thread in the same tree as the warp (the host harness; the kernel splits it over 32 lanes)
-MIX_HD double mix_energy(const int16_t *q, int64_t n) {
+template <typename T>
+MIX_HD double mix_energy(const T *q, int64_t n) {
   float v[1 << MIX_TOP_DEPTH];
   bool p[1 << MIX_TOP_DEPTH];
   for (int l = 0; l < (1 << MIX_TOP_DEPTH); ++l) {
@@ -178,7 +185,8 @@ MIX_HD double mix_gain(double e_ref, double factor, double e_track) {
 }
 
 // A further track's sample in a float32 mix: f32(f32(g) * x); gain32 = 1 for an unscaled track (1 * x = x exactly)
-MIX_HD float mix_added_sample(float gain32, int16_t q) { return MIX_FMUL(gain32, mix_widen(q)); }
+template <typename T>
+MIX_HD float mix_added_sample(float gain32, T q) { return MIX_FMUL(gain32, mix_widen(q)); }
 
 // The mix position read for output sample p of a mix of `mix_len` samples: p itself, or np.pad(mode="reflect") past the end
 MIX_HD int64_t mix_source_pos(int64_t p, int64_t mix_len) { return p < mix_len ? p : 2 * (mix_len - 1) - p; }
@@ -195,10 +203,18 @@ MIX_HD float mix_track_gain(const b200feat_mix_cut &cut, const b200feat_mix_trac
   return g > 0.0 ? MIX_D2F(g) : 1.0f;
 }
 
+// Sample x of track `tr` at mix position pos (inside the track): +0 for padding, q / 32768 of an int16 source, the float32
+// sample of the track buffer as it is
+MIX_HD float mix_track_x(const int16_t *src0, const int16_t *src1, const float *src2, const b200feat_mix_track &tr, int64_t pos) {
+  const int64_t i = tr.src_elem + pos - tr.mix_offset;
+  if (tr.source == B200FEAT_MIX_SRC_F32) return mix_widen(src2[i]);
+  return mix_widen(tr.source < 0 ? (int16_t)0 : (tr.source == 0 ? src0 : src1)[i]);
+}
+
 // Output sample p of a cut: the tracks that cover its mix position added in track order to a zero of the mix's dtype,
 // returned as float32 (a float64 mix is rounded once here).
-MIX_HD float mix_sample(const int16_t *src0, const int16_t *src1, const b200feat_mix_track *tracks, const b200feat_mix_cut &cut,
-                        const float *gain32, double scale, int64_t p) {
+MIX_HD float mix_sample(const int16_t *src0, const int16_t *src1, const float *src2, const b200feat_mix_track *tracks,
+                        const b200feat_mix_cut &cut, const float *gain32, double scale, int64_t p) {
   const int64_t pos = mix_source_pos(p, cut.mix_len);
   const int64_t t0 = cut.first_track, t1 = cut.first_track + cut.num_tracks;
   if (scale > 0.0) {  // the first track went through _scale_audio_for_snr: a float64 mix
@@ -206,8 +222,8 @@ MIX_HD float mix_sample(const int16_t *src0, const int16_t *src1, const b200feat
     for (int64_t t = t0; t < t1; ++t) {
       const b200feat_mix_track &tr = tracks[t];
       if (tr.role != B200FEAT_MIX_ROLE_MIXED || pos < tr.mix_offset || pos >= tr.mix_offset + tr.num_samples) continue;
-      const int16_t q = tr.source < 0 ? (int16_t)0 : (tr.source == 0 ? src0 : src1)[tr.src_elem + pos - tr.mix_offset];
-      m = MIX_DADD(m, t == t0 ? MIX_DMUL((double)mix_widen(q), scale) : (double)mix_added_sample(gain32[t], q));
+      const float x = mix_track_x(src0, src1, src2, tr, pos);
+      m = MIX_DADD(m, t == t0 ? MIX_DMUL((double)x, scale) : (double)mix_added_sample(gain32[t], x));
     }
     return MIX_D2F(m);
   }
@@ -215,8 +231,7 @@ MIX_HD float mix_sample(const int16_t *src0, const int16_t *src1, const b200feat
   for (int64_t t = t0; t < t1; ++t) {
     const b200feat_mix_track &tr = tracks[t];
     if (tr.role != B200FEAT_MIX_ROLE_MIXED || pos < tr.mix_offset || pos >= tr.mix_offset + tr.num_samples) continue;
-    const int16_t q = tr.source < 0 ? (int16_t)0 : (tr.source == 0 ? src0 : src1)[tr.src_elem + pos - tr.mix_offset];
-    m = MIX_FADD(m, mix_added_sample(gain32[t], q));
+    m = MIX_FADD(m, mix_added_sample(gain32[t], mix_track_x(src0, src1, src2, tr, pos)));
   }
   return m;
 }
@@ -230,8 +245,24 @@ MIX_HD bool mix_needs_energy(const b200feat_mix_cut &cut, const b200feat_mix_tra
 #define MIX_THREADS 128
 #define MIX_MIX_THREADS 256
 
+// The warp's energy sum of one track: lane `lane` walks its subtree at depth MIX_TOP_DEPTH, the shuffles combine the subtrees
+// in NumPy's order; every lane returns the whole sum.
+template <typename T>
+__device__ __forceinline__ float mix_warp_sum(const T *__restrict__ q, int64_t n, int lane) {
+  int64_t s = 0, m = 0;
+  bool present = mix_top_node(n, lane, &s, &m);
+  float v = present ? mix_pairwise(q + s, m) : 0.0f;
+  for (int b = 0; b < MIX_TOP_DEPTH; ++b) {  // siblings differ in bit b of the lane: the tree above depth 5, bottom up
+    const float other = __shfl_xor_sync(0xffffffffu, v, 1 << b);
+    const bool other_present = __shfl_xor_sync(0xffffffffu, (int)present, 1 << b) != 0;
+    mix_combine(&v, &present, other, other_present);
+  }
+  return v;
+}
+
 // One block per cut, one warp per track: the energies the cut needs (its reference, every track with an SNR), then the gains.
 __global__ void __launch_bounds__(MIX_THREADS) mix_energy_kernel(const int16_t *__restrict__ src0, const int16_t *__restrict__ src1,
+                                                                  const float *__restrict__ src2,
                                                                   const b200feat_mix_track *__restrict__ tracks,
                                                                   const b200feat_mix_cut *__restrict__ cuts, double *__restrict__ energy,
                                                                   float *__restrict__ gain32, double *__restrict__ scale64) {
@@ -244,15 +275,9 @@ __global__ void __launch_bounds__(MIX_THREADS) mix_energy_kernel(const int16_t *
       if (lane == 0) energy[t] = 0.0;
       continue;
     }
-    const int16_t *q = (tr.source == 0 ? src0 : src1) + tr.src_elem;
-    int64_t s = 0, m = 0;
-    bool present = mix_top_node(tr.num_samples, lane, &s, &m);
-    float v = present ? mix_pairwise(q + s, m) : 0.0f;
-    for (int b = 0; b < MIX_TOP_DEPTH; ++b) {  // siblings differ in bit b of the lane: the tree above depth 5, bottom up
-      const float other = __shfl_xor_sync(0xffffffffu, v, 1 << b);
-      const bool other_present = __shfl_xor_sync(0xffffffffu, (int)present, 1 << b) != 0;
-      mix_combine(&v, &present, other, other_present);
-    }
+    const float v = tr.source == B200FEAT_MIX_SRC_F32  // warp-uniform: the source is chosen once per track
+                        ? mix_warp_sum(src2 + tr.src_elem, tr.num_samples, lane)
+                        : mix_warp_sum((tr.source == 0 ? src0 : src1) + tr.src_elem, tr.num_samples, lane);
     if (lane == 0) energy[t] = mix_energy_of_sum(v, tr.num_samples);
   }
   __syncthreads();
@@ -267,6 +292,7 @@ __global__ void __launch_bounds__(MIX_THREADS) mix_energy_kernel(const int16_t *
 
 // grid (x, cuts), a grid-stride loop over each cut's output samples
 __global__ void __launch_bounds__(MIX_MIX_THREADS) mix_kernel(const int16_t *__restrict__ src0, const int16_t *__restrict__ src1,
+                                                              const float *__restrict__ src2,
                                                               const b200feat_mix_track *__restrict__ tracks,
                                                               const b200feat_mix_cut *__restrict__ cuts,
                                                               const float *__restrict__ gain32, const double *__restrict__ scale64,
@@ -274,6 +300,6 @@ __global__ void __launch_bounds__(MIX_MIX_THREADS) mix_kernel(const int16_t *__r
   const b200feat_mix_cut cut = cuts[blockIdx.y];
   const double scale = scale64[blockIdx.y];
   for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < cut.target_len; p += (int64_t)gridDim.x * blockDim.x)
-    out[cut.out_elem + p] = mix_sample(src0, src1, tracks, cut, gain32, scale, p);
+    out[cut.out_elem + p] = mix_sample(src0, src1, src2, tracks, cut, gain32, scale, p);
 }
 #endif

@@ -79,6 +79,7 @@ MIX_CUT_DTYPE = np.dtype([("struct_size", "<i4"), ("mode", "<i4"), ("out_elem", 
                           ("first_track", "<i4"), ("num_tracks", "<i4"), ("ref_track", "<i4"), ("reserved", "<i4")])
 MIX_ROLE_MIXED, MIX_ROLE_ENERGY = 0, 1
 MIX_F32, MIX_SCALED_FIRST = 0, 1
+MIX_SRC_F32 = 2  # b200feat_mix_track.source of a track in the float32 track buffer (src2)
 
 # b200feat_resample_stage as a numpy record layout (the transform route's stage table is built with vector operations)
 RESAMPLE_STAGE_DTYPE = np.dtype([("struct_size", "<i4"), ("table", "<i4"), ("source", "<i4"), ("target", "<i4"), ("depth", "<i4"),
@@ -95,7 +96,7 @@ EXPORTS = [
     "b200feat_extract_host_at", "b200feat_desc_num_frames",
     "b200feat_get_table", "b200feat_get_stats", "b200feat_set_output_affine", "b200feat_extract_host_ptrs",
     "b200feat_flac_index", "b200feat_flac_decode", "b200feat_mix_work_bytes", "b200feat_mix",
-    "b200feat_resample_table", "b200feat_resample_work_bytes", "b200feat_resample",
+    "b200feat_resample_table", "b200feat_resample_work_bytes", "b200feat_resample", "b200feat_mix_ex",
 ]
 
 
@@ -163,6 +164,8 @@ def load_library():
         lib.b200feat_mix_work_bytes.argtypes = [i32, i32]
         lib.b200feat_mix.restype = C.c_int
         lib.b200feat_mix.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
+        lib.b200feat_mix_ex.restype = C.c_int
+        lib.b200feat_mix_ex.argtypes = [vp, vp, i64, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
         lib.b200feat_resample_table.restype = C.c_int
         lib.b200feat_resample_table.argtypes = [vp, i32, i32, vp, i32, i32, i32, C.POINTER(i32)]
         lib.b200feat_resample_work_bytes.restype = i64
@@ -233,22 +236,23 @@ def flac_decode(bytes_dev: torch.Tensor, jobs_dev: torch.Tensor, njobs: int, out
 
 
 def mix(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], tracks: np.ndarray, cuts: np.ndarray, out: torch.Tensor,
-        handle=None) -> None:
-    """Launches `b200feat_mix` on the current stream of `out`'s device (asynchronous): the int16 device sources (None =
-    empty), the host track / cut tables (MIX_TRACK_DTYPE / MIX_CUT_DTYPE arrays, pinned or not: they are read by a copy on the
-    same stream, so a pinned table must not change until that copy has run) and the float32 output.  Raises B200FeatError
-    when the library refuses the tables."""
+        handle=None, src2: Optional[torch.Tensor] = None) -> None:
+    """Launches `b200feat_mix_ex` on the current stream of `out`'s device (asynchronous): the int16 device sources and the
+    float32 track buffer `src2` (None = empty), the host track / cut tables (MIX_TRACK_DTYPE / MIX_CUT_DTYPE arrays, pinned or
+    not: they are read by a copy on the same stream, so a pinned table must not change until that copy has run) and the
+    float32 output.  Raises B200FeatError when the library refuses the tables."""
     lib = load_library()
     stream = torch.cuda.current_stream(out.device).cuda_stream
     assert tracks.dtype == MIX_TRACK_DTYPE and cuts.dtype == MIX_CUT_DTYPE and out.dtype == torch.float32
+    assert src2 is None or src2.dtype == torch.float32
     work = torch.empty(max(int(lib.b200feat_mix_work_bytes(len(tracks), len(cuts))), 1), dtype=torch.uint8, device=out.device)
 
     def src(t):
         return (None, 0) if t is None or t.numel() == 0 else (t.data_ptr(), t.numel())
 
-    (p0, n0), (p1, n1) = src(src0), src(src1)
-    rc = lib.b200feat_mix(handle, p0, n0, p1, n1, tracks.ctypes.data, len(tracks), cuts.ctypes.data, len(cuts), out.data_ptr(),
-                          out.numel(), work.data_ptr(), work.numel(), stream)
+    (p0, n0), (p1, n1), (p2, n2) = src(src0), src(src1), src(src2)
+    rc = lib.b200feat_mix_ex(handle, p0, n0, p1, n1, p2, n2, tracks.ctypes.data, len(tracks), cuts.ctypes.data, len(cuts),
+                             out.data_ptr(), out.numel(), work.data_ptr(), work.numel(), stream)
     if rc != 0:
         msg = (lib.b200feat_last_error(handle) if handle is not None else lib.b200feat_global_error()).decode()
         raise B200FeatError(rc, msg)

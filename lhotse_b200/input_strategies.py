@@ -34,6 +34,7 @@ class FusedOnTheFlyFeatures:
         features_on_device: bool = True,
         pcm16_fast_path: bool = True,
         global_mvn=None,
+        perturbed_tracks: bool = False,
     ) -> None:
         if not hasattr(extractor, "extract_batch_padded"):
             raise TypeError("FusedOnTheFlyFeatures needs a lhotse_b200 extractor (extract_batch_padded)")
@@ -55,8 +56,12 @@ class FusedOnTheFlyFeatures:
         # slice, the tracks are staged as int16 by those rings and mixed on the GPU, bit-identical to lhotse ("mix").
         # When the batch holds speed-perturbed, volume-perturbed or resampled cuts of such files (and no MixedCut), the
         # source slices are staged as int16 and the transforms run on the GPU, bit-identical to lhotse ("transform").
-        # `pcm16_fast_path=False` turns all staged routes off.
+        # `perturbed_tracks=True` lets the "mix" route also take MixedCut tracks (and plain cuts beside them) with such
+        # transforms: the resample kernel loads them into a float32 track buffer that the mix kernels read.  It is off by
+        # default so that existing pipelines keep exactly their routes; whether to turn it on by default is decided once H100
+        # measurements of it exist.  `pcm16_fast_path=False` turns all staged routes off.
         self.pcm16_fast_path = pcm16_fast_path and hasattr(extractor, "extract_staged_padded")
+        self.perturbed_tracks = perturbed_tracks
         self._ring = None
         self._flac_ring = None
         self._mix_ring = None
@@ -136,7 +141,7 @@ class FusedOnTheFlyFeatures:
     def _try_mix(self, cuts):
         from .pcm_staging import MixStagingRing, mix_requests_for_batch
 
-        reqs = mix_requests_for_batch(cuts)
+        reqs = mix_requests_for_batch(cuts, perturbed_tracks=self.perturbed_tracks)
         if reqs is None:
             return None  # a cut the mix route cannot take: the float route
         if self._mix_ring is None:

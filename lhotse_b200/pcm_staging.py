@@ -572,7 +572,7 @@ def flac_request_for_cut(cut) -> Optional[FlacRequest]:
 
 @dataclass(frozen=True)
 class MixTrackRequest:
-    source: Optional[object]  # PcmRequest | FlacRequest; None = a PaddingCut (zeros)
+    source: Optional[object]  # PcmRequest | FlacRequest | TransformRequest (a perturbed track); None = a PaddingCut (zeros)
     num_samples: int
     offset: int               # first sample in the mix
     snr_factor: float         # 10 ** (-snr / 10) as Python evaluates it; NaN = no SNR
@@ -592,12 +592,18 @@ def _numpy2() -> bool:
     return int(np.__version__.split(".")[0]) >= 2
 
 
-def mix_request_for_cut(cut) -> Optional[MixRequest]:
+def mix_request_for_cut(cut, perturbed_tracks: bool = False) -> Optional[MixRequest]:
     """What `MixedCut.load_audio()` (lhotse/cut/mixed.py) amounts to for a MixedCut of mono 16-bit WAV / FLAC slices and
     PaddingCuts: tracks, offsets, SNR factors, reference and length.  None when the cut is not eligible: not a MixedCut,
     cut-level transforms, a track that `pcm16_request_for_cut` / `flac_request_for_cut` refuse (MultiCut, nested MixedCut,
     recording transforms, other formats), a sampling rate other than the cut's, an empty track, a length outside lhotse's
-    duration-mismatch tolerance, or NumPy 1.x (whose promotion of np.float64 * float32 arrays differs)."""
+    duration-mismatch tolerance, or NumPy 1.x (whose promotion of np.float64 * float32 arrays differs).
+
+    `perturbed_tracks=True` also takes a MonoCut track whose recording carries a chain `transform_request_for_cut` accepts
+    (Speed / Volume / Resample): its source is that TransformRequest and its length the request's, the resample kernel loads
+    it into a float32 track buffer and the mix kernels read it there (DESIGN.md §3.1h).  The default is False so that
+    existing callers keep exactly the routes they have; turning it on by default is a decision for when H100 measurements
+    of the route exist."""
     if not _numpy2():
         return None
     try:
@@ -630,7 +636,10 @@ def mix_request_for_cut(cut) -> Optional[MixRequest]:
         if isinstance(c, PaddingCut):
             src, n = None, compute_num_samples(c.duration, sr)
         elif isinstance(c, MonoCut) and not isinstance(c, MixedCut):
-            src = pcm16_request_for_cut(c) or flac_request_for_cut(c)
+            if perturbed_tracks and _has_transforms(c):
+                src = transform_request_for_cut(c)  # num_samples: the chain's output after lhotse's length fix
+            else:
+                src = pcm16_request_for_cut(c) or flac_request_for_cut(c)
             if src is None:
                 return None
             n = src.num_samples
@@ -660,27 +669,39 @@ def mix_request_for_cut(cut) -> Optional[MixRequest]:
                       num_samples=target)
 
 
-def _plain_mix_request(cut) -> Optional[MixRequest]:
-    """A plain 16-bit WAV / FLAC slice as a mix of one track (the kernel writes x = q / 32768, what the float route reads)."""
+def _plain_mix_request(cut, perturbed_tracks: bool = False) -> Optional[MixRequest]:
+    """A plain 16-bit WAV / FLAC slice as a mix of one track (the kernel writes x = q / 32768, what the float route reads);
+    with `perturbed_tracks`, also a MonoCut with an eligible transform chain (the kernel copies the chain's float32 output)."""
     from .engine import MIX_F32, MIX_ROLE_MIXED
 
     if getattr(cut, "tracks", None) is not None:
         return None
-    src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
+    if perturbed_tracks and _has_transforms(cut):
+        src = transform_request_for_cut(cut)
+    else:
+        src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
     if src is None or src.num_samples <= 0:
         return None
     return MixRequest(tracks=(MixTrackRequest(src, int(src.num_samples), 0, float("nan"), MIX_ROLE_MIXED),), ref=0,
                       mode=MIX_F32, mix_len=int(src.num_samples), num_samples=int(src.num_samples))
 
 
-def mix_requests_for_batch(cuts) -> Optional[List[MixRequest]]:
+def _mix_or_plain_request(cut, perturbed_tracks: bool = False) -> Optional[MixRequest]:
+    if getattr(cut, "tracks", None) is not None:
+        return mix_request_for_cut(cut, perturbed_tracks=perturbed_tracks)
+    return _plain_mix_request(cut, perturbed_tracks=perturbed_tracks)
+
+
+def mix_requests_for_batch(cuts, perturbed_tracks: bool = False) -> Optional[List[MixRequest]]:
     """The "mix" route's requests for a batch: every cut a plain 16-bit WAV / FLAC slice or an eligible MixedCut, and at least
-    one MixedCut (batches of plain slices keep the "pcm16" / "flac" / "float" routes).  None otherwise."""
+    one MixedCut (batches of plain slices keep the "pcm16" / "flac" / "float" routes).  None otherwise.  With
+    `perturbed_tracks=True` (see `mix_request_for_cut`; off by default), MixedCut tracks and plain MonoCuts with an eligible
+    Speed / Volume / Resample chain are taken too."""
     if not any(getattr(c, "tracks", None) is not None for c in cuts):
         return None
     reqs = []
     for c in cuts:
-        r = mix_request_for_cut(c) if getattr(c, "tracks", None) is not None else _plain_mix_request(c)
+        r = _mix_or_plain_request(c, perturbed_tracks)
         if r is None:
             return None
         reqs.append(r)
@@ -690,7 +711,8 @@ def mix_requests_for_batch(cuts) -> Optional[List[MixRequest]]:
 @dataclass
 class MixBatch:
     """One staged mix batch: the WAV tracks in the PCM ring's pinned int16 buffer, the FLAC tracks as a staged FlacBatch,
-    and the b200feat_mix track / cut tables (pinned numpy views) that place every cut's float32 mix in the output."""
+    and the b200feat_mix track / cut tables (pinned numpy views) that place every cut's float32 mix in the output; perturbed
+    tracks (source 2) as a staged TransformBatch whose "cuts" are those tracks, run into the float32 track buffer first."""
     pcm: Optional[torch.Tensor]
     flac: Optional[FlacBatch]
     tracks: np.ndarray        # engine.MIX_TRACK_DTYPE
@@ -698,11 +720,13 @@ class MixBatch:
     lens: List[int]
     offsets: List[int]
     out_elems: int
+    transform: Optional[TransformBatch] = None
 
 
 class MixStagingRing(_PinnedRing):
-    """A PcmStagingRing, a FlacStagingRing and pinned table bytes for one mix batch; `stage(requests)` returns
-    (MixBatch, lengths, offsets, sampling rate), the rate None when the tracks' files have several."""
+    """A PcmStagingRing, a FlacStagingRing and pinned table bytes for one mix batch, plus a TransformStagingRing for the
+    perturbed tracks (made when a batch first has one); `stage(requests)` returns (MixBatch, lengths, offsets, sampling rate),
+    the rate None when the tracks have several."""
 
     ALIGN = 4
 
@@ -710,23 +734,28 @@ class MixStagingRing(_PinnedRing):
         super().__init__(pin_memory)
         self.pcm = PcmStagingRing(initial_samples=1 << 20, pin_memory=self._pin)
         self.flac = FlacStagingRing(initial_bytes=1 << 16, pin_memory=self._pin)
+        self.transform: Optional[TransformStagingRing] = None
         self._tables = torch.empty(1 << 16, dtype=torch.uint8, pin_memory=self._pin)
 
     def mark_in_flight(self, device=None) -> None:
         super().mark_in_flight(device)
         self.pcm.mark_in_flight(device)
         self.flac.mark_in_flight(device)
+        if self.transform is not None:
+            self.transform.mark_in_flight(device)
 
     def stage(self, requests: Sequence[MixRequest], executor=None) -> Tuple[MixBatch, List[int], List[int], Optional[int]]:
-        from .engine import MIX_CUT_DTYPE, MIX_TRACK_DTYPE
+        from .engine import MIX_CUT_DTYPE, MIX_SRC_F32, MIX_TRACK_DTYPE
 
         self._wait_idle()
         flat = [t for r in requests for t in r.tracks]
-        kind = np.asarray([-1 if t.source is None else (0 if isinstance(t.source, PcmRequest) else 1) for t in flat], dtype=np.int32)
+        kind = np.asarray([-1 if t.source is None else 0 if isinstance(t.source, PcmRequest) else
+                           MIX_SRC_F32 if isinstance(t.source, TransformRequest) else 1 for t in flat], dtype=np.int32)
         wav = [t.source for t, k in zip(flat, kind) if k == 0]
         flac = [t.source for t, k in zip(flat, kind) if k == 1]
+        perturbed = [t.source for t, k in zip(flat, kind) if k == MIX_SRC_F32]
         srs = set()
-        pcm_buf, flac_batch = None, None
+        pcm_buf, flac_batch, transform_batch = None, None, None
         src_elem = np.zeros(len(flat), dtype=np.int64)
         if wav:
             pcm_buf, _, offs0, sr0 = self.pcm.stage(wav, executor=executor)
@@ -736,6 +765,12 @@ class MixStagingRing(_PinnedRing):
             flac_batch, _, offs1, sr1 = self.flac.stage(flac, executor=executor)
             src_elem[kind == 1] = offs1
             srs.add(sr1)
+        if perturbed:
+            if self.transform is None:
+                self.transform = TransformStagingRing(pin_memory=self._pin)
+            transform_batch, _, offs2, sr2 = self.transform.stage(perturbed, executor=executor)
+            src_elem[kind == MIX_SRC_F32] = offs2
+            srs.add(sr2)
         B, T = len(requests), len(flat)
         lens = [int(r.num_samples) for r in requests]
         offs, out_elems = _aligned_offsets(lens, self.ALIGN)
@@ -762,35 +797,39 @@ class MixStagingRing(_PinnedRing):
         cuts["num_tracks"] = ntr
         cuts["ref_track"] = [r.ref for r in requests]
         cuts["reserved"] = 0
-        batch = MixBatch(pcm=pcm_buf, flac=flac_batch, tracks=tracks, cuts=cuts, lens=lens, offsets=offs, out_elems=out_elems)
+        batch = MixBatch(pcm=pcm_buf, flac=flac_batch, tracks=tracks, cuts=cuts, lens=lens, offsets=offs, out_elems=out_elems,
+                         transform=transform_batch)
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
 
 
 def mix_staged(batch: MixBatch, device, ring: Optional[_PinnedRing] = None, handle=None) -> Tuple[torch.Tensor, List[int], List[int]]:
-    """The device half of the "mix" route on the current stream: H2D of the WAV tracks, the FLAC decode (if any), the table
-    copies, the energy and mix kernels; then `ring`'s copies are marked in flight.  Returns (float32 mixes on `device`,
-    lengths, offsets)."""
+    """The device half of the "mix" route on the current stream: H2D of the WAV tracks, the FLAC decode (if any), the
+    perturbed tracks' transform stages into the float32 track buffer (if any), the table copies, the energy and mix kernels;
+    then `ring`'s copies are marked in flight.  Returns (float32 mixes on `device`, lengths, offsets)."""
     from .engine import mix
 
     device = torch.device(device)
     with torch.cuda.device(device):
         src0 = batch.pcm.to(device, non_blocking=True) if batch.pcm is not None else None
         src1 = decode_staged(batch.flac, device)[0] if batch.flac is not None else None
+        src2 = transform_staged(batch.transform, device, handle=handle)[0] if batch.transform is not None else None
         out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
-        mix(src0, src1, batch.tracks, batch.cuts, out, handle)
+        mix(src0, src1, batch.tracks, batch.cuts, out, handle, src2=src2)
         if ring is not None:
             ring.mark_in_flight(device)
     return out, batch.lens, batch.offsets
 
 
-def mix_cuts(cuts, device="cuda", executor=None,
-             ring: Optional[MixStagingRing] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
+def mix_cuts(cuts, device="cuda", executor=None, ring: Optional[MixStagingRing] = None,
+             perturbed_tracks: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
     """Mixes MixedCuts (and plain 16-bit WAV / FLAC slices) on the GPU: (float32 device tensor holding every cut's samples at
     its offset, on 4-sample boundaries, lengths, offsets), each cut bit-identical to float32(cut.load_audio()).  Raises
-    ValueError naming the first cut the route cannot take."""
+    ValueError naming the first cut the route cannot take.  `perturbed_tracks=True` also takes tracks (and plain cuts) with
+    Speed / Volume / Resample chains, run on the GPU into a float32 track buffer first (see `mix_request_for_cut`; off by
+    default, so that existing callers keep their behaviour until H100 measurements of the route exist)."""
     reqs = []
     for c in cuts:
-        r = mix_request_for_cut(c) if getattr(c, "tracks", None) is not None else _plain_mix_request(c)
+        r = _mix_or_plain_request(c, perturbed_tracks)
         if r is None:
             raise ValueError(f"cut {getattr(c, 'id', c)!r} cannot be mixed on the GPU (see mix_request_for_cut)")
         reqs.append(r)

@@ -225,6 +225,7 @@ def compute_and_store_features_fused(
     num_workers: int = 4,
     overwrite: bool = False,
     pcm16_fast_path: bool = True,
+    perturbed_tracks: bool = False,
 ):
     """`CutSet.compute_and_store_features_batch(extractor, storage_path, manifest_path, batch_duration, num_workers,
     overwrite=...)` (lhotse/cut/set.py:2197-2408) with the batch kept whole from the GPU to the disk: one packed
@@ -233,7 +234,11 @@ def compute_and_store_features_fused(
 
     Three stages run concurrently, one batch apart: a reader thread samples the next batch and fills a pinned PCM ring
     (`num_workers` file readers), the calling thread moves it through the GPU, a writer thread appends the packed features
-    to the archive and then writes the batch's manifest lines (in this order, so an entry never precedes its data)."""
+    to the archive and then writes the batch's manifest lines (in this order, so an entry never precedes its data).
+
+    `perturbed_tracks=True` lets the "mix" stage also take MixedCuts whose tracks carry Speed / Volume / Resample chains
+    (`pcm_staging.mix_request_for_cut`).  It is off by default so that existing calls keep exactly their routes, until H100
+    measurements of it decide the default."""
     import json
     import queue
     import threading
@@ -329,7 +334,7 @@ def compute_and_store_features_fused(
                     reqs = [flac_request_for_cut(c) for c in batch_cuts]
                 if not all(r is not None for r in reqs):
                     kind, free = "mix", mix_rings
-                    reqs = mix_requests_for_batch(batch_cuts) or [None]
+                    reqs = mix_requests_for_batch(batch_cuts, perturbed_tracks=perturbed_tracks) or [None]
                 if not all(r is not None for r in reqs):
                     kind, free = "transform", transform_rings
                     reqs = transform_requests_for_batch(batch_cuts) or [None]
