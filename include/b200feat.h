@@ -402,6 +402,48 @@ int b200feat_resample(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_
                       int64_t src1_elems, float *mid_dev, int64_t mid_elems, const b200feat_resample_stage *stages,
                       int32_t nstages, float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
 
+/*
+ * Reverberation of mono float32 audio with room impulse responses on the GPU: lhotse's ReverbWithImpulseResponse with a
+ * recorded mono RIR (shift output, normalize_output optional), within a float32 tolerance of a float64 convolution
+ * (DESIGN.md §3.1j).  The RIRs are int16 samples of two device buffers (e.g. a PCM16 batch and a FLAC decode), taken as
+ * f32(q / 32768) * 2^-15 as lhotse scales them; the inputs are float32 samples of one buffer (e.g. what b200feat_resample or
+ * b200feat_mix_ex wrote); every cut's result is written as float32 into a ragged output buffer that b200feat_extract takes as
+ * B200FEAT_F32.
+ */
+#define B200FEAT_REVERB_MAX_RIR 65536  /* the longest RIR, in samples */
+
+typedef struct b200feat_reverb_rir {
+  int32_t struct_size;   /* sizeof(b200feat_reverb_rir) — ABI guard, in every record */
+  int32_t source;        /* 0: src0, 1: src1 */
+  int64_t src_elem;      /* first RIR sample in its source buffer */
+  int64_t num_samples;   /* R, 1 <= R <= B200FEAT_REVERB_MAX_RIR */
+} b200feat_reverb_rir;
+
+typedef struct b200feat_reverb_cut {
+  int32_t struct_size;   /* sizeof(b200feat_reverb_cut) */
+  int32_t rir;           /* index into the RIR table */
+  int32_t normalize;     /* 1: scale the result to the input's power (lhotse's normalize_output), 0: leave it */
+  int32_t reserved;
+  int64_t in_elem;       /* first input sample in the input buffer */
+  int64_t in_len;        /* N, at least 1: the output of the reverb has N samples too */
+  int64_t out_elem;      /* first output sample in the output buffer */
+  int64_t target_len;    /* samples written: N, fewer (trimmed) or at most N - 1 more (np.pad(mode="reflect")) */
+} b200feat_reverb_cut;
+/* The input and output buffers may be one allocation, but no cut's output window [out_elem, out_elem + target_len) may
+ * overlap any cut's input window [in_elem, in_elem + in_len) in memory: b200feat_reverb refuses such tables. */
+
+/* Device scratch b200feat_reverb needs for these tables (0 when a count is negative). */
+int64_t b200feat_reverb_work_bytes(const b200feat_reverb_rir *rirs, int32_t nrirs, const b200feat_reverb_cut *cuts, int32_t ncuts);
+
+/* Checks the host tables (every read inside its source, every write inside the output, RIR indices, 1 <= R <= the cap,
+ * reflect padding shorter than the signal), copies what the kernels read to `work_dev` and launches the RIR spectra,
+ * convolution, gain and output kernels, asynchronously on `stream`.  Output windows must not overlap input windows (above).  Results are identical from run to run.  Errors are
+ * reported through `h` (b200feat_last_error) when it is not NULL, and through b200feat_global_error. */
+int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
+                    const float *in_dev, int64_t in_elems, const b200feat_reverb_rir *rirs, int32_t nrirs,
+                    const b200feat_reverb_cut *cuts, int32_t ncuts, float *out_dev, int64_t out_elems, void *work_dev,
+                    int64_t work_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

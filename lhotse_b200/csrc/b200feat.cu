@@ -7,6 +7,7 @@
 
 #include <immintrin.h>
 
+#include <algorithm>
 #include <atomic>
 #include <condition_variable>
 #include <functional>
@@ -27,6 +28,7 @@
 #include "flac.cuh"
 #include "mix.cuh"
 #include "resample.cuh"
+#include "reverb.cuh"
 
 namespace {
 
@@ -1094,6 +1096,152 @@ int b200feat_resample(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_
     resample_stage_kernel<<<(unsigned)n, RS_THREADS, group_smem[gi], st>>>(d_rs + a, b - a);
     CU_TRY(h, cudaGetLastError());
   }
+  return B200FEAT_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The reverb work buffer: the kernels' RIR and cut tables, the shifts, the RIR spectra, y, the per-CTA partials and the gains
+struct RvLayout {
+  int64_t rirs, cuts, shift, twiddles, spectra, y, partial, gain, total;
+  int64_t parts, samples, ctas;
+};
+
+RvLayout rv_layout(const b200feat_reverb_rir *rirs, int32_t nrirs, const b200feat_reverb_cut *cuts, int32_t ncuts) {
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  RvLayout l{};
+  for (int32_t i = 0; i < nrirs; ++i) l.parts += rv_parts(std::min<int64_t>(std::max<int64_t>(rirs[i].num_samples, 0), RV_MAX_RIR));
+  for (int32_t i = 0; i < ncuts; ++i) {
+    const int64_t n = std::min<int64_t>(std::max<int64_t>(cuts[i].in_len, 0), (int64_t)1 << 40);
+    l.samples += n;
+    l.ctas += rv_cut_ctas(n);
+  }
+  l.rirs = 0;
+  l.cuts = l.rirs + up((int64_t)nrirs * (int64_t)sizeof(RvRir));
+  l.shift = l.cuts + up((int64_t)ncuts * (int64_t)sizeof(RvCut));
+  l.twiddles = l.shift + up((int64_t)nrirs * 4);
+  l.spectra = l.twiddles + up(RV_B * (int64_t)sizeof(rv_c));
+  l.y = l.spectra + up(l.parts * RV_F * (int64_t)sizeof(rv_c));
+  l.partial = l.y + up(l.samples * 4);
+  l.gain = l.partial + up(l.ctas * 4);
+  l.total = l.gain + up((int64_t)ncuts * 4);
+  return l;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t b200feat_reverb_work_bytes(const b200feat_reverb_rir *rirs, int32_t nrirs, const b200feat_reverb_cut *cuts, int32_t ncuts) {
+  if (nrirs < 0 || ncuts < 0 || (nrirs > 0 && !rirs) || (ncuts > 0 && !cuts)) return 0;
+  return rv_layout(rirs, nrirs, cuts, ncuts).total;
+}
+
+int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev, int64_t src1_elems,
+                    const float *in_dev, int64_t in_elems, const b200feat_reverb_rir *rirs, int32_t nrirs,
+                    const b200feat_reverb_cut *cuts, int32_t ncuts, float *out_dev, int64_t out_elems, void *work_dev,
+                    int64_t work_bytes, void *stream) {
+  if (nrirs < 0 || ncuts < 0 || (ncuts > 0 && (!rirs || !cuts || !in_dev || !out_dev || !work_dev || nrirs < 1)) ||
+      src0_elems < 0 || src1_elems < 0 || in_elems < 0 || out_elems < 0)
+    return fail(h, B200FEAT_EINVAL, "reverb: bad arguments");
+  if (ncuts == 0) return B200FEAT_OK;
+  if (ncuts > 65535) return fail(h, B200FEAT_EINVAL, "reverb: more than 65535 cuts in one call");
+  const int16_t *src[2] = {src0_dev, src1_dev};
+  const int64_t src_elems[2] = {src0_elems, src1_elems};
+  auto where = [](const char *what, int64_t i) { return std::string("reverb: ") + what + " " + std::to_string(i) + ": "; };
+  for (int32_t i = 0; i < nrirs; ++i) {
+    const b200feat_reverb_rir &r = rirs[i];
+    if (r.struct_size != (int32_t)sizeof(b200feat_reverb_rir))
+      return fail(h, B200FEAT_EINVAL, where("rir", i) + "b200feat_reverb_rir size mismatch (ABI)");
+    if (r.source < 0 || r.source > 1) return fail(h, B200FEAT_EINVAL, where("rir", i) + "source must be 0 or 1");
+    if (r.num_samples < 1 || r.num_samples > B200FEAT_REVERB_MAX_RIR)
+      return fail(h, B200FEAT_EINVAL, where("rir", i) + "length outside 1 .. B200FEAT_REVERB_MAX_RIR");
+    if (!src[r.source] || r.src_elem < 0 || r.src_elem > src_elems[r.source] - r.num_samples)
+      return fail(h, B200FEAT_EINVAL, where("rir", i) + "samples outside its source buffer");
+  }
+  for (int32_t c = 0; c < ncuts; ++c) {
+    const b200feat_reverb_cut &cu = cuts[c];
+    if (cu.struct_size != (int32_t)sizeof(b200feat_reverb_cut))
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "b200feat_reverb_cut size mismatch (ABI)");
+    if (cu.rir < 0 || cu.rir >= nrirs) return fail(h, B200FEAT_EINVAL, where("cut", c) + "RIR index out of range");
+    if (cu.normalize != 0 && cu.normalize != 1) return fail(h, B200FEAT_EINVAL, where("cut", c) + "normalize must be 0 or 1");
+    if (cu.in_len < 1 || cu.in_len > ((int64_t)1 << 40) || cu.in_elem < 0 || cu.in_elem > in_elems - cu.in_len)
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "input outside the input buffer");
+    if (cu.target_len < 0 || (cu.target_len > cu.in_len && cu.target_len - cu.in_len > cu.in_len - 1))
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "bad target_len (reflect padding longer than the signal?)");
+    if (cu.out_elem < 0 || cu.out_elem > out_elems - cu.target_len)
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "output outside the output buffer");
+  }
+  {  // no cut's output window may overlap any cut's input window: the output kernel writes while others read
+    std::vector<std::pair<uintptr_t, uintptr_t>> in(ncuts);
+    for (int32_t c = 0; c < ncuts; ++c) {
+      const uintptr_t a = (uintptr_t)(in_dev + cuts[c].in_elem);
+      in[c] = {a, a + (uintptr_t)cuts[c].in_len * sizeof(float)};
+    }
+    std::sort(in.begin(), in.end());
+    std::vector<uintptr_t> reach(ncuts);  // the furthest end among the first i + 1 windows
+    for (int32_t c = 0; c < ncuts; ++c) reach[c] = std::max(in[c].second, c ? reach[c - 1] : 0);
+    for (int32_t c = 0; c < ncuts; ++c) {
+      if (cuts[c].target_len == 0) continue;
+      const uintptr_t a = (uintptr_t)(out_dev + cuts[c].out_elem), b = a + (uintptr_t)cuts[c].target_len * sizeof(float);
+      // the input windows that start before b: one of them overlaps [a, b) iff the furthest of their ends lies past a
+      const auto it = std::lower_bound(in.begin(), in.end(), std::make_pair(b, (uintptr_t)0));
+      if (it != in.begin() && reach[(it - in.begin()) - 1] > a)
+        return fail(h, B200FEAT_EINVAL, where("cut", c) + "output overlaps an input window");
+    }
+  }
+  const RvLayout l = rv_layout(rirs, nrirs, cuts, ncuts);
+  if (work_bytes < l.total) return fail(h, B200FEAT_EINVAL, "reverb: work buffer too small");
+  if (l.parts > 0x7fffffff || l.ctas > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "reverb: too many CTAs in one call");
+  char *w = (char *)work_dev;
+  rv_c *spectra = (rv_c *)(w + l.spectra);
+  float *y = (float *)(w + l.y);
+  std::vector<RvRir> rv((size_t)nrirs);
+  int64_t parts = 0;
+  for (int32_t i = 0; i < nrirs; ++i) {
+    rv[i] = RvRir{src[rirs[i].source] + rirs[i].src_elem, rirs[i].num_samples, parts, (int32_t)rv_parts(rirs[i].num_samples), 0};
+    parts += rv[i].nparts;
+  }
+  std::vector<RvCut> cv((size_t)ncuts);
+  int64_t ctas = 0, samples = 0;
+  int64_t longest = 1;
+  for (int32_t c = 0; c < ncuts; ++c) {
+    const b200feat_reverb_cut &cu = cuts[c];
+    cv[c] = RvCut{in_dev + cu.in_elem, y + samples, out_dev + cu.out_elem, cu.in_len, cu.target_len, ctas, cu.rir, cu.normalize};
+    samples += cu.in_len;
+    ctas += rv_cut_ctas(cu.in_len);
+    longest = std::max(longest, cu.target_len);
+  }
+  // just over the 48 KB a launch gets without asking; set on every call (the attribute belongs to the current device)
+  CU_TRY(h, cudaFuncSetAttribute(reverb_rir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RV_SMEM_BYTES));
+  CU_TRY(h, cudaFuncSetAttribute(reverb_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RV_SMEM_BYTES));
+  const cudaStream_t st = (cudaStream_t)stream;
+  RvRir *d_rirs = (RvRir *)(w + l.rirs);
+  RvCut *d_cuts = (RvCut *)(w + l.cuts);
+  int32_t *d_shift = (int32_t *)(w + l.shift);
+  rv_c *d_twiddles = (rv_c *)(w + l.twiddles);
+  float *d_partial = (float *)(w + l.partial);
+  float *d_gain = (float *)(w + l.gain);
+  static const std::vector<rv_c> twiddles = [] {
+    std::vector<rv_c> t(RV_B);
+    for (int k = 0; k < RV_B; ++k) t[k] = rv_twiddle(k);
+    return t;
+  }();
+  // pageable copies: the call returns once the tables have been staged, so the vectors may go when this function returns
+  CU_TRY(h, cudaMemcpyAsync(d_twiddles, twiddles.data(), RV_B * sizeof(rv_c), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_rirs, rv.data(), rv.size() * sizeof(RvRir), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_cuts, cv.data(), cv.size() * sizeof(RvCut), cudaMemcpyHostToDevice, st));
+  reverb_rir_kernel<<<(unsigned)parts, RV_THREADS, RV_SMEM_BYTES, st>>>(d_rirs, nrirs, spectra, d_shift, d_twiddles);
+  CU_TRY(h, cudaGetLastError());
+  reverb_conv_kernel<<<(unsigned)ctas, RV_THREADS, RV_SMEM_BYTES, st>>>(d_cuts, ncuts, d_rirs, spectra, d_shift, d_twiddles, d_partial);
+  CU_TRY(h, cudaGetLastError());
+  reverb_gain_kernel<<<(unsigned)ncuts, RV_GAIN_THREADS, 0, st>>>(d_cuts, d_partial, d_gain);
+  CU_TRY(h, cudaGetLastError());
+  const int64_t gx = std::min<int64_t>((longest + 4 * RV_OUT_THREADS - 1) / (4 * RV_OUT_THREADS), 1024);
+  reverb_out_kernel<<<dim3((unsigned)gx, (unsigned)ncuts), RV_OUT_THREADS, 0, st>>>(d_cuts, d_gain);
+  CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }
 

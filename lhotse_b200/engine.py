@@ -88,6 +88,12 @@ RESAMPLE_STAGE_DTYPE = np.dtype([("struct_size", "<i4"), ("table", "<i4"), ("sou
 RESAMPLE_SRC0, RESAMPLE_SRC1, RESAMPLE_MID = 0, 1, 2
 RESAMPLE_TO_MID, RESAMPLE_TO_OUT = 0, 1
 
+# b200feat_reverb_rir / b200feat_reverb_cut as numpy record layouts
+REVERB_RIR_DTYPE = np.dtype([("struct_size", "<i4"), ("source", "<i4"), ("src_elem", "<i8"), ("num_samples", "<i8")])
+REVERB_CUT_DTYPE = np.dtype([("struct_size", "<i4"), ("rir", "<i4"), ("normalize", "<i4"), ("reserved", "<i4"), ("in_elem", "<i8"),
+                             ("in_len", "<i8"), ("out_elem", "<i8"), ("target_len", "<i8")])
+REVERB_MAX_RIR = 65536  # B200FEAT_REVERB_MAX_RIR
+
 
 EXPORTS = [
     "b200feat_version", "b200feat_global_error", "b200feat_create", "b200feat_destroy",
@@ -97,6 +103,7 @@ EXPORTS = [
     "b200feat_get_table", "b200feat_get_stats", "b200feat_set_output_affine", "b200feat_extract_host_ptrs",
     "b200feat_flac_index", "b200feat_flac_decode", "b200feat_mix_work_bytes", "b200feat_mix",
     "b200feat_resample_table", "b200feat_resample_work_bytes", "b200feat_resample", "b200feat_mix_ex",
+    "b200feat_reverb_work_bytes", "b200feat_reverb",
 ]
 
 
@@ -172,6 +179,10 @@ def load_library():
         lib.b200feat_resample_work_bytes.argtypes = [i32]
         lib.b200feat_resample.restype = C.c_int
         lib.b200feat_resample.argtypes = [vp, vp, i64, vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, vp]
+        lib.b200feat_reverb_work_bytes.restype = i64
+        lib.b200feat_reverb_work_bytes.argtypes = [vp, i32, vp, i32]
+        lib.b200feat_reverb.restype = C.c_int
+        lib.b200feat_reverb.argtypes = [vp, vp, i64, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -294,6 +305,30 @@ def resample(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], mid: Op
     with torch.cuda.device(out.device):
         rc = lib.b200feat_resample(handle, p0, n0, p1, n1, pm, nm, stages.ctypes.data, len(stages), out.data_ptr(), out.numel(),
                                    work.data_ptr(), work.numel(), stream)
+    if rc != 0:
+        _raise(lib, rc, handle)
+
+
+def reverb(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], x: torch.Tensor, rirs: np.ndarray, cuts: np.ndarray,
+           out: torch.Tensor, handle=None) -> None:
+    """Launches `b200feat_reverb` on the current stream of `out`'s device (asynchronous): the int16 device sources of the
+    RIRs, the float32 input `x`, the host RIR / cut tables (REVERB_RIR_DTYPE / REVERB_CUT_DTYPE; copied before this returns)
+    and the float32 output.  Raises B200FeatError when the library refuses the tables."""
+    lib = load_library()
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    assert rirs.dtype == REVERB_RIR_DTYPE and cuts.dtype == REVERB_CUT_DTYPE
+    assert x.dtype == torch.float32 and out.dtype == torch.float32
+    rirs, cuts = np.ascontiguousarray(rirs), np.ascontiguousarray(cuts)
+    nbytes = int(lib.b200feat_reverb_work_bytes(rirs.ctypes.data, len(rirs), cuts.ctypes.data, len(cuts)))
+    work = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=out.device)
+
+    def src(t):
+        return (None, 0) if t is None or t.numel() == 0 else (t.data_ptr(), t.numel())
+
+    (p0, n0), (p1, n1), (px, nx) = src(src0), src(src1), src(x)
+    with torch.cuda.device(out.device):
+        rc = lib.b200feat_reverb(handle, p0, n0, p1, n1, px, nx, rirs.ctypes.data, len(rirs), cuts.ctypes.data, len(cuts),
+                                 out.data_ptr(), out.numel(), work.data_ptr(), work.numel(), stream)
     if rc != 0:
         _raise(lib, rc, handle)
 

@@ -35,6 +35,7 @@ class FusedOnTheFlyFeatures:
         pcm16_fast_path: bool = True,
         global_mvn=None,
         perturbed_tracks: bool = False,
+        reverb: bool = False,
     ) -> None:
         if not hasattr(extractor, "extract_batch_padded"):
             raise TypeError("FusedOnTheFlyFeatures needs a lhotse_b200 extractor (extract_batch_padded)")
@@ -59,9 +60,16 @@ class FusedOnTheFlyFeatures:
         # `perturbed_tracks=True` lets the "mix" route also take MixedCut tracks (and plain cuts beside them) with such
         # transforms: the resample kernel loads them into a float32 track buffer that the mix kernels read.  It is off by
         # default so that existing pipelines keep exactly their routes; whether to turn it on by default is decided once H100
-        # measurements of it exist.  `pcm16_fast_path=False` turns all staged routes off.
+        # measurements of it exist.  `reverb=True` lets the "transform" and "mix" routes also take cuts reverberated with a
+        # recorded RIR (`cut.reverb_rir`, `MixedCut.reverb_rir` with mix_first, lhotse's ReverbWithImpulseResponse cut
+        # transform): the RIR is staged beside the speech and convolved on the GPU.  The float route's own FFT convolution
+        # is not bit-reproducible (its bits change with the CPU and the torch thread count), so this one is held to a float32
+        # tolerance of a float64 convolution instead of bit equality; it is off by default so that existing pipelines keep
+        # exactly their routes and features, and whether to turn it on by default is decided once H100 measurements of it
+        # exist.  `pcm16_fast_path=False` turns all staged routes off.
         self.pcm16_fast_path = pcm16_fast_path and hasattr(extractor, "extract_staged_padded")
         self.perturbed_tracks = perturbed_tracks
+        self.reverb = reverb
         self._ring = None
         self._flac_ring = None
         self._mix_ring = None
@@ -141,7 +149,7 @@ class FusedOnTheFlyFeatures:
     def _try_mix(self, cuts):
         from .pcm_staging import MixStagingRing, mix_requests_for_batch
 
-        reqs = mix_requests_for_batch(cuts, perturbed_tracks=self.perturbed_tracks)
+        reqs = mix_requests_for_batch(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb)
         if reqs is None:
             return None  # a cut the mix route cannot take: the float route
         if self._mix_ring is None:
@@ -161,7 +169,7 @@ class FusedOnTheFlyFeatures:
     def _try_transform(self, cuts):
         from .pcm_staging import TransformStagingRing, transform_requests_for_batch
 
-        reqs = transform_requests_for_batch(cuts)
+        reqs = transform_requests_for_batch(cuts, reverb=self.reverb)
         if reqs is None:
             return None  # a cut the transform route cannot take: the float route
         if self._transform_ring is None:

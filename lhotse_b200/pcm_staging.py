@@ -586,13 +586,14 @@ class MixRequest:
     mode: int                            # engine.MIX_F32 | engine.MIX_SCALED_FIRST
     mix_len: int                         # max(offset + length) over the mixed tracks
     num_samples: int                     # the cut's length: the mix is trimmed or reflect-padded to it
+    reverb: Optional["ReverbRequest"] = None  # a cut-level ReverbWithImpulseResponse, run on the length-fixed mix
 
 
 def _numpy2() -> bool:
     return int(np.__version__.split(".")[0]) >= 2
 
 
-def mix_request_for_cut(cut, perturbed_tracks: bool = False) -> Optional[MixRequest]:
+def mix_request_for_cut(cut, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[MixRequest]:
     """What `MixedCut.load_audio()` (lhotse/cut/mixed.py) amounts to for a MixedCut of mono 16-bit WAV / FLAC slices and
     PaddingCuts: tracks, offsets, SNR factors, reference and length.  None when the cut is not eligible: not a MixedCut,
     cut-level transforms, a track that `pcm16_request_for_cut` / `flac_request_for_cut` refuse (MultiCut, nested MixedCut,
@@ -603,19 +604,34 @@ def mix_request_for_cut(cut, perturbed_tracks: bool = False) -> Optional[MixRequ
     (Speed / Volume / Resample): its source is that TransformRequest and its length the request's, the resample kernel loads
     it into a float32 track buffer and the mix kernels read it there (DESIGN.md §3.1h).  The default is False so that
     existing callers keep exactly the routes they have; turning it on by default is a decision for when H100 measurements
-    of the route exist."""
+    of the route exist.
+
+    `reverb=True` also takes a MixedCut whose `transforms` are exactly one ReverbWithImpulseResponse that `reverb_request`
+    accepts (what `MixedCut.reverb_rir(mix_first=True)` makes) over a float32 mix: the mix goes to a float32 buffer and the
+    reverb kernel writes the cut, within a float32 tolerance of a float64 convolution (DESIGN.md §3.1j).  Tracks that carry a
+    reverb of their own (mix_first=False) stay refused.  Off by default."""
     if not _numpy2():
         return None
     try:
         from lhotse.audio.utils import get_audio_duration_mismatch_tolerance
+        from lhotse.augmentation.rir import ReverbWithImpulseResponse
+        from lhotse.augmentation.transform import AudioTransform
         from lhotse.cut import MixedCut, MonoCut, PaddingCut
         from lhotse.utils import compute_num_samples
     except ImportError:
         return None
     from .engine import MIX_F32, MIX_ROLE_ENERGY, MIX_ROLE_MIXED, MIX_SCALED_FIRST
 
-    if not isinstance(cut, MixedCut) or getattr(cut, "transforms", None) or not cut.tracks:
+    if not isinstance(cut, MixedCut) or not cut.tracks:
         return None
+    rv = None
+    if getattr(cut, "transforms", None):
+        tfs = [t if isinstance(t, AudioTransform) else AudioTransform.from_dict(t) for t in cut.transforms]
+        if not reverb or len(tfs) != 1 or type(tfs[0]) is not ReverbWithImpulseResponse:
+            return None
+        rv = reverb_request(tfs[0], cut.sampling_rate)
+        if rv is None:
+            return None
     sr = cut.sampling_rate
     tracks = list(cut.tracks)
     if all(isinstance(t.cut, PaddingCut) for t in tracks):
@@ -665,19 +681,30 @@ def mix_request_for_cut(cut, perturbed_tracks: bool = False) -> Optional[MixRequ
         return None
     first = audible[0]
     mode = MIX_SCALED_FIRST if (ref is not first and first.snr is not None) else MIX_F32
+    if rv is not None and mode != MIX_F32:
+        return None  # a float64 mix would be reverberated in float64
     return MixRequest(tracks=tuple(reqs), ref=next(i for i, t in enumerate(chosen) if t is ref), mode=mode, mix_len=mix_len,
-                      num_samples=target)
+                      num_samples=target, reverb=rv)
 
 
-def _plain_mix_request(cut, perturbed_tracks: bool = False) -> Optional[MixRequest]:
+def _plain_mix_request(cut, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[MixRequest]:
     """A plain 16-bit WAV / FLAC slice as a mix of one track (the kernel writes x = q / 32768, what the float route reads);
-    with `perturbed_tracks`, also a MonoCut with an eligible transform chain (the kernel copies the chain's float32 output)."""
+    with `perturbed_tracks`, also a MonoCut with an eligible transform chain (the kernel copies the chain's float32 output);
+    with `reverb`, also a plain slice whose only transform is an eligible reverb (a one-track mix, then the reverb), and with
+    both, a chain that ends in such a reverb (the transform route reverberates it into the track buffer, the kernel copies
+    that)."""
     from .engine import MIX_F32, MIX_ROLE_MIXED
 
     if getattr(cut, "tracks", None) is not None:
         return None
+    if reverb and _has_transforms(cut):
+        r = transform_request_for_cut(cut, reverb=True)
+        if r is not None and r.reverb is not None and not r.ops and r.num_samples == r.source.num_samples > 0:
+            n = int(r.num_samples)
+            return MixRequest(tracks=(MixTrackRequest(r.source, n, 0, float("nan"), MIX_ROLE_MIXED),), ref=0, mode=MIX_F32,
+                              mix_len=n, num_samples=n, reverb=r.reverb)
     if perturbed_tracks and _has_transforms(cut):
-        src = transform_request_for_cut(cut)
+        src = transform_request_for_cut(cut, reverb=reverb)
     else:
         src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
     if src is None or src.num_samples <= 0:
@@ -686,13 +713,13 @@ def _plain_mix_request(cut, perturbed_tracks: bool = False) -> Optional[MixReque
                       mode=MIX_F32, mix_len=int(src.num_samples), num_samples=int(src.num_samples))
 
 
-def _mix_or_plain_request(cut, perturbed_tracks: bool = False) -> Optional[MixRequest]:
+def _mix_or_plain_request(cut, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[MixRequest]:
     if getattr(cut, "tracks", None) is not None:
-        return mix_request_for_cut(cut, perturbed_tracks=perturbed_tracks)
-    return _plain_mix_request(cut, perturbed_tracks=perturbed_tracks)
+        return mix_request_for_cut(cut, perturbed_tracks=perturbed_tracks, reverb=reverb)
+    return _plain_mix_request(cut, perturbed_tracks=perturbed_tracks, reverb=reverb)
 
 
-def mix_requests_for_batch(cuts, perturbed_tracks: bool = False) -> Optional[List[MixRequest]]:
+def mix_requests_for_batch(cuts, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[List[MixRequest]]:
     """The "mix" route's requests for a batch: every cut a plain 16-bit WAV / FLAC slice or an eligible MixedCut, and at least
     one MixedCut (batches of plain slices keep the "pcm16" / "flac" / "float" routes).  None otherwise.  With
     `perturbed_tracks=True` (see `mix_request_for_cut`; off by default), MixedCut tracks and plain MonoCuts with an eligible
@@ -701,7 +728,7 @@ def mix_requests_for_batch(cuts, perturbed_tracks: bool = False) -> Optional[Lis
         return None
     reqs = []
     for c in cuts:
-        r = _mix_or_plain_request(c, perturbed_tracks)
+        r = _mix_or_plain_request(c, perturbed_tracks, reverb)
         if r is None:
             return None
         reqs.append(r)
@@ -721,6 +748,9 @@ class MixBatch:
     offsets: List[int]
     out_elems: int
     transform: Optional[TransformBatch] = None
+    pre_elems: int = 0                        # the reverberated cuts' mixes, after the output in the same buffer
+    reverb_rirs: Optional[np.ndarray] = None  # engine.REVERB_RIR_DTYPE
+    reverb_cuts: Optional[np.ndarray] = None  # engine.REVERB_CUT_DTYPE, reading and writing that buffer
 
 
 class MixStagingRing(_PinnedRing):
@@ -753,17 +783,20 @@ class MixStagingRing(_PinnedRing):
                            MIX_SRC_F32 if isinstance(t.source, TransformRequest) else 1 for t in flat], dtype=np.int32)
         wav = [t.source for t, k in zip(flat, kind) if k == 0]
         flac = [t.source for t, k in zip(flat, kind) if k == 1]
+        nwav, nflac = len(wav), len(flac)
         perturbed = [t.source for t, k in zip(flat, kind) if k == MIX_SRC_F32]
         srs = set()
         pcm_buf, flac_batch, transform_batch = None, None, None
         src_elem = np.zeros(len(flat), dtype=np.int64)
+        rirs, where = _stage_rirs(requests, wav, flac)  # at the cut's rate (reverb_request), so one rate per ring still holds
+        offs0 = offs1 = []
         if wav:
             pcm_buf, _, offs0, sr0 = self.pcm.stage(wav, executor=executor)
-            src_elem[kind == 0] = offs0
+            src_elem[kind == 0] = offs0[:nwav]
             srs.add(sr0)
         if flac:
             flac_batch, _, offs1, sr1 = self.flac.stage(flac, executor=executor)
-            src_elem[kind == 1] = offs1
+            src_elem[kind == 1] = offs1[:nflac]
             srs.add(sr1)
         if perturbed:
             if self.transform is None:
@@ -788,9 +821,16 @@ class MixStagingRing(_PinnedRing):
         tracks["snr_factor"] = [t.snr_factor for t in flat]
         tracks["cut"] = np.repeat(np.arange(B), ntr)
         tracks["role"] = [t.role for t in flat]
+        # a reverberated cut's mix goes to the pre-reverb region after the output, in the same buffer
+        rv_ix = [i for i, r in enumerate(requests) if r.reverb is not None]
+        pre_offs, pre_elems = _aligned_offsets([lens[i] for i in rv_ix], self.ALIGN)
+        base = (out_elems + self.ALIGN - 1) // self.ALIGN * self.ALIGN
+        mix_out = list(offs)
+        for i, o in zip(rv_ix, pre_offs):
+            mix_out[i] = base + o
         cuts["struct_size"] = MIX_CUT_DTYPE.itemsize
         cuts["mode"] = [r.mode for r in requests]
-        cuts["out_elem"] = offs
+        cuts["out_elem"] = mix_out
         cuts["mix_len"] = [r.mix_len for r in requests]
         cuts["target_len"] = lens
         cuts["first_track"] = np.concatenate(([0], np.cumsum(ntr)[:-1])) if B else []
@@ -799,37 +839,48 @@ class MixStagingRing(_PinnedRing):
         cuts["reserved"] = 0
         batch = MixBatch(pcm=pcm_buf, flac=flac_batch, tracks=tracks, cuts=cuts, lens=lens, offsets=offs, out_elems=out_elems,
                          transform=transform_batch)
+        if rv_ix:
+            rir_elem = [offs0[j] if k == 0 else offs1[j] for k, j in where]
+            batch.pre_elems = base - out_elems + pre_elems
+            batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(
+                rirs, where, rir_elem, [(requests[i].reverb, mix_out[i], lens[i], offs[i], lens[i]) for i in rv_ix])
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
 
 
 def mix_staged(batch: MixBatch, device, ring: Optional[_PinnedRing] = None, handle=None) -> Tuple[torch.Tensor, List[int], List[int]]:
     """The device half of the "mix" route on the current stream: H2D of the WAV tracks, the FLAC decode (if any), the
-    perturbed tracks' transform stages into the float32 track buffer (if any), the table copies, the energy and mix kernels;
-    then `ring`'s copies are marked in flight.  Returns (float32 mixes on `device`, lengths, offsets)."""
-    from .engine import mix
+    perturbed tracks' transform stages into the float32 track buffer (if any), the table copies, the energy and mix kernels,
+    the reverb of the reverberated cuts (if any); then `ring`'s copies are marked in flight.  Returns (float32 mixes on
+    `device`, lengths, offsets)."""
+    from .engine import mix, reverb
 
     device = torch.device(device)
     with torch.cuda.device(device):
         src0 = batch.pcm.to(device, non_blocking=True) if batch.pcm is not None else None
         src1 = decode_staged(batch.flac, device)[0] if batch.flac is not None else None
         src2 = transform_staged(batch.transform, device, handle=handle)[0] if batch.transform is not None else None
-        out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
+        out = torch.zeros(max(batch.out_elems + batch.pre_elems, 1), dtype=torch.float32, device=device)
         mix(src0, src1, batch.tracks, batch.cuts, out, handle, src2=src2)
+        if batch.reverb_cuts is not None:
+            reverb(src0, src1, out, batch.reverb_rirs, batch.reverb_cuts, out, handle)
+            out = out[: max(batch.out_elems, 1)]
         if ring is not None:
             ring.mark_in_flight(device)
     return out, batch.lens, batch.offsets
 
 
 def mix_cuts(cuts, device="cuda", executor=None, ring: Optional[MixStagingRing] = None,
-             perturbed_tracks: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
+             perturbed_tracks: bool = False, reverb: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
     """Mixes MixedCuts (and plain 16-bit WAV / FLAC slices) on the GPU: (float32 device tensor holding every cut's samples at
     its offset, on 4-sample boundaries, lengths, offsets), each cut bit-identical to float32(cut.load_audio()).  Raises
     ValueError naming the first cut the route cannot take.  `perturbed_tracks=True` also takes tracks (and plain cuts) with
     Speed / Volume / Resample chains, run on the GPU into a float32 track buffer first (see `mix_request_for_cut`; off by
-    default, so that existing callers keep their behaviour until H100 measurements of the route exist)."""
+    default, so that existing callers keep their behaviour until H100 measurements of the route exist).  `reverb=True` also
+    takes MixedCut-level reverbs and plain slices whose only transform is a reverb, reverberated on the GPU within a float32
+    tolerance of a float64 convolution (see `mix_request_for_cut`; off by default)."""
     reqs = []
     for c in cuts:
-        r = _mix_or_plain_request(c, perturbed_tracks)
+        r = _mix_or_plain_request(c, perturbed_tracks, reverb)
         if r is None:
             raise ValueError(f"cut {getattr(c, 'id', c)!r} cannot be mixed on the GPU (see mix_request_for_cut)")
         reqs.append(r)
@@ -957,26 +1008,67 @@ def resample_probe(orig: int, new: int) -> bool:
 
 
 @dataclass(frozen=True)
+class ReverbRequest:
+    rir: object                # PcmRequest | FlacRequest: the RIR's samples, what `rir.load_audio()` reads
+    normalize: bool            # lhotse's normalize_output
+
+
+@dataclass(frozen=True)
 class TransformRequest:
     source: object             # PcmRequest | FlacRequest: the slice of the file the chain starts from
     ops: Tuple[tuple, ...]     # in chain order: ("volume", float32 factor) | ("resample", orig, new)
     num_samples: int           # the cut's length: the chain's output is trimmed or reflect-padded to it
     sampling_rate: int         # the cut's (the recording's, after the chain)
+    reverb: Optional[ReverbRequest] = None  # a last ReverbWithImpulseResponse, run on the chain's output before the length fix
+
+
+def reverb_request(t, sampling_rate: int) -> Optional[ReverbRequest]:
+    """The RIR read of a ReverbWithImpulseResponse with a recorded mono RIR, as its __call__ loads it: `rir.to_cut()` for a
+    Recording, `with_channels(rir_channels)`, `truncate(duration=0.05)` when early_only, then a cut that
+    `pcm16_request_for_cut` / `flac_request_for_cut` accept, with no transforms of its own and 1 <= R <= REVERB_MAX_RIR
+    samples, at `sampling_rate` (the cut's).  None otherwise: the RIR generator, several RIR channels (a MultiCut), other
+    formats, longer RIRs, an RIR at another rate (lhotse convolves it as it is stored; this route does not take it)."""
+    from lhotse import Recording
+    from lhotse.cut import MonoCut
+
+    from .engine import REVERB_MAX_RIR
+
+    if t.rir is None or len(t.rir_channels) != 1:
+        return None
+    try:
+        rir = t.rir.to_cut() if isinstance(t.rir, Recording) else t.rir
+        rir = rir.with_channels(list(t.rir_channels))
+        if t.early_only:
+            rir = rir.truncate(duration=0.05)
+    except Exception:  # lhotse would raise on the float route too
+        return None
+    if not isinstance(rir, MonoCut) or getattr(rir, "tracks", None) is not None or rir.sampling_rate != sampling_rate:
+        return None
+    src = pcm16_request_for_cut(rir) or flac_request_for_cut(rir)
+    if src is None or not 1 <= src.num_samples <= REVERB_MAX_RIR:
+        return None
+    return ReverbRequest(rir=src, normalize=bool(t.normalize_output))
 
 
 def _samples(seconds: float, sr: int) -> int:
     return int(math.floor(round(seconds * sr, 8) + 0.5))  # lhotse's compute_num_samples
 
 
-def transform_request_for_cut(cut) -> Optional[TransformRequest]:
+def transform_request_for_cut(cut, reverb: bool = False) -> Optional[TransformRequest]:
     """What `cut.load_audio()` (audio/recording.py load_audio) amounts to for a MonoCut over a single-channel 16-bit WAV or
     FLAC file whose recording carries a non-empty chain of Speed, Volume and Resample transforms: the source slice (the
     transforms' own reverse_timestamps applied to the cut's range, a read to the end of the file when the cut's duration is
     within 1 ms of the recording's), the chain, and the cut's length.  None when not eligible: another kind of cut or
     transform, a Resample lhotse would not run through its torch resampler (sox backend, no torchaudio), a resampling stage
     whose padded input is too short for oneDNN, oneDNN off, a rate pair whose probe fails, or a length outside lhotse's
-    duration-mismatch tolerance."""
+    duration-mismatch tolerance.
+
+    `reverb=True` also takes a chain whose last transform is a ReverbWithImpulseResponse that `reverb_request` accepts (a
+    reverb alone included): the stages before it write the pre-reverb signal, and the reverb kernel (csrc/reverb.cuh) writes
+    the cut, within a float32 tolerance of a float64 convolution rather than bit for bit (DESIGN.md §3.1j).  Off by default
+    so that existing callers keep exactly the routes and samples they have."""
     try:
+        from lhotse.augmentation.rir import ReverbWithImpulseResponse
         from lhotse.audio.resampling_backend import get_current_resampling_backend
         from lhotse.audio.utils import get_audio_duration_mismatch_tolerance
         from lhotse.augmentation import torchaudio as lta
@@ -992,6 +1084,12 @@ def transform_request_for_cut(cut) -> Optional[TransformRequest]:
     if torch.get_default_dtype() != torch.float32:
         return None  # lhotse's table phases and output lengths are evaluated in the default dtype
     tfs = [t if isinstance(t, AudioTransform) else AudioTransform.from_dict(t) for t in rec.transforms]
+    rv = None
+    if reverb and type(tfs[-1]) is ReverbWithImpulseResponse:
+        rv = reverb_request(tfs[-1], rec.sampling_rate)
+        if rv is None:
+            return None
+        tfs = tfs[:-1]
     if any(type(t) not in (lta.Speed, lta.Volume, lta.Resample) for t in tfs):
         return None
     sources = rec.sources or []
@@ -1046,26 +1144,27 @@ def transform_request_for_cut(cut) -> Optional[TransformRequest]:
     if abs(diff) > int(math.ceil(get_audio_duration_mismatch_tolerance() * sr)) or diff > L - 1:
         return None
     return TransformRequest(source=make(path=h.path, first_sample=first, num_samples=n), ops=tuple(ops), num_samples=target,
-                            sampling_rate=int(sr))
+                            sampling_rate=int(sr), reverb=rv)
 
 
 def _has_transforms(cut) -> bool:
     return bool(getattr(getattr(cut, "recording", None), "transforms", None))
 
 
-def transform_requests_for_batch(cuts) -> Optional[List[TransformRequest]]:
+def transform_requests_for_batch(cuts, reverb: bool = False) -> Optional[List[TransformRequest]]:
     """The "transform" route's requests for a batch: no MixedCut, every cut a plain 16-bit WAV / FLAC slice or an eligible
-    transformed MonoCut, and at least one of the latter (batches of plain slices keep their routes).  None otherwise."""
+    transformed MonoCut, and at least one of the latter (batches of plain slices keep their routes).  None otherwise.
+    `reverb=True`: see `transform_request_for_cut`."""
     if any(getattr(c, "tracks", None) is not None for c in cuts) or not any(_has_transforms(c) for c in cuts):
         return None
-    reqs = [_transform_or_plain_request(c) for c in cuts]
+    reqs = [_transform_or_plain_request(c, reverb) for c in cuts]
     return None if any(r is None for r in reqs) else reqs
 
 
-def _transform_or_plain_request(cut) -> Optional[TransformRequest]:
+def _transform_or_plain_request(cut, reverb: bool = False) -> Optional[TransformRequest]:
     """transform_request_for_cut, or a plain 16-bit WAV / FLAC slice as an empty chain (a copy of x = q / 32768)."""
     if _has_transforms(cut):
-        r = transform_request_for_cut(cut)
+        r = transform_request_for_cut(cut, reverb=reverb)
     else:
         src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
         r = (TransformRequest(source=src, ops=(), num_samples=int(src.num_samples), sampling_rate=int(cut.sampling_rate))
@@ -1106,6 +1205,42 @@ class TransformBatch:
     lens: List[int]
     offsets: List[int]
     out_elems: int
+    reverb_rirs: Optional[np.ndarray] = None  # engine.REVERB_RIR_DTYPE: the batch's distinct RIRs in the two int16 sources
+    reverb_cuts: Optional[np.ndarray] = None  # engine.REVERB_CUT_DTYPE: the reverberated cuts, reading `mid`
+
+
+def _stage_rirs(reqs, wav: list, flac: list) -> Tuple[List[object], List[Tuple[int, int]]]:
+    """The distinct RIRs of `reqs` (objects with a `reverb` field) appended to the WAV / FLAC source lists, so that they cross
+    with the batch's own samples: (the RIR reads in order, (source, index in its list) of each)."""
+    rirs, at = [], {}
+    for r in reqs:
+        rv = getattr(r, "reverb", None)
+        if rv is not None and rv.rir not in at:
+            lst, k = (wav, 0) if isinstance(rv.rir, PcmRequest) else (flac, 1)
+            at[rv.rir] = (k, len(lst))
+            lst.append(rv.rir)
+            rirs.append(rv.rir)
+    return rirs, [at[r] for r in rirs]
+
+
+def _reverb_tables(rirs, where, rir_elem, cuts) -> Tuple[np.ndarray, np.ndarray]:
+    """The b200feat_reverb tables: RIR i in source where[i][0] at rir_elem[i]; cuts = [(ReverbRequest, in_elem, in_len,
+    out_elem, target_len)]."""
+    from .engine import REVERB_CUT_DTYPE, REVERB_RIR_DTYPE
+
+    rt = np.zeros(len(rirs), dtype=REVERB_RIR_DTYPE)
+    rt["struct_size"] = REVERB_RIR_DTYPE.itemsize
+    rt["source"] = [k for k, _ in where]
+    rt["src_elem"] = rir_elem
+    rt["num_samples"] = [r.num_samples for r in rirs]
+    ix = {r: i for i, r in enumerate(rirs)}
+    ct = np.zeros(len(cuts), dtype=REVERB_CUT_DTYPE)
+    ct["struct_size"] = REVERB_CUT_DTYPE.itemsize
+    ct["rir"] = [ix[rv.rir] for rv, *_ in cuts]
+    ct["normalize"] = [int(rv.normalize) for rv, *_ in cuts]
+    for name, col in zip(("in_elem", "in_len", "out_elem", "target_len"), range(1, 5)):
+        ct[name] = [c[col] for c in cuts]
+    return rt, ct
 
 
 class TransformStagingRing(_PinnedRing):
@@ -1148,17 +1283,23 @@ class TransformStagingRing(_PinnedRing):
         kind = np.asarray([0 if isinstance(r.source, PcmRequest) else 1 for r in requests], dtype=np.int32)
         src_elem = np.zeros(len(requests), dtype=np.int64)
         pcm_buf, flac_batch = None, None
-        if (kind == 0).any():
-            pcm_buf, offs0 = self._stage_wav([r.source for r, k in zip(requests, kind) if k == 0], executor)
-            src_elem[kind == 0] = offs0
-        if (kind == 1).any():
-            flac_batch, _, offs1, _ = self.flac.stage([r.source for r, k in zip(requests, kind) if k == 1], executor=executor)
-            src_elem[kind == 1] = offs1
+        wav = [r.source for r, k in zip(requests, kind) if k == 0]
+        flac = [r.source for r, k in zip(requests, kind) if k == 1]
+        nwav, nflac = len(wav), len(flac)
+        rirs, where = _stage_rirs(requests, wav, flac)
+        offs0 = offs1 = []
+        if wav:
+            pcm_buf, offs0 = self._stage_wav(wav, executor)
+            src_elem[kind == 0] = offs0[:nwav]
+        if flac:
+            flac_batch, _, offs1, _ = self.flac.stage(flac, executor=executor)
+            src_elem[kind == 1] = offs1[:nflac]
         srs = {r.sampling_rate for r in requests}
         lens = [int(r.num_samples) for r in requests]
         offs, out_elems = _aligned_offsets(lens, self.ALIGN)
         pairs, pair_ix = [], {}
         rows = []  # (depth, cut, table pair, source, in_elem, in_len, target, out_elem, out_len, target_len, scale_in, scale_out)
+        rv_cuts = []  # (ReverbRequest, in_elem, in_len, out_elem, target_len)
         mid = 0
         for i, r in enumerate(requests):
             chain = _chain_stages(r.ops)
@@ -1173,11 +1314,14 @@ class TransformStagingRing(_PinnedRing):
                     N, O, _, _ = _resample_geometry(*pair)
                     n_out = resampled_len(N, L, O)
                 last = d == len(chain) - 1
-                out_elem = offs[i] if last else mid
-                rows.append((d, i, pi, source, in_elem, L, RESAMPLE_TO_OUT if last else RESAMPLE_TO_MID, out_elem, n_out,
-                             lens[i] if last else n_out, s_in, s_out))
-                if not last:
+                to_out = last and r.reverb is None  # a reverberated cut's last stage writes the pre-reverb signal into `mid`
+                out_elem = offs[i] if to_out else mid
+                rows.append((d, i, pi, source, in_elem, L, RESAMPLE_TO_OUT if to_out else RESAMPLE_TO_MID, out_elem, n_out,
+                             lens[i] if to_out else n_out, s_in, s_out))
+                if not to_out:
                     mid += n_out
+                if last and r.reverb is not None:
+                    rv_cuts.append((r.reverb, out_elem, n_out, offs[i], lens[i]))
                 source, in_elem, L = RESAMPLE_MID, out_elem, n_out
         rows.sort(key=lambda row: (row[0], row[1]))
         nb = len(rows) * RESAMPLE_STAGE_DTYPE.itemsize
@@ -1192,15 +1336,18 @@ class TransformStagingRing(_PinnedRing):
         st["reserved"] = 0
         batch = TransformBatch(pcm=pcm_buf, flac=flac_batch, stages=st, pair=np.asarray(cols[2], dtype=np.int64), pairs=pairs,
                                mid_elems=mid, lens=lens, offsets=offs, out_elems=out_elems)
+        if rv_cuts:
+            rir_elem = [offs0[j] if k == 0 else offs1[j] for k, j in where]
+            batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(rirs, where, rir_elem, rv_cuts)
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
 
 
 def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] = None,
                      handle=None) -> Tuple[torch.Tensor, List[int], List[int]]:
     """The device half of the "transform" route on the current stream: the rate pairs' tables (built and uploaded once per
-    device), H2D of the WAV slices, the FLAC decode (if any), the resampling stages; then `ring`'s copies are marked in flight.
-    Returns (float32 samples on `device`, lengths, offsets)."""
-    from .engine import resample, resample_table
+    device), H2D of the WAV slices, the FLAC decode (if any), the resampling stages, the reverb (if any); then `ring`'s copies
+    are marked in flight.  Returns (float32 samples on `device`, lengths, offsets)."""
+    from .engine import resample, resample_table, reverb
 
     device = torch.device(device)
     with torch.cuda.device(device):
@@ -1212,19 +1359,23 @@ def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] 
         mid = torch.empty(batch.mid_elems, dtype=torch.float32, device=device) if batch.mid_elems else None
         out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
         resample(src0, src1, mid, batch.stages, out, handle)
+        if batch.reverb_cuts is not None:
+            reverb(src0, src1, mid, batch.reverb_rirs, batch.reverb_cuts, out, handle)
         if ring is not None:
             ring.mark_in_flight(device)
     return out, batch.lens, batch.offsets
 
 
-def transform_cuts(cuts, device="cuda", executor=None,
-                   ring: Optional[TransformStagingRing] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
+def transform_cuts(cuts, device="cuda", executor=None, ring: Optional[TransformStagingRing] = None,
+                   reverb: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
     """Loads speed-perturbed, volume-perturbed and resampled cuts (and plain 16-bit WAV / FLAC slices) with the transforms run
     on the GPU: (float32 device tensor holding every cut's samples at its offset, on 4-sample boundaries, lengths, offsets),
-    each cut bit-identical to float32(cut.load_audio()).  Raises ValueError naming the first cut the route cannot take."""
+    each cut bit-identical to float32(cut.load_audio()).  Raises ValueError naming the first cut the route cannot take.
+    `reverb=True` also takes chains that end in a ReverbWithImpulseResponse with a recorded RIR, reverberated on the GPU
+    within a float32 tolerance of a float64 convolution (see `transform_request_for_cut`; off by default)."""
     reqs = []
     for c in cuts:
-        r = _transform_or_plain_request(c)
+        r = _transform_or_plain_request(c, reverb)
         if r is None:
             raise ValueError(f"cut {getattr(c, 'id', c)!r} cannot be loaded on the GPU (see transform_request_for_cut)")
         reqs.append(r)

@@ -226,6 +226,7 @@ def compute_and_store_features_fused(
     overwrite: bool = False,
     pcm16_fast_path: bool = True,
     perturbed_tracks: bool = False,
+    reverb: bool = False,
 ):
     """`CutSet.compute_and_store_features_batch(extractor, storage_path, manifest_path, batch_duration, num_workers,
     overwrite=...)` (lhotse/cut/set.py:2197-2408) with the batch kept whole from the GPU to the disk: one packed
@@ -238,7 +239,10 @@ def compute_and_store_features_fused(
 
     `perturbed_tracks=True` lets the "mix" stage also take MixedCuts whose tracks carry Speed / Volume / Resample chains
     (`pcm_staging.mix_request_for_cut`).  It is off by default so that existing calls keep exactly their routes, until H100
-    measurements of it decide the default."""
+    measurements of it decide the default.  `reverb=True` lets the "transform" and "mix" stages also take cuts reverberated
+    with a recorded RIR (`pcm_staging.transform_request_for_cut`, `mix_request_for_cut`); off by default because those
+    samples match the float route within a float32 tolerance, not bit for bit (the float route's own convolution is not
+    bit-reproducible), until H100 measurements of it decide the default."""
     import json
     import queue
     import threading
@@ -334,10 +338,10 @@ def compute_and_store_features_fused(
                     reqs = [flac_request_for_cut(c) for c in batch_cuts]
                 if not all(r is not None for r in reqs):
                     kind, free = "mix", mix_rings
-                    reqs = mix_requests_for_batch(batch_cuts, perturbed_tracks=perturbed_tracks) or [None]
+                    reqs = mix_requests_for_batch(batch_cuts, perturbed_tracks=perturbed_tracks, reverb=reverb) or [None]
                 if not all(r is not None for r in reqs):
                     kind, free = "transform", transform_rings
-                    reqs = transform_requests_for_batch(batch_cuts) or [None]
+                    reqs = transform_requests_for_batch(batch_cuts, reverb=reverb) or [None]
                 if all(r is not None for r in reqs):
                     ring = free.get()  # handed back by stage 2 once the batch's host-to-device copy has completed
                     staged, lens, offs, fsr = ring.stage(reqs, executor=pool)
