@@ -444,6 +444,45 @@ int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_el
                     const b200feat_reverb_cut *cuts, int32_t ncuts, float *out_dev, int64_t out_elems, void *work_dev,
                     int64_t work_bytes, void *stream);
 
+/*
+ * SpecAugment on a padded (B, T, F) float32 feature batch on the GPU: what lhotse's SpecAugment.forward computes from the
+ * same random draws (DESIGN.md §3.1k).  The host draws the numbers and hands over two tables: the time warps (bicubic along
+ * time, within a float32 tolerance of lhotse's F.interpolate) and the mask rectangles, which are filled with the mean of the
+ * sequence's whole warped (T, F) matrix.  Everything outside warped segments and masks is copied bit for bit.
+ */
+#define B200FEAT_SPECAUG_TIME 0     /* b200feat_specaug_mask.axis: frames [start, end) of every feature bin */
+#define B200FEAT_SPECAUG_FEATURE 1  /* feature bins [start, end) of every frame */
+
+typedef struct b200feat_specaug_warp {
+  int32_t struct_size;   /* sizeof(b200feat_specaug_warp) — ABI guard, in every record */
+  int32_t seq;           /* sequence index, in [0, B) */
+  int32_t start;         /* first frame of the segment; the segments of one sequence must not overlap */
+  int32_t len;           /* its frames: [start, start + len) inside [0, T) */
+  int32_t center;        /* 0 < center < len: input frames [0, center) of the segment ... */
+  int32_t warped;        /* 0 < warped < len: ... become its output frames [0, warped), the rest the rest */
+} b200feat_specaug_warp;
+
+typedef struct b200feat_specaug_mask {
+  int32_t struct_size;   /* sizeof(b200feat_specaug_mask) */
+  int32_t seq;           /* sequence index, in [0, B) */
+  int32_t axis;          /* B200FEAT_SPECAUG_TIME | B200FEAT_SPECAUG_FEATURE */
+  int32_t start;         /* 0 <= start <= end <= T (time) or F (feature) */
+  int32_t end;
+  int32_t reserved;
+} b200feat_specaug_mask;
+
+/* Device scratch b200feat_specaug needs (0 when an argument is out of range). */
+int64_t b200feat_specaug_work_bytes(int32_t B, int32_t T, int32_t F, int32_t nwarps, int32_t nmasks);
+
+/* Checks the host tables (sequence indices, every segment inside [0, T) with 0 < center, warped < len, the segments of a
+ * sequence disjoint, every rectangle inside its axis with start <= end, in_dev != out_dev, T * F < 2^31), copies them to
+ * `work_dev` and launches the warp-and-copy, mean and mask-fill kernels, asynchronously on `stream`: three launches whatever
+ * B is.  `in_dev` is read only; every element of `out_dev` is written.  Results are identical from run to run.  Errors are
+ * reported through `h` (b200feat_last_error) when it is not NULL, and through b200feat_global_error. */
+int b200feat_specaug(b200feat_handle *h, const float *in_dev, float *out_dev, int32_t B, int32_t T, int32_t F,
+                     const b200feat_specaug_warp *warps, int32_t nwarps, const b200feat_specaug_mask *masks, int32_t nmasks,
+                     void *work_dev, int64_t work_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

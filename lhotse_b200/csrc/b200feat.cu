@@ -29,6 +29,7 @@
 #include "mix.cuh"
 #include "resample.cuh"
 #include "reverb.cuh"
+#include "specaug.cuh"
 
 namespace {
 
@@ -1241,6 +1242,125 @@ int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_el
   CU_TRY(h, cudaGetLastError());
   const int64_t gx = std::min<int64_t>((longest + 4 * RV_OUT_THREADS - 1) / (4 * RV_OUT_THREADS), 1024);
   reverb_out_kernel<<<dim3((unsigned)gx, (unsigned)ncuts), RV_OUT_THREADS, 0, st>>>(d_cuts, d_gain);
+  CU_TRY(h, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The SpecAugment work buffer: the tables the kernels read (one copy), then the per-CTA partial sums and the means
+struct SaLayout {
+  int64_t warp_begin, warps, masks, tables_end, partial, mean, total;
+  int64_t tiles;
+};
+
+SaLayout sa_layout(int32_t B, int32_t T, int32_t F, int32_t nwarps, int32_t nmasks) {
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  SaLayout l{};
+  l.tiles = sa_tiles(T, F);
+  l.warp_begin = 0;
+  l.warps = l.warp_begin + up(((int64_t)B + 1) * 4);
+  l.masks = l.warps + up((int64_t)nwarps * (int64_t)sizeof(SaWarp));
+  l.tables_end = l.masks + up((int64_t)nmasks * (int64_t)sizeof(SaMask));
+  l.partial = l.tables_end;
+  l.mean = l.partial + up((int64_t)B * l.tiles * 8);
+  l.total = l.mean + up((int64_t)B * 4);
+  return l;
+}
+
+bool sa_shape_ok(int32_t B, int32_t T, int32_t F) {
+  return B >= 1 && T >= 1 && F >= 1 && (int64_t)T * F <= 0x7fffffff && (int64_t)B * sa_tiles(T, F) <= 0x7fffffff;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t b200feat_specaug_work_bytes(int32_t B, int32_t T, int32_t F, int32_t nwarps, int32_t nmasks) {
+  if (!sa_shape_ok(B, T, F) || nwarps < 0 || nmasks < 0) return 0;
+  return sa_layout(B, T, F, nwarps, nmasks).total;
+}
+
+int b200feat_specaug(b200feat_handle *h, const float *in_dev, float *out_dev, int32_t B, int32_t T, int32_t F,
+                     const b200feat_specaug_warp *warps, int32_t nwarps, const b200feat_specaug_mask *masks, int32_t nmasks,
+                     void *work_dev, int64_t work_bytes, void *stream) {
+  if (!in_dev || !out_dev || !work_dev || nwarps < 0 || nmasks < 0 || (nwarps > 0 && !warps) || (nmasks > 0 && !masks))
+    return fail(h, B200FEAT_EINVAL, "specaug: bad arguments");
+  if (!sa_shape_ok(B, T, F)) return fail(h, B200FEAT_EINVAL, "specaug: B, T, F must be positive, T * F and the CTA count below 2^31");
+  if (nmasks > 0x7fffffff / 2) return fail(h, B200FEAT_EINVAL, "specaug: too many masks in one call");
+  {  // the warp reads rows of `in` that other CTAs have already overwritten in `out` if the two share memory
+    const uintptr_t a = (uintptr_t)in_dev, b = (uintptr_t)out_dev, bytes = (uintptr_t)B * T * F * sizeof(float);
+    if (a < b + bytes && b < a + bytes) return fail(h, B200FEAT_EINVAL, "specaug: the output overlaps the input");
+  }
+  const SaLayout l = sa_layout(B, T, F, nwarps, nmasks);
+  if (work_bytes < l.total) return fail(h, B200FEAT_EINVAL, "specaug: work buffer too small");
+  auto where = [](const char *what, int64_t i) { return std::string("specaug: ") + what + " " + std::to_string(i) + ": "; };
+  std::vector<int32_t> order((size_t)nwarps);
+  for (int32_t i = 0; i < nwarps; ++i) {
+    const b200feat_specaug_warp &w = warps[i];
+    if (w.struct_size != (int32_t)sizeof(b200feat_specaug_warp))
+      return fail(h, B200FEAT_EINVAL, where("warp", i) + "b200feat_specaug_warp size mismatch (ABI)");
+    if (w.seq < 0 || w.seq >= B) return fail(h, B200FEAT_EINVAL, where("warp", i) + "sequence index out of range");
+    if (w.start < 0 || w.len < 1 || w.start > T - w.len) return fail(h, B200FEAT_EINVAL, where("warp", i) + "segment outside [0, T)");
+    if (w.center < 1 || w.center >= w.len || w.warped < 1 || w.warped >= w.len)
+      return fail(h, B200FEAT_EINVAL, where("warp", i) + "center and warped must lie in (0, len)");
+    order[i] = i;
+  }
+  std::sort(order.begin(), order.end(), [&](int32_t a, int32_t b) {
+    return warps[a].seq != warps[b].seq ? warps[a].seq < warps[b].seq : warps[a].start != warps[b].start ? warps[a].start < warps[b].start : a < b;
+  });
+  for (int32_t k = 1; k < nwarps; ++k) {
+    const b200feat_specaug_warp &p = warps[order[k - 1]], &w = warps[order[k]];
+    if (p.seq == w.seq && w.start < p.start + p.len)
+      return fail(h, B200FEAT_EINVAL, where("warp", order[k]) + "overlaps another segment of its sequence");
+  }
+  for (int32_t i = 0; i < nmasks; ++i) {
+    const b200feat_specaug_mask &m = masks[i];
+    if (m.struct_size != (int32_t)sizeof(b200feat_specaug_mask))
+      return fail(h, B200FEAT_EINVAL, where("mask", i) + "b200feat_specaug_mask size mismatch (ABI)");
+    if (m.seq < 0 || m.seq >= B) return fail(h, B200FEAT_EINVAL, where("mask", i) + "sequence index out of range");
+    if (m.axis != B200FEAT_SPECAUG_TIME && m.axis != B200FEAT_SPECAUG_FEATURE) return fail(h, B200FEAT_EINVAL, where("mask", i) + "bad axis");
+    if (m.start < 0 || m.start > m.end || m.end > (m.axis == B200FEAT_SPECAUG_TIME ? T : F))
+      return fail(h, B200FEAT_EINVAL, where("mask", i) + "rectangle outside its axis");
+  }
+  // the kernels' tables in one host block: segments per sequence sorted by start, rectangles as they came
+  std::vector<char> tables((size_t)l.tables_end, 0);
+  int32_t *warp_begin = (int32_t *)(tables.data() + l.warp_begin);
+  SaWarp *sw = (SaWarp *)(tables.data() + l.warps);
+  SaMask *sm = (SaMask *)(tables.data() + l.masks);
+  for (int32_t k = 0; k < nwarps; ++k) {
+    const b200feat_specaug_warp &w = warps[order[k]];
+    sw[k] = SaWarp{w.start, w.len, w.center, w.warped};
+    ++warp_begin[w.seq + 1];
+  }
+  for (int32_t b = 0; b < B; ++b) warp_begin[b + 1] += warp_begin[b];
+  int64_t largest = 0;
+  for (int32_t i = 0; i < nmasks; ++i) {
+    sm[i] = SaMask{masks[i].seq, masks[i].axis, masks[i].start, masks[i].end};
+    largest = std::max<int64_t>(largest, sa_mask_elems(sm[i], T, F));
+  }
+  char *w = (char *)work_dev;
+  const cudaStream_t st = (cudaStream_t)stream;
+  double *d_partial = (double *)(w + l.partial);
+  float *d_mean = (float *)(w + l.mean);
+  // a pageable copy: the call returns once the block has been staged, so it may go when this function returns
+  CU_TRY(h, cudaMemcpyAsync(w, tables.data(), tables.size(), cudaMemcpyHostToDevice, st));
+  const unsigned ctas = (unsigned)((int64_t)B * l.tiles);
+  // 128-bit accesses need whole rows of float4 at 16-byte addresses
+  if (F % 4 == 0 && (uintptr_t)in_dev % 16 == 0 && (uintptr_t)out_dev % 16 == 0)
+    specaug_warp_kernel<4><<<ctas, SA_THREADS, 0, st>>>(in_dev, out_dev, T, F, (int)l.tiles, (const SaWarp *)(w + l.warps),
+                                                        (const int32_t *)(w + l.warp_begin), d_partial);
+  else
+    specaug_warp_kernel<1><<<ctas, SA_THREADS, 0, st>>>(in_dev, out_dev, T, F, (int)l.tiles, (const SaWarp *)(w + l.warps),
+                                                        (const int32_t *)(w + l.warp_begin), d_partial);
+  CU_TRY(h, cudaGetLastError());
+  if (nmasks == 0) return B200FEAT_OK;
+  specaug_mean_kernel<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(d_partial, B, (int)l.tiles, (int64_t)T * F, d_mean);
+  CU_TRY(h, cudaGetLastError());
+  const int64_t gy = std::min<int64_t>(std::max<int64_t>((largest + 8 * SA_FILL_THREADS - 1) / (8 * SA_FILL_THREADS), 1), 64);
+  specaug_fill_kernel<<<dim3((unsigned)nmasks, (unsigned)gy), SA_FILL_THREADS, 0, st>>>(out_dev, T, F, (const SaMask *)(w + l.masks), d_mean);
   CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }

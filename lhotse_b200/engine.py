@@ -94,6 +94,13 @@ REVERB_CUT_DTYPE = np.dtype([("struct_size", "<i4"), ("rir", "<i4"), ("normalize
                              ("in_len", "<i8"), ("out_elem", "<i8"), ("target_len", "<i8")])
 REVERB_MAX_RIR = 65536  # B200FEAT_REVERB_MAX_RIR
 
+# b200feat_specaug_warp / b200feat_specaug_mask as numpy record layouts
+SPECAUG_WARP_DTYPE = np.dtype([("struct_size", "<i4"), ("seq", "<i4"), ("start", "<i4"), ("len", "<i4"), ("center", "<i4"),
+                               ("warped", "<i4")])
+SPECAUG_MASK_DTYPE = np.dtype([("struct_size", "<i4"), ("seq", "<i4"), ("axis", "<i4"), ("start", "<i4"), ("end", "<i4"),
+                               ("reserved", "<i4")])
+SPECAUG_TIME, SPECAUG_FEATURE = 0, 1
+
 
 EXPORTS = [
     "b200feat_version", "b200feat_global_error", "b200feat_create", "b200feat_destroy",
@@ -103,7 +110,7 @@ EXPORTS = [
     "b200feat_get_table", "b200feat_get_stats", "b200feat_set_output_affine", "b200feat_extract_host_ptrs",
     "b200feat_flac_index", "b200feat_flac_decode", "b200feat_mix_work_bytes", "b200feat_mix",
     "b200feat_resample_table", "b200feat_resample_work_bytes", "b200feat_resample", "b200feat_mix_ex",
-    "b200feat_reverb_work_bytes", "b200feat_reverb",
+    "b200feat_reverb_work_bytes", "b200feat_reverb", "b200feat_specaug_work_bytes", "b200feat_specaug",
 ]
 
 
@@ -183,6 +190,10 @@ def load_library():
         lib.b200feat_reverb_work_bytes.argtypes = [vp, i32, vp, i32]
         lib.b200feat_reverb.restype = C.c_int
         lib.b200feat_reverb.argtypes = [vp, vp, i64, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
+        lib.b200feat_specaug_work_bytes.restype = i64
+        lib.b200feat_specaug_work_bytes.argtypes = [i32, i32, i32, i32, i32]
+        lib.b200feat_specaug.restype = C.c_int
+        lib.b200feat_specaug.argtypes = [vp, vp, vp, i32, i32, i32, vp, i32, vp, i32, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -329,6 +340,27 @@ def reverb(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], x: torch.
     with torch.cuda.device(out.device):
         rc = lib.b200feat_reverb(handle, p0, n0, p1, n1, px, nx, rirs.ctypes.data, len(rirs), cuts.ctypes.data, len(cuts),
                                  out.data_ptr(), out.numel(), work.data_ptr(), work.numel(), stream)
+    if rc != 0:
+        _raise(lib, rc, handle)
+
+
+def specaug(x: torch.Tensor, out: torch.Tensor, warps: np.ndarray, masks: np.ndarray, handle=None) -> None:
+    """Launches `b200feat_specaug` on the current stream of `out`'s device (asynchronous, no synchronisation): `x` and `out`
+    are contiguous float32 (B, T, F) device tensors that share no memory, `warps` / `masks` the host tables
+    (SPECAUG_WARP_DTYPE / SPECAUG_MASK_DTYPE; copied before this returns).  Raises B200FeatError when the library refuses
+    the tables."""
+    lib = load_library()
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    assert warps.dtype == SPECAUG_WARP_DTYPE and masks.dtype == SPECAUG_MASK_DTYPE
+    assert x.dtype == torch.float32 and out.dtype == torch.float32 and x.dim() == 3 and x.shape == out.shape
+    assert x.is_contiguous() and out.is_contiguous() and x.device == out.device
+    warps, masks = np.ascontiguousarray(warps), np.ascontiguousarray(masks)
+    B, T, F = x.shape
+    nbytes = int(lib.b200feat_specaug_work_bytes(B, T, F, len(warps), len(masks)))
+    work = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=out.device)
+    with torch.cuda.device(out.device):
+        rc = lib.b200feat_specaug(handle, x.data_ptr(), out.data_ptr(), B, T, F, warps.ctypes.data, len(warps),
+                                  masks.ctypes.data, len(masks), work.data_ptr(), work.numel(), stream)
     if rc != 0:
         _raise(lib, rc, handle)
 
