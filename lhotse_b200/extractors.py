@@ -34,7 +34,7 @@ import torch
 
 from .base import FeatureExtractor, register_extractor
 from .engine import OUT_PADDED, Engine, pack_device
-from .pcm_staging import FlacBatch, MixBatch, TransformBatch, decode_staged, mix_staged, transform_staged
+from .pcm_staging import is_staged_batch, staged_to_device
 from .plan import EPSILON, LOG_EPSILON, FeaturePlan, build_plan
 
 Seconds = float
@@ -273,21 +273,14 @@ class _B200Extractor(FeatureExtractor):
     def _extract_on_device(self, buf: torch.Tensor, lens: Sequence[int], offsets: Sequence[int],
                            engine: Optional[Engine] = None, ring=None, **kw):
         """Moves a staged 1-D batch to the engine's device (then marks `ring`'s copy in flight), adds the dither there and
-        runs the kernels: (features, row prefix) of `Engine.extract_device`.  A staged FLAC batch (`pcm_staging.FlacBatch`)
-        crosses compressed and is decoded on the device into the int16 ragged buffer first, on the same stream; a staged mix
-        batch (`pcm_staging.MixBatch`) is mixed on the device into a float32 ragged buffer first, and a staged transform batch
-        (`pcm_staging.TransformBatch`) is resampled and scaled there."""
+        runs the kernels: (features, row prefix) of `Engine.extract_device`.  A staged FLAC, mix or transform batch of
+        `pcm_staging` is decoded, mixed or resampled on the device into a ragged buffer first, on the same stream
+        (`pcm_staging.staged_to_device`)."""
         eng = engine or self.engine
-        if isinstance(buf, FlacBatch):
-            buf, lens, offsets = decode_staged(buf, eng.device, ring)
-        elif isinstance(buf, MixBatch):
-            buf, lens, offsets = mix_staged(buf, eng.device, ring, handle=eng._h)
-        elif isinstance(buf, TransformBatch):
-            buf, lens, offsets = transform_staged(buf, eng.device, ring, handle=eng._h)
-        else:
-            buf = buf.to(eng.device, non_blocking=True)
-            if ring is not None:
-                ring.mark_in_flight(eng.device)
+        # only the mix and transform stages use the library handle; an engine stand-in without one still takes raw buffers
+        buf, staged_lens, staged_offsets = staged_to_device(buf, eng.device, ring, handle=getattr(eng, "_h", None))
+        if staged_lens is not None:
+            lens, offsets = staged_lens, staged_offsets
         return eng.extract_device(self._dithered(buf), list(lens), offsets=list(offsets), **kw)
 
     def _extract_list_on_device(self, samples: Sequence[ArrayLike], engine: Optional[Engine] = None, **kw):
@@ -447,7 +440,7 @@ class _B200Extractor(FeatureExtractor):
         """`extract_batch_padded` for a batch that already sits in ONE (pinned) host buffer — e.g. the int16 PCM ring of
         `lhotse_b200.pcm_staging` (SURVEY.md §8f-2): one H2D copy of the raw bytes, one launch, features stay on the device."""
         self._check_sr(sampling_rate)
-        assert isinstance(staged, (FlacBatch, MixBatch, TransformBatch)) or (staged.dim() == 1 and staged.dtype in (torch.int16, torch.float32))
+        assert is_staged_batch(staged) or (staged.dim() == 1 and staged.dtype in (torch.int16, torch.float32))
         out, prefix = self._extract_on_device(staged, lens, offsets, engine, ring, out_mode=OUT_PADDED, pad_value=padding_value)
         return out, torch.from_numpy(np.diff(prefix)).to(torch.int64)
 

@@ -70,10 +70,7 @@ class FusedOnTheFlyFeatures:
         self.pcm16_fast_path = pcm16_fast_path and hasattr(extractor, "extract_staged_padded")
         self.perturbed_tracks = perturbed_tracks
         self.reverb = reverb
-        self._ring = None
-        self._flac_ring = None
-        self._mix_ring = None
-        self._transform_ring = None
+        self._rings = {}  # route -> its staging ring, made when a batch first takes the route
         self.last_batch_route = None  # "pcm16" | "flac" | "mix" | "transform" | "float" (introspection for tests / logs)
         self._executor_type = executor_type
         self._executor = None
@@ -103,111 +100,36 @@ class FusedOnTheFlyFeatures:
             self._executor = self._executor_type(max_workers=self.num_workers)
         return self._executor
 
-    def _try_pcm16(self, cuts, recording_field):
+    def _try_staged(self, cuts, recording_field):
         """(route, (features, lengths)) of a staged route, or None: the float route takes the batch."""
         if not self.pcm16_fast_path or self.wave_transforms or self.return_audio or recording_field is not None:
             return None
-        from .pcm_staging import pcm16_request_for_cut
+        from .pcm_staging import new_ring, staged_route
 
-        if len({c.sampling_rate for c in cuts}) != 1:
-            return None  # mixed sampling rates: grouped by the float route
-        if any(getattr(c, "tracks", None) is not None for c in cuts):
-            return self._try_mix(cuts)
-        if any(getattr(getattr(c, "recording", None), "transforms", None) for c in cuts):
-            return self._try_transform(cuts)
-        reqs = []
-        for c in cuts:
-            r = pcm16_request_for_cut(c)
-            if r is None:
-                return self._try_flac(cuts)
-            reqs.append(r)
-        return "pcm16", self._stage_pcm16(cuts, reqs)
-
-    def _try_flac(self, cuts):
-        from .pcm_staging import FlacStagingRing, flac_request_for_cut
-
-        reqs = []
-        for c in cuts:
-            r = flac_request_for_cut(c)
-            if r is None:
-                return None  # not every cut is a FLAC slice (e.g. a WAV / FLAC mix): the float route
-            reqs.append(r)
-        if self._flac_ring is None:
-            self._flac_ring = FlacStagingRing()
-        try:  # a frame that does not decode raises ValueError from the decode, before any feature is handed back
-            staged, lens, offs, sr = self._flac_ring.stage(reqs, executor=self._get_executor())
-            if sr != cuts[0].sampling_rate:
-                return None
-            out = self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON, ring=self._flac_ring,
-                                                       **({"engine": self._mvn_engine} if self._mvn_engine is not None else {}))
-        except (OSError, ValueError):
-            if self.fault_tolerant:
-                return None  # the float route knows how to skip broken cuts
-            raise
-        return "flac", out
-
-    def _try_mix(self, cuts):
-        from .pcm_staging import MixStagingRing, mix_requests_for_batch
-
-        reqs = mix_requests_for_batch(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb)
-        if reqs is None:
-            return None  # a cut the mix route cannot take: the float route
-        if self._mix_ring is None:
-            self._mix_ring = MixStagingRing()
+        chosen = staged_route(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb)
+        if chosen is None:
+            return None  # mixed sampling rates (grouped by the float route) or a cut no staged route takes
+        route, reqs = chosen
+        ring = self._rings.get(route)
+        if ring is None:
+            ring = self._rings[route] = new_ring(route)
         try:  # a FLAC frame that does not decode raises ValueError before any feature is handed back
-            staged, lens, offs, sr = self._mix_ring.stage(reqs, executor=self._get_executor())
+            staged, lens, offs, sr = ring.stage(reqs, executor=self._get_executor())
             if sr != cuts[0].sampling_rate:
                 return None
-            out = self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON, ring=self._mix_ring,
+            out = self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON, ring=ring,
                                                        **({"engine": self._mvn_engine} if self._mvn_engine is not None else {}))
         except (OSError, ValueError):
             if self.fault_tolerant:
                 return None  # the float route knows how to skip broken cuts
             raise
-        return "mix", out
-
-    def _try_transform(self, cuts):
-        from .pcm_staging import TransformStagingRing, transform_requests_for_batch
-
-        reqs = transform_requests_for_batch(cuts, reverb=self.reverb)
-        if reqs is None:
-            return None  # a cut the transform route cannot take: the float route
-        if self._transform_ring is None:
-            self._transform_ring = TransformStagingRing()
-        try:  # a FLAC frame that does not decode raises ValueError before any feature is handed back
-            staged, lens, offs, sr = self._transform_ring.stage(reqs, executor=self._get_executor())
-            if sr != cuts[0].sampling_rate:
-                return None
-            out = self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON,
-                                                       ring=self._transform_ring,
-                                                       **({"engine": self._mvn_engine} if self._mvn_engine is not None else {}))
-        except (OSError, ValueError):
-            if self.fault_tolerant:
-                return None  # the float route knows how to skip broken cuts
-            raise
-        return "transform", out
-
-    def _stage_pcm16(self, cuts, reqs):
-        from .pcm_staging import PcmStagingRing
-
-        if self._ring is None:
-            self._ring = PcmStagingRing()
-        try:
-            staged, lens, offs, sr = self._ring.stage(reqs, executor=self._get_executor())
-        except (OSError, ValueError):
-            if self.fault_tolerant:
-                return None  # the float route knows how to skip broken cuts
-            raise
-        if sr != cuts[0].sampling_rate:
-            return None
-        return self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON, ring=self._ring,
-                                                    **({"engine": self._mvn_engine} if self._mvn_engine is not None else {}))
+        return route, out
 
     def __call__(self, cuts, recording_field: Optional[str] = None):
         from lhotse.dataset.collation import collate_vectors, read_audio_from_cuts
 
-        fast = self._try_pcm16(cuts, recording_field)
-        if fast is not None and fast[1] is not None:
+        fast = self._try_staged(cuts, recording_field)
+        if fast is not None:
             self.last_batch_route, (feats, feat_lens) = fast
             if not self.features_on_device:
                 feats = feats.cpu()

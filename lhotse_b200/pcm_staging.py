@@ -10,13 +10,18 @@ ragged buffer (no float copy on the host), cross PCIe as 2 bytes per sample and 
 
   * `WavPcm16.open(path)`        minimal RIFF/WAVE reader (PCM or EXTENSIBLE/PCM, 16 bit, any channel count)
   * `PcmStagingRing`             grow-only pinned int16 buffer; `stage(requests)` fills it back to back
-  * `pcm16_request_for_cut(cut)` the (path, first sample, sample count, channel) of a lhotse MonoCut when it is eligible
-                                 (one "file" source, .wav, no augmentation transforms); None otherwise
-  * `FlacStream`, `FlacStagingRing`, `flac_request_for_cut`, `decode_flac`: the same for 16-bit FLAC files, whose frames
-                                 cross PCIe compressed and are decoded by the sm_90a kernel of csrc/flac.cuh
+  * `slice_request_for_cut(cut)` the (path, first sample, sample count, channel) of a lhotse MonoCut when it is a plain
+                                 slice (one "file" source, no augmentation transforms) of a 16-bit .wav (`PcmRequest`) or
+                                 .flac (`FlacRequest`) file; None otherwise.  `pcm16_request_for_cut` / `flac_request_for_cut`
+                                 take one of the two kinds
+  * `FlacStream`, `FlacStagingRing`, `decode_flac`: 16-bit FLAC files, whose frames cross PCIe compressed and are decoded by
+                                 the sm_90a kernel of csrc/flac.cuh
   * `mix_request_for_cut`, `MixStagingRing`, `mix_cuts`: MixedCuts of such slices, mixed by csrc/mix.cuh
   * `transform_request_for_cut`, `TransformStagingRing`, `transform_cuts`: speed / volume perturbed and resampled slices, the
                                  transforms run by csrc/resample.cuh
+The mix and transform rings stage their int16 sources (WAV and FLAC slices, RIRs) through one `_SourceRing`.
+`staged_route(cuts)` picks the route of a batch (one of `STAGED_ROUTES`) with its requests, `new_ring(route)` makes the ring
+that stages them, and `staged_to_device` runs the device half of any staged batch.
 Everything here is host-side I/O; the arithmetic stays in the CUDA kernels.
 """
 from __future__ import annotations
@@ -250,11 +255,26 @@ def _for_each(n: int, one, executor) -> None:
 
 
 @dataclass(frozen=True)
-class PcmRequest:
+class _SliceRequest:
     path: str
     first_sample: int
     num_samples: int
     channel: int = 0
+
+
+@dataclass(frozen=True)
+class PcmRequest(_SliceRequest):
+    """Samples [first_sample, first_sample + num_samples) of `channel` of a 16-bit PCM WAV file."""
+
+
+def _samples(seconds: float, sr: int) -> int:
+    return int(math.floor(round(seconds * sr, 8) + 0.5))  # lhotse's compute_num_samples
+
+
+def _one_rate(srs) -> int:
+    if len(srs) != 1:
+        raise ValueError(f"one sampling rate per batch expected, got {sorted(srs)}")
+    return next(iter(srs))
 
 
 class _PinnedRing:
@@ -303,6 +323,11 @@ class PcmStagingRing(_PinnedRing):
     ALIGN = 4
 
     def stage(self, requests: Sequence[PcmRequest], executor=None) -> Tuple[torch.Tensor, List[int], List[int], int]:
+        buf, lens, offs, srs = self._fill(requests, executor)
+        return buf, lens, offs, _one_rate(srs)
+
+    def _fill(self, requests: Sequence[PcmRequest], executor=None) -> Tuple[torch.Tensor, List[int], List[int], set]:
+        """`stage` without the one-rate check: (buffer view, lengths, offsets, the files' sampling rates)."""
         self._wait_idle()
         lens = [int(r.num_samples) for r in requests]
         offs, total = _aligned_offsets(lens, self.ALIGN)
@@ -318,36 +343,7 @@ class PcmStagingRing(_PinnedRing):
             h.read_into(view[offs[i]: offs[i] + lens[i]], r.first_sample, r.channel)
 
         _for_each(len(requests), one, executor)
-        if len(srs) != 1:
-            raise ValueError(f"one sampling rate per batch expected, got {sorted(srs)}")
-        return self._buf[:total], lens, offs, srs.pop()
-
-
-def pcm16_request_for_cut(cut) -> Optional[PcmRequest]:
-    """The raw-PCM read that `cut.load_audio()` amounts to (cut/data.py + audio/recording.py:load_audio with
-    offset = cut.start, duration = cut.duration), when it is nothing but a slice of one 16-bit PCM WAV file:
-    a MonoCut over a single-source "file" recording with no augmentation transforms.  None when not eligible."""
-    rec = getattr(cut, "recording", None)
-    if rec is None or getattr(cut, "tracks", None) is not None or getattr(rec, "transforms", None):
-        return None
-    sources = getattr(rec, "sources", None) or []
-    if len(sources) != 1 or sources[0].type != "file" or not str(sources[0].source).lower().endswith(".wav"):
-        return None
-    ch = cut.channel
-    if not isinstance(ch, int) or ch not in sources[0].channels:
-        return None
-    try:
-        h = WavPcm16.open_cached(str(sources[0].source))
-    except (NotPcm16Wav, OSError):
-        return None
-    if h.sampling_rate != cut.sampling_rate or h.channels != len(sources[0].channels):
-        return None
-    # seconds -> samples as lhotse does (utils.py compute_num_samples: round half up after an 8-digit rounding)
-    first = int(math.floor(round(cut.start * h.sampling_rate, 8) + 0.5))
-    n = int(cut.num_samples)
-    if first + n > h.num_samples:
-        return None
-    return PcmRequest(path=h.path, first_sample=first, num_samples=n, channel=sources[0].channels.index(ch))
+        return self._buf[:total], lens, offs, srs
 
 
 # ---- FLAC ----------------------------------------------------------------------------------------------------------
@@ -398,11 +394,8 @@ class FlacStream:
 
 
 @dataclass(frozen=True)
-class FlacRequest:
-    path: str
-    first_sample: int
-    num_samples: int
-    channel: int = 0
+class FlacRequest(_SliceRequest):
+    """Samples [first_sample, first_sample + num_samples) of `channel` of a 16-bit FLAC file."""
 
 
 @dataclass
@@ -538,29 +531,97 @@ def decode_flac(requests: Sequence[FlacRequest], device="cuda", executor=None,
     return decode_staged(batch, device, ring)
 
 
-def flac_request_for_cut(cut) -> Optional[FlacRequest]:
-    """`pcm16_request_for_cut` for a slice of one 16-bit FLAC file: same eligibility (a MonoCut over a single-source "file"
-    recording with no transforms) and the same seconds -> samples arithmetic.  None when not eligible."""
+def _open_slice_file(path) -> Optional[Tuple[object, type]]:
+    """The cached header of a 16-bit file chosen by its extension, with the request class that reads it: (WavPcm16,
+    PcmRequest) for .wav, (FlacStream, FlacRequest) for .flac; None for another extension or a file the reader refuses."""
+    path = str(path)
+    try:
+        if path.lower().endswith(".wav"):
+            return WavPcm16.open_cached(path), PcmRequest
+        if path.lower().endswith(".flac"):
+            return FlacStream.open_cached(path), FlacRequest
+    except (NotPcm16Wav, NotFlac16, OSError):
+        pass
+    return None
+
+
+def slice_request_for_cut(cut) -> Optional[_SliceRequest]:
+    """The raw read that `cut.load_audio()` amounts to (cut/data.py + audio/recording.py:load_audio with offset = cut.start,
+    duration = cut.duration), when it is nothing but a slice of one 16-bit PCM WAV file (a PcmRequest) or one 16-bit FLAC
+    file (a FlacRequest): a MonoCut over a single-source "file" recording with no augmentation transforms.  None when not
+    eligible."""
     rec = getattr(cut, "recording", None)
     if rec is None or getattr(cut, "tracks", None) is not None or getattr(rec, "transforms", None):
         return None
     sources = getattr(rec, "sources", None) or []
-    if len(sources) != 1 or sources[0].type != "file" or not str(sources[0].source).lower().endswith(".flac"):
+    if len(sources) != 1 or sources[0].type != "file":
         return None
     ch = cut.channel
     if not isinstance(ch, int) or ch not in sources[0].channels:
         return None
-    try:
-        s = FlacStream.open_cached(str(sources[0].source))
-    except (NotFlac16, OSError):
+    opened = _open_slice_file(sources[0].source)
+    if opened is None:
         return None
-    if s.sampling_rate != cut.sampling_rate or s.channels != len(sources[0].channels):
+    h, make = opened
+    if h.sampling_rate != cut.sampling_rate or h.channels != len(sources[0].channels):
         return None
-    first = int(math.floor(round(cut.start * s.sampling_rate, 8) + 0.5))
+    first = _samples(cut.start, h.sampling_rate)
     n = int(cut.num_samples)
-    if first + n > s.num_samples:
+    if first + n > h.num_samples:
         return None
-    return FlacRequest(path=s.path, first_sample=first, num_samples=n, channel=sources[0].channels.index(ch))
+    return make(path=h.path, first_sample=first, num_samples=n, channel=sources[0].channels.index(ch))
+
+
+def pcm16_request_for_cut(cut) -> Optional[PcmRequest]:
+    """`slice_request_for_cut` for a slice of one 16-bit PCM WAV file; None otherwise."""
+    r = slice_request_for_cut(cut)
+    return r if isinstance(r, PcmRequest) else None
+
+
+def flac_request_for_cut(cut) -> Optional[FlacRequest]:
+    """`slice_request_for_cut` for a slice of one 16-bit FLAC file; None otherwise."""
+    r = slice_request_for_cut(cut)
+    return r if isinstance(r, FlacRequest) else None
+
+
+class _SourceRing(_PinnedRing):
+    """The int16 sources of a mix or transform batch: the WAV reads through a PcmStagingRing (files of any rate), the FLAC
+    reads through a FlacStagingRing.  `stage(reads)` returns (pinned int16 view or None, FlacBatch or None, the source of
+    each read: 0 WAV / 1 FLAC, the element offset of each read in its source, (the set of the WAV files' rates, the set of
+    the FLAC batch's rate: None when the FLAC files have several))."""
+
+    def __init__(self, pin_memory: Optional[bool] = None):
+        super().__init__(pin_memory)
+        self.pcm = PcmStagingRing(initial_samples=1 << 20, pin_memory=self._pin)
+        self.flac = FlacStagingRing(initial_bytes=1 << 16, pin_memory=self._pin)
+
+    def mark_in_flight(self, device=None) -> None:
+        super().mark_in_flight(device)
+        self.pcm.mark_in_flight(device)
+        self.flac.mark_in_flight(device)
+
+    def stage(self, reads: Sequence[_SliceRequest], executor=None):
+        kind = np.asarray([0 if isinstance(r, PcmRequest) else 1 for r in reads], dtype=np.int32)
+        elem = np.zeros(len(reads), dtype=np.int64)
+        wav = [r for r, k in zip(reads, kind) if k == 0]
+        flac = [r for r, k in zip(reads, kind) if k == 1]
+        pcm_buf, flac_batch, wav_srs, flac_srs = None, None, set(), set()
+        if wav:
+            pcm_buf, _, offs, wav_srs = self.pcm._fill(wav, executor)
+            elem[kind == 0] = offs
+        if flac:
+            flac_batch, _, offs, sr = self.flac.stage(flac, executor=executor)
+            elem[kind == 1] = offs
+            flac_srs = {sr}
+        return pcm_buf, flac_batch, kind, elem, (wav_srs, flac_srs)
+
+
+def _sources_to_device(batch, device) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+    """The device half of `_SourceRing.stage` for a batch with its `pcm` / `flac` fields: (the WAV reads' int16 H2D copy,
+    the FLAC reads' decode), each None when the batch has no such read."""
+    src0 = batch.pcm.to(device, non_blocking=True) if batch.pcm is not None else None
+    src1 = decode_staged(batch.flac, device)[0] if batch.flac is not None else None
+    return src0, src1
 
 
 # ---- MixedCut ------------------------------------------------------------------------------------------------------
@@ -655,7 +716,7 @@ def mix_request_for_cut(cut, perturbed_tracks: bool = False, reverb: bool = Fals
             if perturbed_tracks and _has_transforms(c):
                 src = transform_request_for_cut(c)  # num_samples: the chain's output after lhotse's length fix
             else:
-                src = pcm16_request_for_cut(c) or flac_request_for_cut(c)
+                src = slice_request_for_cut(c)
             if src is None:
                 return None
             n = src.num_samples
@@ -706,7 +767,7 @@ def _plain_mix_request(cut, perturbed_tracks: bool = False, reverb: bool = False
     if perturbed_tracks and _has_transforms(cut):
         src = transform_request_for_cut(cut, reverb=reverb)
     else:
-        src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
+        src = slice_request_for_cut(cut)
     if src is None or src.num_samples <= 0:
         return None
     return MixRequest(tracks=(MixTrackRequest(src, int(src.num_samples), 0, float("nan"), MIX_ROLE_MIXED),), ref=0,
@@ -754,23 +815,21 @@ class MixBatch:
 
 
 class MixStagingRing(_PinnedRing):
-    """A PcmStagingRing, a FlacStagingRing and pinned table bytes for one mix batch, plus a TransformStagingRing for the
+    """A _SourceRing for the int16 tracks, pinned table bytes for one mix batch, plus a TransformStagingRing for the
     perturbed tracks (made when a batch first has one); `stage(requests)` returns (MixBatch, lengths, offsets, sampling rate),
-    the rate None when the tracks have several."""
+    the rate None when the tracks have several.  WAV tracks of several rates raise ValueError."""
 
     ALIGN = 4
 
     def __init__(self, pin_memory: Optional[bool] = None):
         super().__init__(pin_memory)
-        self.pcm = PcmStagingRing(initial_samples=1 << 20, pin_memory=self._pin)
-        self.flac = FlacStagingRing(initial_bytes=1 << 16, pin_memory=self._pin)
+        self.sources = _SourceRing(pin_memory=self._pin)
         self.transform: Optional[TransformStagingRing] = None
         self._tables = torch.empty(1 << 16, dtype=torch.uint8, pin_memory=self._pin)
 
     def mark_in_flight(self, device=None) -> None:
         super().mark_in_flight(device)
-        self.pcm.mark_in_flight(device)
-        self.flac.mark_in_flight(device)
+        self.sources.mark_in_flight(device)
         if self.transform is not None:
             self.transform.mark_in_flight(device)
 
@@ -779,25 +838,20 @@ class MixStagingRing(_PinnedRing):
 
         self._wait_idle()
         flat = [t for r in requests for t in r.tracks]
-        kind = np.asarray([-1 if t.source is None else 0 if isinstance(t.source, PcmRequest) else
-                           MIX_SRC_F32 if isinstance(t.source, TransformRequest) else 1 for t in flat], dtype=np.int32)
-        wav = [t.source for t, k in zip(flat, kind) if k == 0]
-        flac = [t.source for t, k in zip(flat, kind) if k == 1]
-        nwav, nflac = len(wav), len(flac)
-        perturbed = [t.source for t, k in zip(flat, kind) if k == MIX_SRC_F32]
-        srs = set()
-        pcm_buf, flac_batch, transform_batch = None, None, None
+        ints = [i for i, t in enumerate(flat) if isinstance(t.source, _SliceRequest)]
+        perturbed = [t.source for t in flat if isinstance(t.source, TransformRequest)]
+        # the RIRs are at the cut's rate (reverb_request), so one rate per WAV batch still holds
+        rirs = _stage_rirs(requests)
+        pcm_buf, flac_batch, read_kind, read_elem, (wav_srs, flac_srs) = self.sources.stage(
+            [flat[i].source for i in ints] + rirs, executor=executor)
+        if wav_srs:
+            _one_rate(wav_srs)
+        srs = wav_srs | flac_srs
+        kind = np.asarray([-1 if t.source is None else MIX_SRC_F32 for t in flat], dtype=np.int32)
         src_elem = np.zeros(len(flat), dtype=np.int64)
-        rirs, where = _stage_rirs(requests, wav, flac)  # at the cut's rate (reverb_request), so one rate per ring still holds
-        offs0 = offs1 = []
-        if wav:
-            pcm_buf, _, offs0, sr0 = self.pcm.stage(wav, executor=executor)
-            src_elem[kind == 0] = offs0[:nwav]
-            srs.add(sr0)
-        if flac:
-            flac_batch, _, offs1, sr1 = self.flac.stage(flac, executor=executor)
-            src_elem[kind == 1] = offs1[:nflac]
-            srs.add(sr1)
+        kind[ints] = read_kind[: len(ints)]
+        src_elem[ints] = read_elem[: len(ints)]
+        transform_batch = None
         if perturbed:
             if self.transform is None:
                 self.transform = TransformStagingRing(pin_memory=self._pin)
@@ -840,10 +894,10 @@ class MixStagingRing(_PinnedRing):
         batch = MixBatch(pcm=pcm_buf, flac=flac_batch, tracks=tracks, cuts=cuts, lens=lens, offsets=offs, out_elems=out_elems,
                          transform=transform_batch)
         if rv_ix:
-            rir_elem = [offs0[j] if k == 0 else offs1[j] for k, j in where]
             batch.pre_elems = base - out_elems + pre_elems
             batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(
-                rirs, where, rir_elem, [(requests[i].reverb, mix_out[i], lens[i], offs[i], lens[i]) for i in rv_ix])
+                rirs, read_kind[len(ints):], read_elem[len(ints):],
+                [(requests[i].reverb, mix_out[i], lens[i], offs[i], lens[i]) for i in rv_ix])
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
 
 
@@ -856,8 +910,7 @@ def mix_staged(batch: MixBatch, device, ring: Optional[_PinnedRing] = None, hand
 
     device = torch.device(device)
     with torch.cuda.device(device):
-        src0 = batch.pcm.to(device, non_blocking=True) if batch.pcm is not None else None
-        src1 = decode_staged(batch.flac, device)[0] if batch.flac is not None else None
+        src0, src1 = _sources_to_device(batch, device)
         src2 = transform_staged(batch.transform, device, handle=handle)[0] if batch.transform is not None else None
         out = torch.zeros(max(batch.out_elems + batch.pre_elems, 1), dtype=torch.float32, device=device)
         mix(src0, src1, batch.tracks, batch.cuts, out, handle, src2=src2)
@@ -878,15 +931,22 @@ def mix_cuts(cuts, device="cuda", executor=None, ring: Optional[MixStagingRing] 
     default, so that existing callers keep their behaviour until H100 measurements of the route exist).  `reverb=True` also
     takes MixedCut-level reverbs and plain slices whose only transform is a reverb, reverberated on the GPU within a float32
     tolerance of a float64 convolution (see `mix_request_for_cut`; off by default)."""
-    reqs = []
-    for c in cuts:
-        r = _mix_or_plain_request(c, perturbed_tracks, reverb)
-        if r is None:
-            raise ValueError(f"cut {getattr(c, 'id', c)!r} cannot be mixed on the GPU (see mix_request_for_cut)")
-        reqs.append(r)
+    reqs = _requests_or_raise(cuts, lambda c: _mix_or_plain_request(c, perturbed_tracks, reverb),
+                              "cannot be mixed on the GPU (see mix_request_for_cut)")
     ring = ring or MixStagingRing()
     batch, _, _, _ = ring.stage(reqs, executor=executor)
     return mix_staged(batch, device, ring)
+
+
+def _requests_or_raise(cuts, request, refusal: str) -> list:
+    """[request(cut) for cut in cuts]; ValueError naming the first cut for which `request` returns None."""
+    reqs = []
+    for c in cuts:
+        r = request(c)
+        if r is None:
+            raise ValueError(f"cut {getattr(c, 'id', c)!r} {refusal}")
+        reqs.append(r)
+    return reqs
 
 
 # ---- Speed / Volume / Resample transforms ---------------------------------------------------------------------------
@@ -1044,14 +1104,10 @@ def reverb_request(t, sampling_rate: int) -> Optional[ReverbRequest]:
         return None
     if not isinstance(rir, MonoCut) or getattr(rir, "tracks", None) is not None or rir.sampling_rate != sampling_rate:
         return None
-    src = pcm16_request_for_cut(rir) or flac_request_for_cut(rir)
+    src = slice_request_for_cut(rir)
     if src is None or not 1 <= src.num_samples <= REVERB_MAX_RIR:
         return None
     return ReverbRequest(rir=src, normalize=bool(t.normalize_output))
-
-
-def _samples(seconds: float, sr: int) -> int:
-    return int(math.floor(round(seconds * sr, 8) + 0.5))  # lhotse's compute_num_samples
 
 
 def transform_request_for_cut(cut, reverb: bool = False) -> Optional[TransformRequest]:
@@ -1095,18 +1151,10 @@ def transform_request_for_cut(cut, reverb: bool = False) -> Optional[TransformRe
     sources = rec.sources or []
     if len(sources) != 1 or sources[0].type != "file" or list(sources[0].channels) != [cut.channel]:
         return None
-    path = str(sources[0].source)
-    try:
-        if path.lower().endswith(".wav"):
-            h, make = WavPcm16.open_cached(path), PcmRequest
-        elif path.lower().endswith(".flac"):
-            h, make = FlacStream.open_cached(path), FlacRequest
-        else:
-            return None
-    except (NotPcm16Wav, NotFlac16, OSError):
+    opened = _open_slice_file(sources[0].source)
+    if opened is None or opened[0].channels != 1:
         return None
-    if h.channels != 1:
-        return None
+    h, make = opened
     sr = rec.sampling_rate
     offset, duration = cut.start, cut.duration
     if math.isclose(duration, rec.duration, abs_tol=1e-3):
@@ -1166,7 +1214,7 @@ def _transform_or_plain_request(cut, reverb: bool = False) -> Optional[Transform
     if _has_transforms(cut):
         r = transform_request_for_cut(cut, reverb=reverb)
     else:
-        src = pcm16_request_for_cut(cut) or flac_request_for_cut(cut)
+        src = slice_request_for_cut(cut)
         r = (TransformRequest(source=src, ops=(), num_samples=int(src.num_samples), sampling_rate=int(cut.sampling_rate))
              if src is not None else None)
     return r if r is not None and r.num_samples > 0 else None
@@ -1209,28 +1257,25 @@ class TransformBatch:
     reverb_cuts: Optional[np.ndarray] = None  # engine.REVERB_CUT_DTYPE: the reverberated cuts, reading `mid`
 
 
-def _stage_rirs(reqs, wav: list, flac: list) -> Tuple[List[object], List[Tuple[int, int]]]:
-    """The distinct RIRs of `reqs` (objects with a `reverb` field) appended to the WAV / FLAC source lists, so that they cross
-    with the batch's own samples: (the RIR reads in order, (source, index in its list) of each)."""
-    rirs, at = [], {}
+def _stage_rirs(reqs) -> List[_SliceRequest]:
+    """The distinct RIR reads of `reqs` (objects with a `reverb` field) in order of first use, to be staged after the batch's
+    own reads so that they cross with its samples."""
+    rirs = {}
     for r in reqs:
         rv = getattr(r, "reverb", None)
-        if rv is not None and rv.rir not in at:
-            lst, k = (wav, 0) if isinstance(rv.rir, PcmRequest) else (flac, 1)
-            at[rv.rir] = (k, len(lst))
-            lst.append(rv.rir)
-            rirs.append(rv.rir)
-    return rirs, [at[r] for r in rirs]
+        if rv is not None:
+            rirs.setdefault(rv.rir, None)
+    return list(rirs)
 
 
-def _reverb_tables(rirs, where, rir_elem, cuts) -> Tuple[np.ndarray, np.ndarray]:
-    """The b200feat_reverb tables: RIR i in source where[i][0] at rir_elem[i]; cuts = [(ReverbRequest, in_elem, in_len,
+def _reverb_tables(rirs, source, rir_elem, cuts) -> Tuple[np.ndarray, np.ndarray]:
+    """The b200feat_reverb tables: RIR i in int16 source source[i] at rir_elem[i]; cuts = [(ReverbRequest, in_elem, in_len,
     out_elem, target_len)]."""
     from .engine import REVERB_CUT_DTYPE, REVERB_RIR_DTYPE
 
     rt = np.zeros(len(rirs), dtype=REVERB_RIR_DTYPE)
     rt["struct_size"] = REVERB_RIR_DTYPE.itemsize
-    rt["source"] = [k for k, _ in where]
+    rt["source"] = source
     rt["src_elem"] = rir_elem
     rt["num_samples"] = [r.num_samples for r in rirs]
     ix = {r: i for i, r in enumerate(rirs)}
@@ -1244,56 +1289,28 @@ def _reverb_tables(rirs, where, rir_elem, cuts) -> Tuple[np.ndarray, np.ndarray]
 
 
 class TransformStagingRing(_PinnedRing):
-    """A pinned int16 buffer for the WAV slices, a FlacStagingRing and pinned table bytes for one transform batch;
-    `stage(requests)` returns (TransformBatch, lengths, offsets, the cuts' sampling rate), the rate None when the cuts have
-    several."""
+    """A _SourceRing for the source slices (files of several rates allowed: a Resample chain starts at its file's own rate)
+    and pinned table bytes for one transform batch; `stage(requests)` returns (TransformBatch, lengths, offsets, the cuts'
+    sampling rate), the rate None when the cuts have several."""
 
     ALIGN = 4
 
     def __init__(self, pin_memory: Optional[bool] = None):
         super().__init__(pin_memory)
-        self._pcm = torch.empty(1 << 20, dtype=torch.int16, pin_memory=self._pin)
-        self.flac = FlacStagingRing(initial_bytes=1 << 16, pin_memory=self._pin)
+        self.sources = _SourceRing(pin_memory=self._pin)
         self._tables = torch.empty(1 << 16, dtype=torch.uint8, pin_memory=self._pin)
 
     def mark_in_flight(self, device=None) -> None:
         super().mark_in_flight(device)
-        self.flac.mark_in_flight(device)
-
-    def _stage_wav(self, requests: Sequence[PcmRequest], executor) -> Tuple[torch.Tensor, List[int]]:
-        """The WAV slices back to back on 4-sample boundaries, as PcmStagingRing lays them out, but from files of any rate
-        (a Resample chain starts at its file's own rate): (pinned int16 view, offsets)."""
-        lens = [int(r.num_samples) for r in requests]
-        offs, total = _aligned_offsets(lens, self.ALIGN)
-        self._pcm = self._grown(self._pcm, total)
-        view = self._pcm.numpy()
-        _zero_gaps(view, lens, offs)
-
-        def one(i):
-            r = requests[i]
-            WavPcm16.open_cached(r.path).read_into(view[offs[i]: offs[i] + lens[i]], r.first_sample, r.channel)
-
-        _for_each(len(requests), one, executor)
-        return self._pcm[:total], offs
+        self.sources.mark_in_flight(device)
 
     def stage(self, requests: Sequence[TransformRequest], executor=None) -> Tuple[TransformBatch, List[int], List[int], Optional[int]]:
         from .engine import RESAMPLE_MID, RESAMPLE_STAGE_DTYPE, RESAMPLE_TO_MID, RESAMPLE_TO_OUT
 
         self._wait_idle()
-        kind = np.asarray([0 if isinstance(r.source, PcmRequest) else 1 for r in requests], dtype=np.int32)
-        src_elem = np.zeros(len(requests), dtype=np.int64)
-        pcm_buf, flac_batch = None, None
-        wav = [r.source for r, k in zip(requests, kind) if k == 0]
-        flac = [r.source for r, k in zip(requests, kind) if k == 1]
-        nwav, nflac = len(wav), len(flac)
-        rirs, where = _stage_rirs(requests, wav, flac)
-        offs0 = offs1 = []
-        if wav:
-            pcm_buf, offs0 = self._stage_wav(wav, executor)
-            src_elem[kind == 0] = offs0[:nwav]
-        if flac:
-            flac_batch, _, offs1, _ = self.flac.stage(flac, executor=executor)
-            src_elem[kind == 1] = offs1[:nflac]
+        B = len(requests)
+        rirs = _stage_rirs(requests)
+        pcm_buf, flac_batch, kind, src_elem, _ = self.sources.stage([r.source for r in requests] + rirs, executor=executor)
         srs = {r.sampling_rate for r in requests}
         lens = [int(r.num_samples) for r in requests]
         offs, out_elems = _aligned_offsets(lens, self.ALIGN)
@@ -1337,8 +1354,7 @@ class TransformStagingRing(_PinnedRing):
         batch = TransformBatch(pcm=pcm_buf, flac=flac_batch, stages=st, pair=np.asarray(cols[2], dtype=np.int64), pairs=pairs,
                                mid_elems=mid, lens=lens, offsets=offs, out_elems=out_elems)
         if rv_cuts:
-            rir_elem = [offs0[j] if k == 0 else offs1[j] for k, j in where]
-            batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(rirs, where, rir_elem, rv_cuts)
+            batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(rirs, kind[B:], src_elem[B:], rv_cuts)
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
 
 
@@ -1354,8 +1370,7 @@ def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] 
         ids = np.asarray([resample_table(a, b, *resample_kernel(a, b), device, handle) for a, b in batch.pairs] + [-1],
                          dtype=np.int32)
         batch.stages["table"] = ids[batch.pair]  # pair -1 picks the trailing -1
-        src0 = batch.pcm.to(device, non_blocking=True) if batch.pcm is not None else None
-        src1 = decode_staged(batch.flac, device)[0] if batch.flac is not None else None
+        src0, src1 = _sources_to_device(batch, device)
         mid = torch.empty(batch.mid_elems, dtype=torch.float32, device=device) if batch.mid_elems else None
         out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
         resample(src0, src1, mid, batch.stages, out, handle)
@@ -1373,12 +1388,62 @@ def transform_cuts(cuts, device="cuda", executor=None, ring: Optional[TransformS
     each cut bit-identical to float32(cut.load_audio()).  Raises ValueError naming the first cut the route cannot take.
     `reverb=True` also takes chains that end in a ReverbWithImpulseResponse with a recorded RIR, reverberated on the GPU
     within a float32 tolerance of a float64 convolution (see `transform_request_for_cut`; off by default)."""
-    reqs = []
-    for c in cuts:
-        r = _transform_or_plain_request(c, reverb)
-        if r is None:
-            raise ValueError(f"cut {getattr(c, 'id', c)!r} cannot be loaded on the GPU (see transform_request_for_cut)")
-        reqs.append(r)
+    reqs = _requests_or_raise(cuts, lambda c: _transform_or_plain_request(c, reverb),
+                              "cannot be loaded on the GPU (see transform_request_for_cut)")
     ring = ring or TransformStagingRing()
     batch, _, _, _ = ring.stage(reqs, executor=executor)
     return transform_staged(batch, device, ring)
+
+
+# ---- One entry point per step for the callers ----------------------------------------------------------------------
+
+STAGED_ROUTES = ("pcm16", "flac", "mix", "transform")
+
+
+def staged_route(cuts, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[Tuple[str, list]]:
+    """(route, requests) of the staged route that takes the batch, the route one of STAGED_ROUTES; None when the cuts have
+    more than one sampling rate or no staged route takes them.  A batch with a MixedCut can only go to "mix", else one with
+    recording transforms only to "transform"; a batch of plain slices goes to "pcm16" when they are all WAV, to "flac" when
+    they are all FLAC.  `perturbed_tracks` and `reverb`: see `mix_request_for_cut` and `transform_request_for_cut`."""
+    if len({c.sampling_rate for c in cuts}) != 1:
+        return None
+    if any(getattr(c, "tracks", None) is not None for c in cuts):
+        route, reqs = "mix", mix_requests_for_batch(cuts, perturbed_tracks=perturbed_tracks, reverb=reverb)
+    elif any(_has_transforms(c) for c in cuts):
+        route, reqs = "transform", transform_requests_for_batch(cuts, reverb=reverb)
+    else:
+        reqs = [slice_request_for_cut(c) for c in cuts]
+        route = {PcmRequest: "pcm16", FlacRequest: "flac"}.get(type(reqs[0]))
+        if any(type(r) is not type(reqs[0]) for r in reqs):
+            reqs = None
+    return None if route is None or reqs is None else (route, reqs)
+
+
+def new_ring(route: str, pin_memory: Optional[bool] = None) -> _PinnedRing:
+    """A new ring that stages the requests of `route` (one of STAGED_ROUTES), with that ring's default sizes."""
+    return {"pcm16": PcmStagingRing, "flac": FlacStagingRing, "mix": MixStagingRing,
+            "transform": TransformStagingRing}[route](pin_memory=pin_memory)
+
+
+def is_staged_batch(staged) -> bool:
+    """Whether `staged` is a batch that `staged_to_device` runs through a device stage (FLAC decode, mix or transforms)
+    rather than a raw int16 / float32 buffer that it only copies."""
+    return isinstance(staged, (FlacBatch, MixBatch, TransformBatch))
+
+
+def staged_to_device(staged, device, ring: Optional[_PinnedRing] = None,
+                     handle=None) -> Tuple[torch.Tensor, Optional[List[int]], Optional[List[int]]]:
+    """The device half of any staged route on the current stream, then `ring`'s copies are marked in flight: a raw int16 or
+    float32 buffer is copied as it is, a FlacBatch / MixBatch / TransformBatch goes through `decode_staged` / `mix_staged` /
+    `transform_staged`.  Returns (buffer on `device`, lengths, offsets); a raw buffer's lengths and offsets are None (the
+    caller has them)."""
+    if isinstance(staged, FlacBatch):
+        return decode_staged(staged, device, ring)
+    if isinstance(staged, MixBatch):
+        return mix_staged(staged, device, ring, handle=handle)
+    if isinstance(staged, TransformBatch):
+        return transform_staged(staged, device, ring, handle=handle)
+    buf = staged.to(device, non_blocking=True)
+    if ring is not None:
+        ring.mark_in_flight(device)
+    return buf, None, None

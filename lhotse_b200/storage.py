@@ -256,8 +256,7 @@ def compute_and_store_features_fused(
     from lhotse.qa import validate_features
     from lhotse.utils import fastcopy
 
-    from .pcm_staging import (FlacStagingRing, MixStagingRing, PcmStagingRing, TransformStagingRing, flac_request_for_cut,
-                              mix_requests_for_batch, pcm16_request_for_cut, transform_requests_for_batch)
+    from .pcm_staging import STAGED_ROUTES, new_ring, staged_route
 
     register_with_lhotse()
     frame_shift = extractor.frame_shift
@@ -302,11 +301,8 @@ def compute_and_store_features_fused(
                 cuts_writer.write(m)
 
     failure = []  # first exception of a helper thread, re-raised by the caller
-    rings = queue.Queue()
-    flac_rings = queue.Queue()  # the same hand-back protocol for batches of 16-bit FLAC slices (decoded on the GPU)
-    mix_rings = queue.Queue()  # ... and for batches with MixedCuts of such slices (mixed on the GPU)
-    transform_rings = queue.Queue()  # ... and for batches with speed / volume / resample transforms (run on the GPU)
-    free_rings = {"pcm": rings, "flac": flac_rings, "mix": mix_rings, "transform": transform_rings}
+    # the free rings of each staged route: stage 1 takes one per batch, stage 2 hands it back once its H2D copy has completed
+    free_rings = {route: queue.Queue() for route in STAGED_ROUTES}
     stop = threading.Event()
     cuda_index = None  # the GPU this call works on, resolved in the calling thread ("cuda" without an index = its current device)
     try:
@@ -330,25 +326,16 @@ def compute_and_store_features_fused(
             sr = batch_cuts[0].sampling_rate
             assert all(c.sampling_rate == sr for c in batch_cuts)
             item = None
-            if use_ring:
-                kind, free = "pcm", rings
-                reqs = [pcm16_request_for_cut(c) for c in batch_cuts]
-                if not all(r is not None for r in reqs):
-                    kind, free = "flac", flac_rings
-                    reqs = [flac_request_for_cut(c) for c in batch_cuts]
-                if not all(r is not None for r in reqs):
-                    kind, free = "mix", mix_rings
-                    reqs = mix_requests_for_batch(batch_cuts, perturbed_tracks=perturbed_tracks, reverb=reverb) or [None]
-                if not all(r is not None for r in reqs):
-                    kind, free = "transform", transform_rings
-                    reqs = transform_requests_for_batch(batch_cuts, reverb=reverb) or [None]
-                if all(r is not None for r in reqs):
-                    ring = free.get()  # handed back by stage 2 once the batch's host-to-device copy has completed
-                    staged, lens, offs, fsr = ring.stage(reqs, executor=pool)
-                    if fsr == sr:
-                        item = (kind, batch_cuts, sr, ring, staged, lens, offs)
-                    else:
-                        free.put(ring)
+            chosen = staged_route(batch_cuts, perturbed_tracks=perturbed_tracks, reverb=reverb) if use_ring else None
+            if chosen is not None:
+                kind, reqs = chosen
+                free = free_rings[kind]
+                ring = free.get()  # handed back by stage 2 once the batch's host-to-device copy has completed
+                staged, lens, offs, fsr = ring.stage(reqs, executor=pool)
+                if fsr == sr:
+                    item = (kind, batch_cuts, sr, ring, staged, lens, offs)
+                else:
+                    free.put(ring)
             if item is None:
                 audios, batch_cuts = read_audio_from_cuts(batch_cuts, executor=pool)
                 if not batch_cuts:
@@ -384,10 +371,8 @@ def compute_and_store_features_fused(
     with cuts_writer, B200ArchiveWriter(storage_path, mode="w" if overwrite else "a") as writer:
         if use_ring:
             for _ in range(2 if pipelined else 1):
-                rings.put(PcmStagingRing())
-                flac_rings.put(FlacStagingRing(initial_bytes=1 << 16))
-                mix_rings.put(MixStagingRing())
-                transform_rings.put(TransformStagingRing())
+                for route in STAGED_ROUTES:
+                    free_rings[route].put(new_ring(route))
         if not pipelined:  # stage 1 and 2 in the calling thread, stage 3 one batch behind in a saver thread
             with ThreadPoolExecutor(max_workers=1) as saver:
                 futures = [saver.submit(_store, *_extract(item)) for item in _staged_batches()]
@@ -442,14 +427,9 @@ def compute_and_store_features_fused(
                         staged_q.get(timeout=0.05)
                     except queue.Empty:
                         pass
-                    if use_ring and rings.empty():
-                        rings.put(PcmStagingRing(initial_samples=16, pin_memory=False))
-                    if use_ring and flac_rings.empty():
-                        flac_rings.put(FlacStagingRing(initial_bytes=16, pin_memory=False))
-                    if use_ring and mix_rings.empty():
-                        mix_rings.put(MixStagingRing(pin_memory=False))
-                    if use_ring and transform_rings.empty():
-                        transform_rings.put(TransformStagingRing(pin_memory=False))
+                    for route in STAGED_ROUTES:
+                        if use_ring and free_rings[route].empty():
+                            free_rings[route].put(new_ring(route, pin_memory=False))
                 t_read.join()
     if pool is not None:
         pool.shutdown()
