@@ -95,14 +95,24 @@ def _host_mix(harness, tmp_path, cuts):
     assert reqs is not None
     batch, lens, offs, sr = MixStagingRing(pin_memory=False).stage(reqs)
     assert sr == 16000 and batch.flac is None and all(o % 4 == 0 for o in offs)
-    batch.pcm.numpy().tofile(tmp_path / "s0.i16")
-    np.zeros(0, np.int16).tofile(tmp_path / "s1.i16")
-    batch.tracks.tofile(tmp_path / "t.bin")
-    batch.cuts.tofile(tmp_path / "c.bin")
-    _run(harness, "mix", tmp_path / "s0.i16", tmp_path / "s1.i16", tmp_path / "t.bin", tmp_path / "c.bin", batch.out_elems,
-         tmp_path / "o.f32")
-    out = np.fromfile(tmp_path / "o.f32", dtype=np.float32)
+    out = run_mix(harness, tmp_path, batch.pcm.numpy(), np.zeros(0, np.int16), batch.tracks, batch.cuts, batch.out_elems)
     return [out[o:o + n] for o, n in zip(offs, lens)], batch
+
+
+def run_mix(harness, tmp_path, src0, src1, tracks, cuts, out_elems, src2=None):
+    """b200feat_mix_ex through the host harness: the int16 sources, the float32 track buffer `src2` (None: none) and the
+    MIX_TRACK_DTYPE / MIX_CUT_DTYPE tables -> the float32 output buffer (zeros outside the cuts' windows)."""
+    np.asarray(src0, np.int16).tofile(tmp_path / "s0.i16")
+    np.asarray(src1, np.int16).tofile(tmp_path / "s1.i16")
+    tracks.tofile(tmp_path / "t.bin")
+    cuts.tofile(tmp_path / "c.bin")
+    extra = []
+    if src2 is not None:
+        np.asarray(src2, np.float32).tofile(tmp_path / "s2.f32")
+        extra = [tmp_path / "s2.f32"]
+    _run(harness, "mix", tmp_path / "s0.i16", tmp_path / "s1.i16", tmp_path / "t.bin", tmp_path / "c.bin", out_elems,
+         tmp_path / "o.f32", *extra)
+    return np.fromfile(tmp_path / "o.f32", dtype=np.float32)
 
 
 @needs_ref

@@ -56,21 +56,30 @@ def host_transform(harness, tmp_path, cuts):
     assert reqs is not None
     batch, lens, offs, _ = TransformStagingRing(pin_memory=False).stage(reqs)
     assert batch.flac is None and all(o % 4 == 0 for o in offs)
-    batch.pcm.numpy().tofile(tmp_path / "s0.i16")
-    np.zeros(0, np.int16).tofile(tmp_path / "s1.i16")
+    st = batch.stages.copy()
+    st["table"] = batch.pair
+    out = run_stages(harness, tmp_path, batch.pcm.numpy(), np.zeros(0, np.int16), batch.pairs, st, batch.mid_elems,
+                     batch.out_elems)
+    return [out[o:o + n] for o, n in zip(offs, lens)], batch
+
+
+def run_stages(harness, tmp_path, src0, src1, pairs, stages, mid_elems, out_elems):
+    """b200feat_resample through the host harness: the int16 sources, the rate pairs and RESAMPLE_STAGE_DTYPE records whose
+    `table` indexes `pairs` (-1: no resampling) -> the float32 output buffer (zeros outside the stages' windows)."""
+    from lhotse_b200.pcm_staging import resample_kernel
+
+    np.asarray(src0, np.int16).tofile(tmp_path / "s0.i16")
+    np.asarray(src1, np.int16).tofile(tmp_path / "s1.i16")
     with open(tmp_path / "tables.bin", "wb") as f:
-        for a, b in batch.pairs:
+        for a, b in pairs:
             table, width = resample_kernel(a, b)
             N, K = table.shape
             np.asarray([N, K - 2 * width, K, width], np.int32).tofile(f)
             table.tofile(f)
-    st = batch.stages.copy()
-    st["table"] = batch.pair
-    st.tofile(tmp_path / "st.bin")
-    _run(harness, tmp_path / "s0.i16", tmp_path / "s1.i16", tmp_path / "tables.bin", tmp_path / "st.bin", batch.mid_elems,
-         batch.out_elems, tmp_path / "o.f32")
-    out = np.fromfile(tmp_path / "o.f32", dtype=np.float32)
-    return [out[o:o + n] for o, n in zip(offs, lens)], batch
+    stages.tofile(tmp_path / "st.bin")
+    _run(harness, tmp_path / "s0.i16", tmp_path / "s1.i16", tmp_path / "tables.bin", tmp_path / "st.bin", mid_elems, out_elems,
+         tmp_path / "o.f32")
+    return np.fromfile(tmp_path / "o.f32", dtype=np.float32)
 
 
 def _run(exe, *args):
