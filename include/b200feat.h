@@ -444,6 +444,51 @@ int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_el
                     const b200feat_reverb_cut *cuts, int32_t ncuts, float *out_dev, int64_t out_elems, void *work_dev,
                     int64_t work_bytes, void *stream);
 
+#define B200FEAT_REVERB_RIR_F32 2  /* b200feat_reverb_rir.source of b200feat_reverb_ex: the float32 RIR buffer */
+
+/* b200feat_reverb with a third RIR source: records whose `source` is B200FEAT_REVERB_RIR_F32 read float32 samples of
+ * `rir32_dev` (for example RIRs that b200feat_rir_generate and b200feat_resample wrote), scaled by 2^-15 as lhotse scales
+ * them; the shift is the first index of their maximum.  The same checks, plus: such an RIR lies inside rir32.
+ * b200feat_reverb is this call with no rir32.  The work buffer is b200feat_reverb_work_bytes of the same tables. */
+int b200feat_reverb_ex(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev,
+                       int64_t src1_elems, const float *rir32_dev, int64_t rir32_elems, const float *in_dev, int64_t in_elems,
+                       const b200feat_reverb_rir *rirs, int32_t nrirs, const b200feat_reverb_cut *cuts, int32_t ncuts,
+                       float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
+
+/*
+ * lhotse's FastRandomRIRGenerator (one source) on the GPU, from draws made on the host (DESIGN.md §3.1l): the Dirac comb at
+ * 64 x sr, its 8 -> 1 resampling and torchaudio's 80 Hz highpass biquad, written as float32 at 8 x sr.  b200feat_resample
+ * with the same 8 -> 1 table then gives the RIR at sr.  Results are identical from run to run.
+ */
+#define B200FEAT_RIRGEN_TAPS 106  /* the 8 -> 1 resampler table: 2 * 49 + 8 taps */
+
+typedef struct b200feat_rir_gen {
+  int32_t struct_size;   /* sizeof(b200feat_rir_gen) — ABI guard, in every record */
+  int32_t sampling_rate; /* the generator's sr, 1 .. 192000: 2 sr image sources, a comb at 64 sr */
+  double t60;            /* room_rng's T60 draw, > 0 */
+  double r;              /* room_rng's R draw */
+  double d0;             /* source_rng's distance draw, > 0 */
+  double tau;            /* the generator's tau */
+  float b0, b1, b2, a1, a2;  /* highpass_biquad(., 8 sr, 80)'s coefficients divided by a0, as torchaudio's lfilter takes them */
+  int32_t reserved;
+  int64_t cdf_elem;      /* first of the 2 sr entries of the normalised cumulative distribution (float32, last one 1) */
+  int64_t draw_elem;     /* first of the 2 sr multinomial uniforms in the draws buffer; the 2 sr perturbations follow */
+  int64_t comb_len;      /* L = ceil(64 sr T60) as lhotse computes it, 1 .. 2^31 - 1 */
+  int64_t out_elem;      /* first output sample */
+  int64_t out_len;       /* min(ceil(f32(L / 8)), L / 8 + 1): what lhotse's first resampler keeps */
+} b200feat_rir_gen;
+
+/* Device scratch b200feat_rir_generate needs for these records (0 when the count is negative or a record is malformed). */
+int64_t b200feat_rir_generate_work_bytes(const b200feat_rir_gen *rirs, int32_t nrirs);
+
+/* Checks the records (every read inside its buffer, every output inside `out_dev` and disjoint from the others, the lengths
+ * as above), copies them and the host table `table` (B200FEAT_RIRGEN_TAPS floats, lhotse's 8 -> 1 resampler) to `work_dev`
+ * and launches the entry kernel, the segmented sort, the window kernel and the biquad kernel, asynchronously on `stream`.
+ * Errors are reported through `h` (b200feat_last_error) when it is not NULL, and through b200feat_global_error. */
+int b200feat_rir_generate(b200feat_handle *h, const double *draws_dev, int64_t draws_elems, const float *cdf_dev,
+                          int64_t cdf_elems, const float *table, const b200feat_rir_gen *rirs, int32_t nrirs, float *out_dev,
+                          int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
+
 /*
  * SpecAugment on a padded (B, T, F) float32 feature batch on the GPU: what lhotse's SpecAugment.forward computes from the
  * same random draws (DESIGN.md §3.1k).  The host draws the numbers and hands over two tables: the time warps (bicubic along

@@ -30,6 +30,9 @@
 #include "resample.cuh"
 #include "reverb.cuh"
 #include "specaug.cuh"
+#include "rirgen.cuh"
+
+#include <cub/device/device_segmented_radix_sort.cuh>
 
 namespace {
 
@@ -1144,8 +1147,16 @@ int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_el
                     const float *in_dev, int64_t in_elems, const b200feat_reverb_rir *rirs, int32_t nrirs,
                     const b200feat_reverb_cut *cuts, int32_t ncuts, float *out_dev, int64_t out_elems, void *work_dev,
                     int64_t work_bytes, void *stream) {
+  return b200feat_reverb_ex(h, src0_dev, src0_elems, src1_dev, src1_elems, nullptr, 0, in_dev, in_elems, rirs, nrirs, cuts,
+                            ncuts, out_dev, out_elems, work_dev, work_bytes, stream);
+}
+
+int b200feat_reverb_ex(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_elems, const int16_t *src1_dev,
+                       int64_t src1_elems, const float *rir32_dev, int64_t rir32_elems, const float *in_dev, int64_t in_elems,
+                       const b200feat_reverb_rir *rirs, int32_t nrirs, const b200feat_reverb_cut *cuts, int32_t ncuts,
+                       float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream) {
   if (nrirs < 0 || ncuts < 0 || (ncuts > 0 && (!rirs || !cuts || !in_dev || !out_dev || !work_dev || nrirs < 1)) ||
-      src0_elems < 0 || src1_elems < 0 || in_elems < 0 || out_elems < 0)
+      src0_elems < 0 || src1_elems < 0 || rir32_elems < 0 || in_elems < 0 || out_elems < 0)
     return fail(h, B200FEAT_EINVAL, "reverb: bad arguments");
   if (ncuts == 0) return B200FEAT_OK;
   if (ncuts > 65535) return fail(h, B200FEAT_EINVAL, "reverb: more than 65535 cuts in one call");
@@ -1156,10 +1167,12 @@ int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_el
     const b200feat_reverb_rir &r = rirs[i];
     if (r.struct_size != (int32_t)sizeof(b200feat_reverb_rir))
       return fail(h, B200FEAT_EINVAL, where("rir", i) + "b200feat_reverb_rir size mismatch (ABI)");
-    if (r.source < 0 || r.source > 1) return fail(h, B200FEAT_EINVAL, where("rir", i) + "source must be 0 or 1");
+    if (r.source < 0 || r.source > 2) return fail(h, B200FEAT_EINVAL, where("rir", i) + "source must be 0, 1 or 2");
     if (r.num_samples < 1 || r.num_samples > B200FEAT_REVERB_MAX_RIR)
       return fail(h, B200FEAT_EINVAL, where("rir", i) + "length outside 1 .. B200FEAT_REVERB_MAX_RIR");
-    if (!src[r.source] || r.src_elem < 0 || r.src_elem > src_elems[r.source] - r.num_samples)
+    const bool f32 = r.source == B200FEAT_REVERB_RIR_F32;
+    if ((f32 ? !rir32_dev : !src[r.source]) || r.src_elem < 0 ||
+        r.src_elem > (f32 ? rir32_elems : src_elems[r.source]) - r.num_samples)
       return fail(h, B200FEAT_EINVAL, where("rir", i) + "samples outside its source buffer");
   }
   for (int32_t c = 0; c < ncuts; ++c) {
@@ -1202,7 +1215,9 @@ int b200feat_reverb(b200feat_handle *h, const int16_t *src0_dev, int64_t src0_el
   std::vector<RvRir> rv((size_t)nrirs);
   int64_t parts = 0;
   for (int32_t i = 0; i < nrirs; ++i) {
-    rv[i] = RvRir{src[rirs[i].source] + rirs[i].src_elem, rirs[i].num_samples, parts, (int32_t)rv_parts(rirs[i].num_samples), 0};
+    const bool f32 = rirs[i].source == B200FEAT_REVERB_RIR_F32;
+    rv[i] = RvRir{f32 ? nullptr : src[rirs[i].source] + rirs[i].src_elem, rirs[i].num_samples, parts,
+                  (int32_t)rv_parts(rirs[i].num_samples), 0, f32 ? rir32_dev + rirs[i].src_elem : nullptr};
     parts += rv[i].nparts;
   }
   std::vector<RvCut> cv((size_t)ncuts);
@@ -1361,6 +1376,139 @@ int b200feat_specaug(b200feat_handle *h, const float *in_dev, float *out_dev, in
   CU_TRY(h, cudaGetLastError());
   const int64_t gy = std::min<int64_t>(std::max<int64_t>((largest + 8 * SA_FILL_THREADS - 1) / (8 * SA_FILL_THREADS), 1), 64);
   specaug_fill_kernel<<<dim3((unsigned)nmasks, (unsigned)gy), SA_FILL_THREADS, 0, st>>>(out_dev, T, F, (const SaMask *)(w + l.masks), d_mean);
+  CU_TRY(h, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The generator's work buffer: the kernels' RIR table, the resampler table, the segment offsets, the entries before and after
+// the sort, the sort's own scratch
+struct RgLayout {
+  int64_t rirs, table, offsets, pos_in, val_in, pos_out, val_out, temp, temp_bytes, total;
+  int64_t entries;
+  int end_bit;
+};
+
+// Whether the record is one b200feat_rir_generate takes (the buffer bounds are checked by the call)
+bool rg_record_ok(const b200feat_rir_gen &g) {
+  return g.struct_size == (int32_t)sizeof(b200feat_rir_gen) && g.sampling_rate >= 1 && g.sampling_rate <= 192000 &&
+         g.t60 > 0.0 && g.d0 > 0.0 && isfinite(g.t60) && isfinite(g.r) && isfinite(g.d0) && isfinite(g.tau) &&
+         g.comb_len >= 1 && g.comb_len <= 0x7fffffff && g.out_len >= 1 && g.out_len <= g.comb_len / RG_O + 1;
+}
+
+// false when a record is malformed or the entries do not fit the sort's int offsets
+bool rg_layout(const b200feat_rir_gen *rirs, int32_t n, RgLayout *l) {
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  *l = RgLayout{};
+  int64_t longest = 1;
+  for (int32_t i = 0; i < n; ++i) {
+    if (!rg_record_ok(rirs[i])) return false;
+    l->entries += 2 * (int64_t)rirs[i].sampling_rate + 1;
+    longest = std::max(longest, rirs[i].comb_len);
+  }
+  if (l->entries > 0x7fffffff) return false;
+  l->end_bit = 1;
+  while (l->end_bit < 31 && ((int64_t)1 << l->end_bit) < longest) ++l->end_bit;
+  size_t temp = 0;
+  if (n > 0 && cub::DeviceSegmentedRadixSort::SortPairs(nullptr, temp, (const int32_t *)nullptr, (int32_t *)nullptr,
+                                                        (const float *)nullptr, (float *)nullptr, (int)l->entries, n,
+                                                        (const int *)nullptr, (const int *)nullptr + 1, 0, l->end_bit) != cudaSuccess)
+    return false;
+  l->temp_bytes = (int64_t)temp;
+  l->rirs = 0;
+  l->table = l->rirs + up((int64_t)n * (int64_t)sizeof(RgRir));
+  l->offsets = l->table + up(RG_TAPS * 4);
+  l->pos_in = l->offsets + up(((int64_t)n + 1) * 4);
+  l->val_in = l->pos_in + up(l->entries * 4);
+  l->pos_out = l->val_in + up(l->entries * 4);
+  l->val_out = l->pos_out + up(l->entries * 4);
+  l->temp = l->val_out + up(l->entries * 4);
+  l->total = l->temp + up(std::max<int64_t>(l->temp_bytes, 1));
+  return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t b200feat_rir_generate_work_bytes(const b200feat_rir_gen *rirs, int32_t nrirs) {
+  RgLayout l;
+  if (nrirs < 0 || (nrirs > 0 && !rirs) || !rg_layout(rirs, nrirs, &l)) return 0;
+  return l.total;
+}
+
+int b200feat_rir_generate(b200feat_handle *h, const double *draws_dev, int64_t draws_elems, const float *cdf_dev,
+                          int64_t cdf_elems, const float *table, const b200feat_rir_gen *rirs, int32_t nrirs, float *out_dev,
+                          int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream) {
+  if (nrirs < 0 || (nrirs > 0 && (!rirs || !draws_dev || !cdf_dev || !table || !out_dev || !work_dev)) || draws_elems < 0 ||
+      cdf_elems < 0 || out_elems < 0)
+    return fail(h, B200FEAT_EINVAL, "rir_generate: bad arguments");
+  if (nrirs == 0) return B200FEAT_OK;
+  auto where = [](int64_t i) { return std::string("rir_generate: rir ") + std::to_string(i) + ": "; };
+  std::vector<std::pair<int64_t, int64_t>> outs((size_t)nrirs);
+  for (int32_t i = 0; i < nrirs; ++i) {
+    const b200feat_rir_gen &g = rirs[i];
+    if (g.struct_size != (int32_t)sizeof(b200feat_rir_gen))
+      return fail(h, B200FEAT_EINVAL, where(i) + "b200feat_rir_gen size mismatch (ABI)");
+    if (!rg_record_ok(g))
+      return fail(h, B200FEAT_EINVAL, where(i) + "bad sampling rate, draws or lengths (T60 and d0 must be positive, "
+                                                 "out_len at most comb_len / 8 + 1)");
+    const int64_t images = 2 * (int64_t)g.sampling_rate;
+    if (g.cdf_elem < 0 || g.cdf_elem > cdf_elems - images)
+      return fail(h, B200FEAT_EINVAL, where(i) + "distribution outside the cdf buffer");
+    if (g.draw_elem < 0 || g.draw_elem > draws_elems - 2 * images)
+      return fail(h, B200FEAT_EINVAL, where(i) + "draws outside the draws buffer");
+    if (g.out_elem < 0 || g.out_elem > out_elems - g.out_len)
+      return fail(h, B200FEAT_EINVAL, where(i) + "output outside the output buffer");
+    outs[i] = {g.out_elem, g.out_elem + g.out_len};
+  }
+  std::sort(outs.begin(), outs.end());
+  for (int32_t i = 1; i < nrirs; ++i)
+    if (outs[i].first < outs[i - 1].second) return fail(h, B200FEAT_EINVAL, "rir_generate: two outputs overlap");
+  RgLayout l;
+  if (!rg_layout(rirs, nrirs, &l)) return fail(h, B200FEAT_EINVAL, "rir_generate: more than 2^31 - 1 entries in one call");
+  if (work_bytes < l.total) return fail(h, B200FEAT_EINVAL, "rir_generate: work buffer too small");
+  char *w = (char *)work_dev;
+  std::vector<RgRir> rg((size_t)nrirs);
+  std::vector<int32_t> offsets((size_t)nrirs + 1);
+  int64_t entries = 0, ctas = 0;
+  for (int32_t i = 0; i < nrirs; ++i) {
+    const b200feat_rir_gen &g = rirs[i];
+    const int32_t images = 2 * g.sampling_rate;
+    rg[i] = RgRir{draws_dev + g.draw_elem, draws_dev + g.draw_elem + images, cdf_dev + g.cdf_elem, out_dev + g.out_elem,
+                  g.t60, g.r, g.d0, g.tau, g.comb_len, g.out_len, entries, ctas, g.sampling_rate, images,
+                  g.b0, g.b1, g.b2, g.a1, g.a2};
+    offsets[i] = (int32_t)entries;
+    entries += images + 1;
+    ctas += (g.out_len + RG_THREADS - 1) / RG_THREADS;
+  }
+  offsets[nrirs] = (int32_t)entries;
+  if (ctas > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "rir_generate: too many CTAs in one call");
+  const cudaStream_t st = (cudaStream_t)stream;
+  RgRir *d_rirs = (RgRir *)(w + l.rirs);
+  float *d_table = (float *)(w + l.table);
+  int32_t *d_offsets = (int32_t *)(w + l.offsets);
+  int32_t *pos_in = (int32_t *)(w + l.pos_in), *pos_out = (int32_t *)(w + l.pos_out);
+  float *val_in = (float *)(w + l.val_in), *val_out = (float *)(w + l.val_out);
+  // pageable copies: the call returns once the tables have been staged, so the vectors may go when this function returns
+  CU_TRY(h, cudaMemcpyAsync(d_rirs, rg.data(), rg.size() * sizeof(RgRir), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_table, table, RG_TAPS * sizeof(float), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_offsets, offsets.data(), offsets.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  rirgen_entry_kernel<<<(unsigned)((entries + RG_THREADS - 1) / RG_THREADS), RG_THREADS, 0, st>>>(d_rirs, nrirs, entries,
+                                                                                                 pos_in, val_in);
+  CU_TRY(h, cudaGetLastError());
+  size_t temp = (size_t)l.temp_bytes;
+  // a stable sort: entries that share a position keep their entry order, so the window kernel can keep the last one
+  CU_TRY(h, cub::DeviceSegmentedRadixSort::SortPairs(w + l.temp, temp, pos_in, pos_out, val_in, val_out, (int)entries, nrirs,
+                                                     d_offsets, d_offsets + 1, 0, l.end_bit, st));
+  if (ctas > 0) {
+    rirgen_window_kernel<<<(unsigned)ctas, RG_THREADS, 0, st>>>(d_rirs, nrirs, pos_out, val_out, d_table);
+    CU_TRY(h, cudaGetLastError());
+  }
+  rirgen_biquad_kernel<<<(unsigned)((nrirs + 31) / 32), 32, 0, st>>>(d_rirs, nrirs);
   CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }

@@ -47,6 +47,7 @@ struct RvRir {
   int64_t part_begin;   // its first partition in the spectra table (and in the RIR kernel's grid)
   int32_t nparts;       // ceil(R / RV_B)
   int32_t reserved;
+  const float *src32;   // or, when set (b200feat_reverb_ex), its R float32 samples h / 2^-15 (a generated RIR)
 };
 
 // One cut as the kernels read it
@@ -99,11 +100,14 @@ MIX_HD rv_c rv_cmac(rv_c acc, rv_c a, rv_c b) {
   return rv_c{RV_FMA(a.x, b.x, RV_FMA(-a.y, b.y, acc.x)), RV_FMA(a.x, b.y, RV_FMA(a.y, b.x, acc.y))};
 }
 
+// RIR sample i before lhotse's 2^-15 scaling: f32(q / 32768) for an int16 RIR, the float32 sample itself otherwise
+MIX_HD float rv_rir_value(const RvRir &r, int64_t i) { return r.src32 ? r.src32[i] : mix_widen(r.src[i]); }
+
 // RIR sample k of partition p as its spectrum takes it: h * 2^-15 * (1 / RV_F), exact; 0 past the RIR
 MIX_HD float rv_rir_sample(const RvRir &r, int p, int k) {
   const int64_t i = (int64_t)p * RV_B + k;
   if (k >= RV_B || i >= r.len) return 0.0f;
-  return MIX_FMUL(mix_widen(r.src[i]), 1.0f / (32768.0f * RV_F));
+  return MIX_FMUL(rv_rir_value(r, i), 1.0f / (32768.0f * RV_F));
 }
 
 // The first input sample of the transform of CTA q's block pair for partition p (its real part; the imaginary part starts
@@ -164,20 +168,29 @@ __global__ void __launch_bounds__(RV_THREADS) reverb_rir_kernel(const RvRir *__r
   for (int k = threadIdx.x; k < RV_F; k += RV_THREADS) dst[k] = a[k];
   if (p != 0) return;
   // first index of the maximum: per thread, then a tree over (value, index) with ties to the lower index
-  int best = -32769, at = 0x7fffffff;
-  for (int64_t i = threadIdx.x; i < r.len; i += RV_THREADS)
-    if (r.src[i] > best) { best = r.src[i]; at = (int)i; }
-  int *red = (int *)(tw + RV_B);
+  // (on the widened samples: the widening of an int16 RIR is monotonic, so its first maximum is the same)
+  float best = -INFINITY;
+  int at = 0x7fffffff;
+  for (int64_t i = threadIdx.x; i < r.len; i += RV_THREADS) {
+    const float v = rv_rir_value(r, i);
+    if (v > best || at == 0x7fffffff) { best = v; at = (int)i; }
+  }
+  float *red = (float *)(tw + RV_B);
+  int *red_at = (int *)(red + 16);
   for (int off = 16; off > 0; off >>= 1) {
-    const int ob = __shfl_down_sync(0xffffffffu, best, off), oa = __shfl_down_sync(0xffffffffu, at, off);
-    if (ob > best || (ob == best && oa < at)) { best = ob; at = oa; }
+    const float ob = __shfl_down_sync(0xffffffffu, best, off);
+    const int oa = __shfl_down_sync(0xffffffffu, at, off);
+    if (oa != 0x7fffffff && (ob > best || (ob == best && oa < at) || at == 0x7fffffff)) { best = ob; at = oa; }
   }
   __syncthreads();
-  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = best; red[16 + (threadIdx.x >> 5)] = at; }
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = best; red_at[threadIdx.x >> 5] = at; }
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < RV_THREADS / 32; ++w)
-      if (red[w] > best || (red[w] == best && red[16 + w] < at)) { best = red[w]; at = red[16 + w]; }
+      if (red_at[w] != 0x7fffffff && (red[w] > best || (red[w] == best && red_at[w] < at) || at == 0x7fffffff)) {
+        best = red[w];
+        at = red_at[w];
+      }
     shift[lo] = at;
   }
 }

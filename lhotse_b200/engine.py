@@ -93,6 +93,14 @@ REVERB_RIR_DTYPE = np.dtype([("struct_size", "<i4"), ("source", "<i4"), ("src_el
 REVERB_CUT_DTYPE = np.dtype([("struct_size", "<i4"), ("rir", "<i4"), ("normalize", "<i4"), ("reserved", "<i4"), ("in_elem", "<i8"),
                              ("in_len", "<i8"), ("out_elem", "<i8"), ("target_len", "<i8")])
 REVERB_MAX_RIR = 65536  # B200FEAT_REVERB_MAX_RIR
+REVERB_RIR_F32 = 2      # B200FEAT_REVERB_RIR_F32: b200feat_reverb_ex's float32 RIR source
+
+# b200feat_rir_gen as a numpy record layout
+RIR_GEN_DTYPE = np.dtype([("struct_size", "<i4"), ("sampling_rate", "<i4"), ("t60", "<f8"), ("r", "<f8"), ("d0", "<f8"),
+                          ("tau", "<f8"), ("b0", "<f4"), ("b1", "<f4"), ("b2", "<f4"), ("a1", "<f4"), ("a2", "<f4"),
+                          ("reserved", "<i4"), ("cdf_elem", "<i8"), ("draw_elem", "<i8"), ("comb_len", "<i8"),
+                          ("out_elem", "<i8"), ("out_len", "<i8")])
+RIRGEN_TAPS = 106  # B200FEAT_RIRGEN_TAPS
 
 # b200feat_specaug_warp / b200feat_specaug_mask as numpy record layouts
 SPECAUG_WARP_DTYPE = np.dtype([("struct_size", "<i4"), ("seq", "<i4"), ("start", "<i4"), ("len", "<i4"), ("center", "<i4"),
@@ -111,6 +119,7 @@ EXPORTS = [
     "b200feat_flac_index", "b200feat_flac_decode", "b200feat_mix_work_bytes", "b200feat_mix",
     "b200feat_resample_table", "b200feat_resample_work_bytes", "b200feat_resample", "b200feat_mix_ex",
     "b200feat_reverb_work_bytes", "b200feat_reverb", "b200feat_specaug_work_bytes", "b200feat_specaug",
+    "b200feat_reverb_ex", "b200feat_rir_generate_work_bytes", "b200feat_rir_generate",
 ]
 
 
@@ -190,6 +199,12 @@ def load_library():
         lib.b200feat_reverb_work_bytes.argtypes = [vp, i32, vp, i32]
         lib.b200feat_reverb.restype = C.c_int
         lib.b200feat_reverb.argtypes = [vp, vp, i64, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
+        lib.b200feat_reverb_ex.restype = C.c_int
+        lib.b200feat_reverb_ex.argtypes = [vp, vp, i64, vp, i64, vp, i64, vp, i64, vp, i32, vp, i32, vp, i64, vp, i64, vp]
+        lib.b200feat_rir_generate_work_bytes.restype = i64
+        lib.b200feat_rir_generate_work_bytes.argtypes = [vp, i32]
+        lib.b200feat_rir_generate.restype = C.c_int
+        lib.b200feat_rir_generate.argtypes = [vp, vp, i64, vp, i64, vp, vp, i32, vp, i64, vp, i64, vp]
         lib.b200feat_specaug_work_bytes.restype = i64
         lib.b200feat_specaug_work_bytes.argtypes = [i32, i32, i32, i32, i32]
         lib.b200feat_specaug.restype = C.c_int
@@ -321,10 +336,11 @@ def resample(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], mid: Op
 
 
 def reverb(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], x: torch.Tensor, rirs: np.ndarray, cuts: np.ndarray,
-           out: torch.Tensor, handle=None) -> None:
-    """Launches `b200feat_reverb` on the current stream of `out`'s device (asynchronous): the int16 device sources of the
+           out: torch.Tensor, handle=None, rir32: Optional[torch.Tensor] = None) -> None:
+    """Launches `b200feat_reverb_ex` on the current stream of `out`'s device (asynchronous): the int16 device sources of the
     RIRs, the float32 input `x`, the host RIR / cut tables (REVERB_RIR_DTYPE / REVERB_CUT_DTYPE; copied before this returns)
-    and the float32 output.  Raises B200FeatError when the library refuses the tables."""
+    and the float32 output; `rir32`, the float32 RIRs of records whose source is REVERB_RIR_F32 (generated ones).  Raises
+    B200FeatError when the library refuses the tables."""
     lib = load_library()
     stream = torch.cuda.current_stream(out.device).cuda_stream
     assert rirs.dtype == REVERB_RIR_DTYPE and cuts.dtype == REVERB_CUT_DTYPE
@@ -336,10 +352,32 @@ def reverb(src0: Optional[torch.Tensor], src1: Optional[torch.Tensor], x: torch.
     def src(t):
         return (None, 0) if t is None or t.numel() == 0 else (t.data_ptr(), t.numel())
 
-    (p0, n0), (p1, n1), (px, nx) = src(src0), src(src1), src(x)
+    (p0, n0), (p1, n1), (p2, n2), (px, nx) = src(src0), src(src1), src(rir32), src(x)
     with torch.cuda.device(out.device):
-        rc = lib.b200feat_reverb(handle, p0, n0, p1, n1, px, nx, rirs.ctypes.data, len(rirs), cuts.ctypes.data, len(cuts),
-                                 out.data_ptr(), out.numel(), work.data_ptr(), work.numel(), stream)
+        rc = lib.b200feat_reverb_ex(handle, p0, n0, p1, n1, p2, n2, px, nx, rirs.ctypes.data, len(rirs), cuts.ctypes.data,
+                                    len(cuts), out.data_ptr(), out.numel(), work.data_ptr(), work.numel(), stream)
+    if rc != 0:
+        _raise(lib, rc, handle)
+
+
+def rir_generate(draws: torch.Tensor, cdf: torch.Tensor, table: np.ndarray, rirs: np.ndarray, out: torch.Tensor,
+                 handle=None) -> None:
+    """Launches `b200feat_rir_generate` on the current stream of `out`'s device (asynchronous): the float64 device draws, the
+    float32 device distributions, the host 8 -> 1 resampler table (RIRGEN_TAPS floats) and records (RIR_GEN_DTYPE; both
+    copied before this returns) and the float32 output at 8 x sr.  Raises B200FeatError when the library refuses them."""
+    lib = load_library()
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    assert rirs.dtype == RIR_GEN_DTYPE and draws.dtype == torch.float64 and cdf.dtype == torch.float32
+    assert out.dtype == torch.float32
+    rirs = np.ascontiguousarray(rirs)
+    table = np.ascontiguousarray(table, dtype=np.float32)
+    assert table.shape == (RIRGEN_TAPS,)
+    with torch.cuda.device(out.device):  # the sort's scratch query depends on the device
+        nbytes = int(lib.b200feat_rir_generate_work_bytes(rirs.ctypes.data, len(rirs)))
+        work = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=out.device)
+        rc = lib.b200feat_rir_generate(handle, draws.data_ptr(), draws.numel(), cdf.data_ptr(), cdf.numel(),
+                                       table.ctypes.data, rirs.ctypes.data, len(rirs), out.data_ptr(), out.numel(),
+                                       work.data_ptr(), work.numel(), stream)
     if rc != 0:
         _raise(lib, rc, handle)
 

@@ -36,6 +36,7 @@ class FusedOnTheFlyFeatures:
         global_mvn=None,
         perturbed_tracks: bool = False,
         reverb: bool = False,
+        generated_rir: bool = False,
     ) -> None:
         if not hasattr(extractor, "extract_batch_padded"):
             raise TypeError("FusedOnTheFlyFeatures needs a lhotse_b200 extractor (extract_batch_padded)")
@@ -66,10 +67,14 @@ class FusedOnTheFlyFeatures:
         # is not bit-reproducible (its bits change with the CPU and the torch thread count), so this one is held to a float32
         # tolerance of a float64 convolution instead of bit equality; it is off by default so that existing pipelines keep
         # exactly their routes and features, and whether to turn it on by default is decided once H100 measurements of it
-        # exist.  `pcm16_fast_path=False` turns all staged routes off.
+        # exist.  `generated_rir=True` does the same for cuts whose RIR lhotse generates (no RIR corpus): the generator's
+        # random numbers are drawn on the host from the same generators in the same order, the RIRs are built on the GPU
+        # (DESIGN.md §3.1l); it is a separate flag so that `reverb=True` pipelines keep exactly their routes.
+        # `pcm16_fast_path=False` turns all staged routes off.
         self.pcm16_fast_path = pcm16_fast_path and hasattr(extractor, "extract_staged_padded")
         self.perturbed_tracks = perturbed_tracks
         self.reverb = reverb
+        self.generated_rir = generated_rir
         self._rings = {}  # route -> its staging ring, made when a batch first takes the route
         self.last_batch_route = None  # "pcm16" | "flac" | "mix" | "transform" | "float" (introspection for tests / logs)
         self._executor_type = executor_type
@@ -104,22 +109,26 @@ class FusedOnTheFlyFeatures:
         """(route, (features, lengths)) of a staged route, or None: the float route takes the batch."""
         if not self.pcm16_fast_path or self.wave_transforms or self.return_audio or recording_field is not None:
             return None
-        from .pcm_staging import new_ring, staged_route
+        from .pcm_staging import new_ring, staged_route, undo_draws
 
-        chosen = staged_route(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb)
+        chosen = staged_route(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb,
+                              generated_rir=self.generated_rir)
         if chosen is None:
             return None  # mixed sampling rates (grouped by the float route) or a cut no staged route takes
         route, reqs = chosen
         ring = self._rings.get(route)
         if ring is None:
             ring = self._rings[route] = new_ring(route)
+        staged = None
         try:  # a FLAC frame that does not decode raises ValueError before any feature is handed back
             staged, lens, offs, sr = ring.stage(reqs, executor=self._get_executor())
             if sr != cuts[0].sampling_rate:
+                undo_draws(staged)  # the float route draws the generated RIRs again
                 return None
             out = self.extractor.extract_staged_padded(staged, lens, offs, sr, padding_value=LOG_EPSILON, ring=ring,
                                                        **({"engine": self._mvn_engine} if self._mvn_engine is not None else {}))
         except (OSError, ValueError):
+            undo_draws(staged)
             if self.fault_tolerant:
                 return None  # the float route knows how to skip broken cuts
             raise

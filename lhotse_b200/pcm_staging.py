@@ -654,7 +654,8 @@ def _numpy2() -> bool:
     return int(np.__version__.split(".")[0]) >= 2
 
 
-def mix_request_for_cut(cut, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[MixRequest]:
+def mix_request_for_cut(cut, perturbed_tracks: bool = False, reverb: bool = False,
+                        generated_rir: bool = False) -> Optional[MixRequest]:
     """What `MixedCut.load_audio()` (lhotse/cut/mixed.py) amounts to for a MixedCut of mono 16-bit WAV / FLAC slices and
     PaddingCuts: tracks, offsets, SNR factors, reference and length.  None when the cut is not eligible: not a MixedCut,
     cut-level transforms, a track that `pcm16_request_for_cut` / `flac_request_for_cut` refuse (MultiCut, nested MixedCut,
@@ -670,7 +671,8 @@ def mix_request_for_cut(cut, perturbed_tracks: bool = False, reverb: bool = Fals
     `reverb=True` also takes a MixedCut whose `transforms` are exactly one ReverbWithImpulseResponse that `reverb_request`
     accepts (what `MixedCut.reverb_rir(mix_first=True)` makes) over a float32 mix: the mix goes to a float32 buffer and the
     reverb kernel writes the cut, within a float32 tolerance of a float64 convolution (DESIGN.md §3.1j).  Tracks that carry a
-    reverb of their own (mix_first=False) stay refused.  Off by default."""
+    reverb of their own (mix_first=False) stay refused.  Off by default.  `generated_rir=True` takes such a reverb with an RIR
+    that lhotse generates (see `reverb_request`), also off by default."""
     if not _numpy2():
         return None
     try:
@@ -688,9 +690,9 @@ def mix_request_for_cut(cut, perturbed_tracks: bool = False, reverb: bool = Fals
     rv = None
     if getattr(cut, "transforms", None):
         tfs = [t if isinstance(t, AudioTransform) else AudioTransform.from_dict(t) for t in cut.transforms]
-        if not reverb or len(tfs) != 1 or type(tfs[0]) is not ReverbWithImpulseResponse:
+        if not (reverb or generated_rir) or len(tfs) != 1 or type(tfs[0]) is not ReverbWithImpulseResponse:
             return None
-        rv = reverb_request(tfs[0], cut.sampling_rate)
+        rv = reverb_request(tfs[0], cut.sampling_rate, reverb, generated_rir)
         if rv is None:
             return None
     sr = cut.sampling_rate
@@ -748,7 +750,8 @@ def mix_request_for_cut(cut, perturbed_tracks: bool = False, reverb: bool = Fals
                       num_samples=target, reverb=rv)
 
 
-def _plain_mix_request(cut, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[MixRequest]:
+def _plain_mix_request(cut, perturbed_tracks: bool = False, reverb: bool = False,
+                       generated_rir: bool = False) -> Optional[MixRequest]:
     """A plain 16-bit WAV / FLAC slice as a mix of one track (the kernel writes x = q / 32768, what the float route reads);
     with `perturbed_tracks`, also a MonoCut with an eligible transform chain (the kernel copies the chain's float32 output);
     with `reverb`, also a plain slice whose only transform is an eligible reverb (a one-track mix, then the reverb), and with
@@ -758,14 +761,14 @@ def _plain_mix_request(cut, perturbed_tracks: bool = False, reverb: bool = False
 
     if getattr(cut, "tracks", None) is not None:
         return None
-    if reverb and _has_transforms(cut):
-        r = transform_request_for_cut(cut, reverb=True)
+    if (reverb or generated_rir) and _has_transforms(cut):
+        r = transform_request_for_cut(cut, reverb=reverb, generated_rir=generated_rir)
         if r is not None and r.reverb is not None and not r.ops and r.num_samples == r.source.num_samples > 0:
             n = int(r.num_samples)
             return MixRequest(tracks=(MixTrackRequest(r.source, n, 0, float("nan"), MIX_ROLE_MIXED),), ref=0, mode=MIX_F32,
                               mix_len=n, num_samples=n, reverb=r.reverb)
     if perturbed_tracks and _has_transforms(cut):
-        src = transform_request_for_cut(cut, reverb=reverb)
+        src = transform_request_for_cut(cut, reverb=reverb, generated_rir=generated_rir)
     else:
         src = slice_request_for_cut(cut)
     if src is None or src.num_samples <= 0:
@@ -774,13 +777,15 @@ def _plain_mix_request(cut, perturbed_tracks: bool = False, reverb: bool = False
                       mode=MIX_F32, mix_len=int(src.num_samples), num_samples=int(src.num_samples))
 
 
-def _mix_or_plain_request(cut, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[MixRequest]:
+def _mix_or_plain_request(cut, perturbed_tracks: bool = False, reverb: bool = False,
+                          generated_rir: bool = False) -> Optional[MixRequest]:
     if getattr(cut, "tracks", None) is not None:
-        return mix_request_for_cut(cut, perturbed_tracks=perturbed_tracks, reverb=reverb)
-    return _plain_mix_request(cut, perturbed_tracks=perturbed_tracks, reverb=reverb)
+        return mix_request_for_cut(cut, perturbed_tracks=perturbed_tracks, reverb=reverb, generated_rir=generated_rir)
+    return _plain_mix_request(cut, perturbed_tracks=perturbed_tracks, reverb=reverb, generated_rir=generated_rir)
 
 
-def mix_requests_for_batch(cuts, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[List[MixRequest]]:
+def mix_requests_for_batch(cuts, perturbed_tracks: bool = False, reverb: bool = False,
+                           generated_rir: bool = False) -> Optional[List[MixRequest]]:
     """The "mix" route's requests for a batch: every cut a plain 16-bit WAV / FLAC slice or an eligible MixedCut, and at least
     one MixedCut (batches of plain slices keep the "pcm16" / "flac" / "float" routes).  None otherwise.  With
     `perturbed_tracks=True` (see `mix_request_for_cut`; off by default), MixedCut tracks and plain MonoCuts with an eligible
@@ -789,7 +794,7 @@ def mix_requests_for_batch(cuts, perturbed_tracks: bool = False, reverb: bool = 
         return None
     reqs = []
     for c in cuts:
-        r = _mix_or_plain_request(c, perturbed_tracks, reverb)
+        r = _mix_or_plain_request(c, perturbed_tracks, reverb, generated_rir)
         if r is None:
             return None
         reqs.append(r)
@@ -812,6 +817,7 @@ class MixBatch:
     pre_elems: int = 0                        # the reverberated cuts' mixes, after the output in the same buffer
     reverb_rirs: Optional[np.ndarray] = None  # engine.REVERB_RIR_DTYPE
     reverb_cuts: Optional[np.ndarray] = None  # engine.REVERB_CUT_DTYPE, reading and writing that buffer
+    generated: Optional["GeneratedRirs"] = None  # the generated RIRs of the batch and of its perturbed tracks
 
 
 class MixStagingRing(_PinnedRing):
@@ -842,6 +848,8 @@ class MixStagingRing(_PinnedRing):
         perturbed = [t.source for t in flat if isinstance(t.source, TransformRequest)]
         # the RIRs are at the cut's rate (reverb_request), so one rate per WAV batch still holds
         rirs = _stage_rirs(requests)
+        gen_reqs = _generated_in(requests)
+        generated = GeneratedRirs(gen_reqs) if gen_reqs else None
         pcm_buf, flac_batch, read_kind, read_elem, (wav_srs, flac_srs) = self.sources.stage(
             [flat[i].source for i in ints] + rirs, executor=executor)
         if wav_srs:
@@ -855,7 +863,7 @@ class MixStagingRing(_PinnedRing):
         if perturbed:
             if self.transform is None:
                 self.transform = TransformStagingRing(pin_memory=self._pin)
-            transform_batch, _, offs2, sr2 = self.transform.stage(perturbed, executor=executor)
+            transform_batch, _, offs2, sr2 = self.transform.stage(perturbed, executor=executor, generated=generated)
             src_elem[kind == MIX_SRC_F32] = offs2
             srs.add(sr2)
         B, T = len(requests), len(flat)
@@ -893,11 +901,14 @@ class MixStagingRing(_PinnedRing):
         cuts["reserved"] = 0
         batch = MixBatch(pcm=pcm_buf, flac=flac_batch, tracks=tracks, cuts=cuts, lens=lens, offsets=offs, out_elems=out_elems,
                          transform=transform_batch)
+        batch.generated = generated
         if rv_ix:
             batch.pre_elems = base - out_elems + pre_elems
             batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(
                 rirs, read_kind[len(ints):], read_elem[len(ints):],
-                [(requests[i].reverb, mix_out[i], lens[i], offs[i], lens[i]) for i in rv_ix])
+                [(requests[i].reverb, mix_out[i], lens[i], offs[i], lens[i]) for i in rv_ix], generated)
+        if generated is not None:
+            generated.draw()  # after every read of the batch, its perturbed tracks' included
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
 
 
@@ -906,16 +917,18 @@ def mix_staged(batch: MixBatch, device, ring: Optional[_PinnedRing] = None, hand
     perturbed tracks' transform stages into the float32 track buffer (if any), the table copies, the energy and mix kernels,
     the reverb of the reverberated cuts (if any); then `ring`'s copies are marked in flight.  Returns (float32 mixes on
     `device`, lengths, offsets)."""
-    from .engine import mix, reverb
+    from .engine import mix
 
     device = torch.device(device)
     with torch.cuda.device(device):
         src0, src1 = _sources_to_device(batch, device)
-        src2 = transform_staged(batch.transform, device, handle=handle)[0] if batch.transform is not None else None
+        rir32 = _generate_rirs(batch.generated, device, handle) if batch.generated is not None else None
+        src2 = (transform_staged(batch.transform, device, handle=handle, rir32=rir32)[0]
+                if batch.transform is not None else None)
         out = torch.zeros(max(batch.out_elems + batch.pre_elems, 1), dtype=torch.float32, device=device)
         mix(src0, src1, batch.tracks, batch.cuts, out, handle, src2=src2)
         if batch.reverb_cuts is not None:
-            reverb(src0, src1, out, batch.reverb_rirs, batch.reverb_cuts, out, handle)
+            _reverb_with(batch, src0, src1, out, out, handle, rir32)
             out = out[: max(batch.out_elems, 1)]
         if ring is not None:
             ring.mark_in_flight(device)
@@ -923,15 +936,17 @@ def mix_staged(batch: MixBatch, device, ring: Optional[_PinnedRing] = None, hand
 
 
 def mix_cuts(cuts, device="cuda", executor=None, ring: Optional[MixStagingRing] = None,
-             perturbed_tracks: bool = False, reverb: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
+             perturbed_tracks: bool = False, reverb: bool = False,
+             generated_rir: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
     """Mixes MixedCuts (and plain 16-bit WAV / FLAC slices) on the GPU: (float32 device tensor holding every cut's samples at
     its offset, on 4-sample boundaries, lengths, offsets), each cut bit-identical to float32(cut.load_audio()).  Raises
     ValueError naming the first cut the route cannot take.  `perturbed_tracks=True` also takes tracks (and plain cuts) with
     Speed / Volume / Resample chains, run on the GPU into a float32 track buffer first (see `mix_request_for_cut`; off by
     default, so that existing callers keep their behaviour until H100 measurements of the route exist).  `reverb=True` also
     takes MixedCut-level reverbs and plain slices whose only transform is a reverb, reverberated on the GPU within a float32
-    tolerance of a float64 convolution (see `mix_request_for_cut`; off by default)."""
-    reqs = _requests_or_raise(cuts, lambda c: _mix_or_plain_request(c, perturbed_tracks, reverb),
+    tolerance of a float64 convolution (see `mix_request_for_cut`; off by default).  `generated_rir=True` takes those reverbs
+    with RIRs that lhotse generates, drawn here from the cuts' generators (rir_draws.py; off by default)."""
+    reqs = _requests_or_raise(cuts, lambda c: _mix_or_plain_request(c, perturbed_tracks, reverb, generated_rir),
                               "cannot be mixed on the GPU (see mix_request_for_cut)")
     ring = ring or MixStagingRing()
     batch, _, _, _ = ring.stage(reqs, executor=executor)
@@ -1069,8 +1084,15 @@ def resample_probe(orig: int, new: int) -> bool:
 
 @dataclass(frozen=True)
 class ReverbRequest:
-    rir: object                # PcmRequest | FlacRequest: the RIR's samples, what `rir.load_audio()` reads
+    rir: object                # PcmRequest | FlacRequest: the RIR's samples, what `rir.load_audio()` reads; or a GeneratedRirRequest
     normalize: bool            # lhotse's normalize_output
+
+
+@dataclass(frozen=True, eq=False)
+class GeneratedRirRequest:
+    """An RIR that lhotse's FastRandomRIRGenerator `generator` makes when the cut is loaded (no recorded RIR): drawn on the host
+    when the batch is staged (rir_draws.py) and built on the GPU (csrc/rirgen.cuh).  Every request is its own RIR."""
+    generator: object
 
 
 @dataclass(frozen=True)
@@ -1082,18 +1104,33 @@ class TransformRequest:
     reverb: Optional[ReverbRequest] = None  # a last ReverbWithImpulseResponse, run on the chain's output before the length fix
 
 
-def reverb_request(t, sampling_rate: int) -> Optional[ReverbRequest]:
+def reverb_request(t, sampling_rate: int, reverb: bool = True, generated_rir: bool = False) -> Optional[ReverbRequest]:
     """The RIR read of a ReverbWithImpulseResponse with a recorded mono RIR, as its __call__ loads it: `rir.to_cut()` for a
     Recording, `with_channels(rir_channels)`, `truncate(duration=0.05)` when early_only, then a cut that
     `pcm16_request_for_cut` / `flac_request_for_cut` accept, with no transforms of its own and 1 <= R <= REVERB_MAX_RIR
-    samples, at `sampling_rate` (the cut's).  None otherwise: the RIR generator, several RIR channels (a MultiCut), other
-    formats, longer RIRs, an RIR at another rate (lhotse convolves it as it is stored; this route does not take it)."""
+    samples, at `sampling_rate` (the cut's).  None otherwise: several RIR channels (a MultiCut), other formats, longer RIRs,
+    an RIR at another rate (lhotse convolves it as it is stored; this route does not take it).  `reverb=False` refuses
+    recorded RIRs.
+
+    `generated_rir=True` also takes a ReverbWithImpulseResponse with no RIR whose generator `rir_draws.generator_eligible`
+    accepts (exactly lhotse's FastRandomRIRGenerator, torchaudio present, float32 default dtype, a restatement of torch's
+    multinomial that holds here), one RIR channel and RIRs of at most REVERB_MAX_RIR samples; lhotse ignores early_only
+    for a generated RIR, and so does this route."""
     from lhotse import Recording
     from lhotse.cut import MonoCut
 
     from .engine import REVERB_MAX_RIR
 
-    if t.rir is None or len(t.rir_channels) != 1:
+    if len(t.rir_channels) != 1:
+        return None
+    if t.rir is None:
+        from . import rir_draws
+
+        gen = getattr(t, "rir_generator", None)
+        if not generated_rir or not rir_draws.generator_eligible(gen) or rir_draws.max_rir_len(gen) > REVERB_MAX_RIR:
+            return None
+        return ReverbRequest(rir=GeneratedRirRequest(gen), normalize=bool(t.normalize_output))
+    if not reverb:
         return None
     try:
         rir = t.rir.to_cut() if isinstance(t.rir, Recording) else t.rir
@@ -1110,7 +1147,7 @@ def reverb_request(t, sampling_rate: int) -> Optional[ReverbRequest]:
     return ReverbRequest(rir=src, normalize=bool(t.normalize_output))
 
 
-def transform_request_for_cut(cut, reverb: bool = False) -> Optional[TransformRequest]:
+def transform_request_for_cut(cut, reverb: bool = False, generated_rir: bool = False) -> Optional[TransformRequest]:
     """What `cut.load_audio()` (audio/recording.py load_audio) amounts to for a MonoCut over a single-channel 16-bit WAV or
     FLAC file whose recording carries a non-empty chain of Speed, Volume and Resample transforms: the source slice (the
     transforms' own reverse_timestamps applied to the cut's range, a read to the end of the file when the cut's duration is
@@ -1122,7 +1159,8 @@ def transform_request_for_cut(cut, reverb: bool = False) -> Optional[TransformRe
     `reverb=True` also takes a chain whose last transform is a ReverbWithImpulseResponse that `reverb_request` accepts (a
     reverb alone included): the stages before it write the pre-reverb signal, and the reverb kernel (csrc/reverb.cuh) writes
     the cut, within a float32 tolerance of a float64 convolution rather than bit for bit (DESIGN.md §3.1j).  Off by default
-    so that existing callers keep exactly the routes and samples they have."""
+    so that existing callers keep exactly the routes and samples they have.  `generated_rir=True` takes such a last
+    reverb with an RIR that lhotse generates (see `reverb_request`; DESIGN.md §3.1l), also off by default."""
     try:
         from lhotse.augmentation.rir import ReverbWithImpulseResponse
         from lhotse.audio.resampling_backend import get_current_resampling_backend
@@ -1141,8 +1179,8 @@ def transform_request_for_cut(cut, reverb: bool = False) -> Optional[TransformRe
         return None  # lhotse's table phases and output lengths are evaluated in the default dtype
     tfs = [t if isinstance(t, AudioTransform) else AudioTransform.from_dict(t) for t in rec.transforms]
     rv = None
-    if reverb and type(tfs[-1]) is ReverbWithImpulseResponse:
-        rv = reverb_request(tfs[-1], rec.sampling_rate)
+    if (reverb or generated_rir) and type(tfs[-1]) is ReverbWithImpulseResponse:
+        rv = reverb_request(tfs[-1], rec.sampling_rate, reverb, generated_rir)
         if rv is None:
             return None
         tfs = tfs[:-1]
@@ -1199,20 +1237,20 @@ def _has_transforms(cut) -> bool:
     return bool(getattr(getattr(cut, "recording", None), "transforms", None))
 
 
-def transform_requests_for_batch(cuts, reverb: bool = False) -> Optional[List[TransformRequest]]:
+def transform_requests_for_batch(cuts, reverb: bool = False, generated_rir: bool = False) -> Optional[List[TransformRequest]]:
     """The "transform" route's requests for a batch: no MixedCut, every cut a plain 16-bit WAV / FLAC slice or an eligible
     transformed MonoCut, and at least one of the latter (batches of plain slices keep their routes).  None otherwise.
     `reverb=True`: see `transform_request_for_cut`."""
     if any(getattr(c, "tracks", None) is not None for c in cuts) or not any(_has_transforms(c) for c in cuts):
         return None
-    reqs = [_transform_or_plain_request(c, reverb) for c in cuts]
+    reqs = [_transform_or_plain_request(c, reverb, generated_rir) for c in cuts]
     return None if any(r is None for r in reqs) else reqs
 
 
-def _transform_or_plain_request(cut, reverb: bool = False) -> Optional[TransformRequest]:
+def _transform_or_plain_request(cut, reverb: bool = False, generated_rir: bool = False) -> Optional[TransformRequest]:
     """transform_request_for_cut, or a plain 16-bit WAV / FLAC slice as an empty chain (a copy of x = q / 32768)."""
     if _has_transforms(cut):
-        r = transform_request_for_cut(cut, reverb=reverb)
+        r = transform_request_for_cut(cut, reverb=reverb, generated_rir=generated_rir)
     else:
         src = slice_request_for_cut(cut)
         r = (TransformRequest(source=src, ops=(), num_samples=int(src.num_samples), sampling_rate=int(cut.sampling_rate))
@@ -1255,6 +1293,7 @@ class TransformBatch:
     out_elems: int
     reverb_rirs: Optional[np.ndarray] = None  # engine.REVERB_RIR_DTYPE: the batch's distinct RIRs in the two int16 sources
     reverb_cuts: Optional[np.ndarray] = None  # engine.REVERB_CUT_DTYPE: the reverberated cuts, reading `mid`
+    generated: Optional["GeneratedRirs"] = None  # the generated RIRs, after the recorded ones in `reverb_rirs`
 
 
 def _stage_rirs(reqs) -> List[_SliceRequest]:
@@ -1263,22 +1302,123 @@ def _stage_rirs(reqs) -> List[_SliceRequest]:
     rirs = {}
     for r in reqs:
         rv = getattr(r, "reverb", None)
-        if rv is not None:
+        if rv is not None and not isinstance(rv.rir, GeneratedRirRequest):
             rirs.setdefault(rv.rir, None)
     return list(rirs)
 
 
-def _reverb_tables(rirs, source, rir_elem, cuts) -> Tuple[np.ndarray, np.ndarray]:
-    """The b200feat_reverb tables: RIR i in int16 source source[i] at rir_elem[i]; cuts = [(ReverbRequest, in_elem, in_len,
-    out_elem, target_len)]."""
-    from .engine import REVERB_CUT_DTYPE, REVERB_RIR_DTYPE
+class GeneratedRirs:
+    """The generated RIRs of one staged batch, in batch order: each one's place in the float32 RIR buffer (room for the
+    longest RIR its generator can give, so that the places are known before the draws), and once `draw` has run, the draws
+    (rir_draws.RirDraws) and the generator states from before them."""
 
-    rt = np.zeros(len(rirs), dtype=REVERB_RIR_DTYPE)
+    ALIGN = 4
+
+    def __init__(self, reqs: Sequence[GeneratedRirRequest]):
+        from . import rir_draws
+
+        self.reqs = list(reqs)
+        self.index = {id(r): i for i, r in enumerate(self.reqs)}
+        self.elems, self.elems_total = _aligned_offsets([rir_draws.max_rir_len(r.generator) for r in self.reqs], self.ALIGN)
+        self.draws = None
+        self.snapshot = None
+
+    def draw(self) -> None:
+        """Draws every RIR, after saving the state of every generator the draws touch (see `undo_draws`)."""
+        from . import rir_draws
+
+        gens = [r.generator for r in self.reqs]
+        self.snapshot = rir_draws.snapshot(gens)
+        try:
+            self.draws = rir_draws.draw(gens)
+        except BaseException:
+            self.undo()
+            raise
+
+    def undo(self) -> None:
+        from . import rir_draws
+
+        rir_draws.restore(self.snapshot)
+        self.snapshot, self.draws = None, None
+
+
+def _generated_in(reqs) -> List[GeneratedRirRequest]:
+    """The generated RIRs of `reqs` (TransformRequests, or MixRequests whose perturbed tracks may carry one), in batch order."""
+    out = []
+    for r in reqs:
+        for t in getattr(r, "tracks", ()):
+            rv = getattr(t.source, "reverb", None)
+            if rv is not None and isinstance(rv.rir, GeneratedRirRequest):
+                out.append(rv.rir)
+        rv = getattr(r, "reverb", None)
+        if rv is not None and isinstance(rv.rir, GeneratedRirRequest):
+            out.append(rv.rir)
+    return out
+
+
+def undo_draws(staged) -> None:
+    """Restores the generator states from before the draws of a staged batch that will not be used (the batch falls back
+    to the float route, which then draws the same numbers); nothing for a batch without generated RIRs."""
+    gen = getattr(staged, "generated", None)
+    if gen is not None:
+        gen.undo()
+
+
+def _generate_rirs(gen: GeneratedRirs, device, handle=None) -> torch.Tensor:
+    """The device half of the generated RIRs on the current stream: the draws' upload, b200feat_rir_generate at 8 x sr, then
+    b200feat_resample with lhotse's 8 -> 1 table to sr.  Returns the float32 RIR buffer (RIR i at gen.elems[i])."""
+    from .engine import RESAMPLE_MID, RESAMPLE_STAGE_DTYPE, RESAMPLE_TO_OUT, resample, resample_table, rir_generate
+
+    d = gen.draws
+    rec = d.records.copy()
+    lens8 = [int(n) for n in rec["out_len"]]
+    offs8, total8 = _aligned_offsets(lens8, GeneratedRirs.ALIGN)
+    rec["out_elem"] = offs8
+    table, width = resample_kernel(8, 1)
+    draws = torch.from_numpy(d.draws).to(device)
+    cdf = torch.from_numpy(d.cdf).to(device)
+    mid = torch.empty(max(total8, 1), dtype=torch.float32, device=device)
+    rir_generate(draws, cdf, table[0], rec, mid, handle)
+    st = np.zeros(len(rec), dtype=RESAMPLE_STAGE_DTYPE)
+    st["struct_size"] = RESAMPLE_STAGE_DTYPE.itemsize
+    st["table"] = resample_table(8, 1, table, width, device, handle)
+    st["source"], st["target"], st["scale_in"], st["scale_out"] = RESAMPLE_MID, RESAMPLE_TO_OUT, 1.0, 1.0
+    st["in_elem"], st["in_len"] = offs8, lens8
+    st["out_elem"], st["out_len"], st["target_len"] = gen.elems, d.lens, d.lens
+    out = torch.zeros(max(gen.elems_total, 1), dtype=torch.float32, device=device)
+    resample(None, None, mid, st, out, handle)
+    return out
+
+
+def _reverb_with(batch, src0, src1, x, out, handle, rir32) -> None:
+    """b200feat_reverb_ex over a staged batch's reverb tables, the generated RIRs' lengths filled in from their draws."""
+    from .engine import reverb
+
+    rt = batch.reverb_rirs
+    if batch.generated is not None:
+        rt = rt.copy()
+        rt["num_samples"][len(rt) - len(batch.generated.reqs):] = batch.generated.draws.lens
+    reverb(src0, src1, x, rt, batch.reverb_cuts, out, handle, rir32=rir32)
+
+
+def _reverb_tables(rirs, source, rir_elem, cuts, generated: Optional[GeneratedRirs] = None) -> Tuple[np.ndarray, np.ndarray]:
+    """The b200feat_reverb_ex tables: RIR i in int16 source source[i] at rir_elem[i], then the generated RIRs of `generated`
+    (their lengths filled in by `_reverb_with` once drawn); cuts = [(ReverbRequest, in_elem, in_len, out_elem,
+    target_len)]."""
+    from .engine import REVERB_CUT_DTYPE, REVERB_RIR_DTYPE, REVERB_RIR_F32
+
+    ng = len(generated.reqs) if generated is not None else 0
+    rt = np.zeros(len(rirs) + ng, dtype=REVERB_RIR_DTYPE)
     rt["struct_size"] = REVERB_RIR_DTYPE.itemsize
-    rt["source"] = source
-    rt["src_elem"] = rir_elem
-    rt["num_samples"] = [r.num_samples for r in rirs]
+    rt["source"][: len(rirs)] = source
+    rt["src_elem"][: len(rirs)] = rir_elem
+    rt["num_samples"][: len(rirs)] = [r.num_samples for r in rirs]
+    if ng:
+        rt["source"][len(rirs):] = REVERB_RIR_F32
+        rt["src_elem"][len(rirs):] = generated.elems
     ix = {r: i for i, r in enumerate(rirs)}
+    if ng:
+        ix.update({r: len(rirs) + i for i, r in enumerate(generated.reqs)})
     ct = np.zeros(len(cuts), dtype=REVERB_CUT_DTYPE)
     ct["struct_size"] = REVERB_CUT_DTYPE.itemsize
     ct["rir"] = [ix[rv.rir] for rv, *_ in cuts]
@@ -1304,12 +1444,19 @@ class TransformStagingRing(_PinnedRing):
         super().mark_in_flight(device)
         self.sources.mark_in_flight(device)
 
-    def stage(self, requests: Sequence[TransformRequest], executor=None) -> Tuple[TransformBatch, List[int], List[int], Optional[int]]:
+    def stage(self, requests: Sequence[TransformRequest], executor=None,
+              generated: Optional[GeneratedRirs] = None) -> Tuple[TransformBatch, List[int], List[int], Optional[int]]:
+        """`generated`: the generated RIRs of an enclosing mix batch, which draws them; without it the generated RIRs of
+        `requests` are drawn here, after the reads."""
         from .engine import RESAMPLE_MID, RESAMPLE_STAGE_DTYPE, RESAMPLE_TO_MID, RESAMPLE_TO_OUT
 
         self._wait_idle()
         B = len(requests)
         rirs = _stage_rirs(requests)
+        gen_reqs = _generated_in(requests)
+        own = generated is None and bool(gen_reqs)
+        if own:
+            generated = GeneratedRirs(gen_reqs)
         pcm_buf, flac_batch, kind, src_elem, _ = self.sources.stage([r.source for r in requests] + rirs, executor=executor)
         srs = {r.sampling_rate for r in requests}
         lens = [int(r.num_samples) for r in requests]
@@ -1354,16 +1501,20 @@ class TransformStagingRing(_PinnedRing):
         batch = TransformBatch(pcm=pcm_buf, flac=flac_batch, stages=st, pair=np.asarray(cols[2], dtype=np.int64), pairs=pairs,
                                mid_elems=mid, lens=lens, offsets=offs, out_elems=out_elems)
         if rv_cuts:
-            batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(rirs, kind[B:], src_elem[B:], rv_cuts)
+            batch.generated = generated if gen_reqs else None
+            batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(rirs, kind[B:], src_elem[B:], rv_cuts, batch.generated)
+        if own:
+            generated.draw()
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
 
 
-def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] = None,
-                     handle=None) -> Tuple[torch.Tensor, List[int], List[int]]:
+def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] = None, handle=None,
+                     rir32: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
     """The device half of the "transform" route on the current stream: the rate pairs' tables (built and uploaded once per
     device), H2D of the WAV slices, the FLAC decode (if any), the resampling stages, the reverb (if any); then `ring`'s copies
-    are marked in flight.  Returns (float32 samples on `device`, lengths, offsets)."""
-    from .engine import resample, resample_table, reverb
+    are marked in flight.  Returns (float32 samples on `device`, lengths, offsets).  The generated RIRs are built first
+    unless `rir32` holds them (an enclosing mix batch built them)."""
+    from .engine import resample, resample_table
 
     device = torch.device(device)
     with torch.cuda.device(device):
@@ -1375,20 +1526,24 @@ def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] 
         out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
         resample(src0, src1, mid, batch.stages, out, handle)
         if batch.reverb_cuts is not None:
-            reverb(src0, src1, mid, batch.reverb_rirs, batch.reverb_cuts, out, handle)
+            if batch.generated is not None and rir32 is None:
+                rir32 = _generate_rirs(batch.generated, device, handle)
+            _reverb_with(batch, src0, src1, mid, out, handle, rir32)
         if ring is not None:
             ring.mark_in_flight(device)
     return out, batch.lens, batch.offsets
 
 
 def transform_cuts(cuts, device="cuda", executor=None, ring: Optional[TransformStagingRing] = None,
-                   reverb: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
+                   reverb: bool = False, generated_rir: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
     """Loads speed-perturbed, volume-perturbed and resampled cuts (and plain 16-bit WAV / FLAC slices) with the transforms run
     on the GPU: (float32 device tensor holding every cut's samples at its offset, on 4-sample boundaries, lengths, offsets),
     each cut bit-identical to float32(cut.load_audio()).  Raises ValueError naming the first cut the route cannot take.
     `reverb=True` also takes chains that end in a ReverbWithImpulseResponse with a recorded RIR, reverberated on the GPU
-    within a float32 tolerance of a float64 convolution (see `transform_request_for_cut`; off by default)."""
-    reqs = _requests_or_raise(cuts, lambda c: _transform_or_plain_request(c, reverb),
+    within a float32 tolerance of a float64 convolution (see `transform_request_for_cut`; off by default).
+    `generated_rir=True` takes such chains whose RIR lhotse generates, drawn here from the cuts' generators (rir_draws.py;
+    off by default)."""
+    reqs = _requests_or_raise(cuts, lambda c: _transform_or_plain_request(c, reverb, generated_rir),
                               "cannot be loaded on the GPU (see transform_request_for_cut)")
     ring = ring or TransformStagingRing()
     batch, _, _, _ = ring.stage(reqs, executor=executor)
@@ -1400,17 +1555,20 @@ def transform_cuts(cuts, device="cuda", executor=None, ring: Optional[TransformS
 STAGED_ROUTES = ("pcm16", "flac", "mix", "transform")
 
 
-def staged_route(cuts, perturbed_tracks: bool = False, reverb: bool = False) -> Optional[Tuple[str, list]]:
+def staged_route(cuts, perturbed_tracks: bool = False, reverb: bool = False,
+                 generated_rir: bool = False) -> Optional[Tuple[str, list]]:
     """(route, requests) of the staged route that takes the batch, the route one of STAGED_ROUTES; None when the cuts have
     more than one sampling rate or no staged route takes them.  A batch with a MixedCut can only go to "mix", else one with
     recording transforms only to "transform"; a batch of plain slices goes to "pcm16" when they are all WAV, to "flac" when
-    they are all FLAC.  `perturbed_tracks` and `reverb`: see `mix_request_for_cut` and `transform_request_for_cut`."""
+    they are all FLAC.  `perturbed_tracks`, `reverb` and `generated_rir`: see `mix_request_for_cut` and
+    `transform_request_for_cut`."""
     if len({c.sampling_rate for c in cuts}) != 1:
         return None
     if any(getattr(c, "tracks", None) is not None for c in cuts):
-        route, reqs = "mix", mix_requests_for_batch(cuts, perturbed_tracks=perturbed_tracks, reverb=reverb)
+        route, reqs = "mix", mix_requests_for_batch(cuts, perturbed_tracks=perturbed_tracks, reverb=reverb,
+                                                    generated_rir=generated_rir)
     elif any(_has_transforms(c) for c in cuts):
-        route, reqs = "transform", transform_requests_for_batch(cuts, reverb=reverb)
+        route, reqs = "transform", transform_requests_for_batch(cuts, reverb=reverb, generated_rir=generated_rir)
     else:
         reqs = [slice_request_for_cut(c) for c in cuts]
         route = {PcmRequest: "pcm16", FlacRequest: "flac"}.get(type(reqs[0]))

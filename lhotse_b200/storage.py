@@ -227,6 +227,7 @@ def compute_and_store_features_fused(
     pcm16_fast_path: bool = True,
     perturbed_tracks: bool = False,
     reverb: bool = False,
+    generated_rir: bool = False,
 ):
     """`CutSet.compute_and_store_features_batch(extractor, storage_path, manifest_path, batch_duration, num_workers,
     overwrite=...)` (lhotse/cut/set.py:2197-2408) with the batch kept whole from the GPU to the disk: one packed
@@ -242,7 +243,8 @@ def compute_and_store_features_fused(
     measurements of it decide the default.  `reverb=True` lets the "transform" and "mix" stages also take cuts reverberated
     with a recorded RIR (`pcm_staging.transform_request_for_cut`, `mix_request_for_cut`); off by default because those
     samples match the float route within a float32 tolerance, not bit for bit (the float route's own convolution is not
-    bit-reproducible), until H100 measurements of it decide the default."""
+    bit-reproducible), until H100 measurements of it decide the default.  `generated_rir=True` does the same for cuts whose
+    RIR lhotse generates (`pcm_staging.reverb_request`, DESIGN.md §3.1l); off by default for the same reason."""
     import json
     import queue
     import threading
@@ -256,7 +258,7 @@ def compute_and_store_features_fused(
     from lhotse.qa import validate_features
     from lhotse.utils import fastcopy
 
-    from .pcm_staging import STAGED_ROUTES, new_ring, staged_route
+    from .pcm_staging import STAGED_ROUTES, new_ring, staged_route, undo_draws
 
     register_with_lhotse()
     frame_shift = extractor.frame_shift
@@ -326,7 +328,8 @@ def compute_and_store_features_fused(
             sr = batch_cuts[0].sampling_rate
             assert all(c.sampling_rate == sr for c in batch_cuts)
             item = None
-            chosen = staged_route(batch_cuts, perturbed_tracks=perturbed_tracks, reverb=reverb) if use_ring else None
+            chosen = (staged_route(batch_cuts, perturbed_tracks=perturbed_tracks, reverb=reverb, generated_rir=generated_rir)
+                      if use_ring else None)
             if chosen is not None:
                 kind, reqs = chosen
                 free = free_rings[kind]
@@ -335,6 +338,7 @@ def compute_and_store_features_fused(
                 if fsr == sr:
                     item = (kind, batch_cuts, sr, ring, staged, lens, offs)
                 else:
+                    undo_draws(staged)  # the float route draws the generated RIRs again
                     free.put(ring)
             if item is None:
                 audios, batch_cuts = read_audio_from_cuts(batch_cuts, executor=pool)
