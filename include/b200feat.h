@@ -467,7 +467,8 @@ typedef struct b200feat_rir_gen {
   int32_t sampling_rate; /* the generator's sr, 1 .. 192000: 2 sr image sources, a comb at 64 sr */
   double t60;            /* room_rng's T60 draw, > 0 */
   double r;              /* room_rng's R draw */
-  double d0;             /* source_rng's distance draw, > 0 */
+  double d0;             /* source_rng's distance draw, > 0 and below 340 t60 (f32(340 t60 / d0 - 1) > 0: the last image
+                            ratio; lhotse's draws always are, d0 <= 12 < 34 <= 340 t60), or the record is refused */
   double tau;            /* the generator's tau */
   float b0, b1, b2, a1, a2;  /* highpass_biquad(., 8 sr, 80)'s coefficients divided by a0, as torchaudio's lfilter takes them */
   int32_t reserved;

@@ -1392,11 +1392,22 @@ struct RgLayout {
   int end_bit;
 };
 
+// Whether every image ratio of the record is positive: rg_room's lin_end, the last one, computed by the same code.  With
+// lin_end <= 0 (d0 >= 340 T60) some distances would be <= 0 and their comb positions negative, which the sort (keys of end_bit
+// bits) and the window's table lookup do not take.
+bool rg_ratios_ok(const b200feat_rir_gen &g) {
+  RgRir r{};
+  r.t60 = g.t60;
+  r.d0 = g.d0;
+  return rg_room(r).lin_end > 0.0f;
+}
+
 // Whether the record is one b200feat_rir_generate takes (the buffer bounds are checked by the call)
 bool rg_record_ok(const b200feat_rir_gen &g) {
   return g.struct_size == (int32_t)sizeof(b200feat_rir_gen) && g.sampling_rate >= 1 && g.sampling_rate <= 192000 &&
          g.t60 > 0.0 && g.d0 > 0.0 && isfinite(g.t60) && isfinite(g.r) && isfinite(g.d0) && isfinite(g.tau) &&
-         g.comb_len >= 1 && g.comb_len <= 0x7fffffff && g.out_len >= 1 && g.out_len <= g.comb_len / RG_O + 1;
+         g.comb_len >= 1 && g.comb_len <= 0x7fffffff && g.out_len >= 1 && g.out_len <= g.comb_len / RG_O + 1 &&
+         rg_ratios_ok(g);
 }
 
 // false when a record is malformed or the entries do not fit the sort's int offsets
@@ -1453,6 +1464,9 @@ int b200feat_rir_generate(b200feat_handle *h, const double *draws_dev, int64_t d
     const b200feat_rir_gen &g = rirs[i];
     if (g.struct_size != (int32_t)sizeof(b200feat_rir_gen))
       return fail(h, B200FEAT_EINVAL, where(i) + "b200feat_rir_gen size mismatch (ABI)");
+    if (g.t60 > 0.0 && g.d0 > 0.0 && isfinite(g.t60) && isfinite(g.d0) && !rg_ratios_ok(g))
+      return fail(h, B200FEAT_EINVAL, where(i) + "d0 must be below 340 T60 (its last image ratio 340 T60 / d0 - 1 is not "
+                                                 "positive)");
     if (!rg_record_ok(g))
       return fail(h, B200FEAT_EINVAL, where(i) + "bad sampling rate, draws or lengths (T60 and d0 must be positive, "
                                                  "out_len at most comb_len / 8 + 1)");

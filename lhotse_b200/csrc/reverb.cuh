@@ -103,7 +103,9 @@ MIX_HD rv_c rv_cmac(rv_c acc, rv_c a, rv_c b) {
 // RIR sample i before lhotse's 2^-15 scaling: f32(q / 32768) for an int16 RIR, the float32 sample itself otherwise
 MIX_HD float rv_rir_value(const RvRir &r, int64_t i) { return r.src32 ? r.src32[i] : mix_widen(r.src[i]); }
 
-// RIR sample k of partition p as its spectrum takes it: h * 2^-15 * (1 / RV_F), exact; 0 past the RIR
+// RIR sample k of partition p as its spectrum takes it: h * 2^-15 * (1 / RV_F), 0 past the RIR.  Exact for every int16 RIR
+// and for float32 samples with |h| >= 2^-99; below that the product is subnormal and rounded once (no flush to zero: the
+// library is built without -ftz or fast math, so the device rounds as the host does)
 MIX_HD float rv_rir_sample(const RvRir &r, int p, int k) {
   const int64_t i = (int64_t)p * RV_B + k;
   if (k >= RV_B || i >= r.len) return 0.0f;

@@ -3,8 +3,9 @@
 // allocated to its exact size so that AddressSanitizer sees any access outside them.  No GPU needed; the header also
 // compiles as plain C++:
 //   g++ -x c++ -std=c++17 -O1 -g -fsanitize=address -o reverb_host_check scripts/micro/reverb_host_check.cu
-//   ./reverb_host_check src0.i16 rirs.bin cuts.bin in.f32 out.f32
-//        b200feat_reverb over the int16 RIR source (every RIR record's source 0), the b200feat_reverb_rir /
+//   ./reverb_host_check src0.i16 rirs.bin cuts.bin in.f32 out.f32 [rir32.f32]
+//        b200feat_reverb_ex over the int16 RIR source (RIR records of source 0) and, when given, the float32 one (records of
+//        source B200FEAT_REVERB_RIR_F32, read from rir32.f32), the b200feat_reverb_rir /
 //        b200feat_reverb_cut tables and the float32 input buffer (no argument checks: the tables are expected to be valid);
 //        each cut's target_len samples are written back to back to out.f32.  The per-CTA partial sums of y^2 are added in
 //        thread order here (the kernel uses a shuffle tree), so pa may differ from the device in the last bits.
@@ -44,33 +45,40 @@ static void fft(rv_c *a, const rv_c *tw, bool inverse) {
 }
 
 int main(int argc, char **argv) {
-  if (argc != 6) {
-    fprintf(stderr, "usage: %s src0.i16 rirs.bin cuts.bin in.f32 out.f32\n", argv[0]);
+  if (argc != 6 && argc != 7) {
+    fprintf(stderr, "usage: %s src0.i16 rirs.bin cuts.bin in.f32 out.f32 [rir32.f32]\n", argv[0]);
     return 2;
   }
   const std::vector<int16_t> s0 = load<int16_t>(argv[1]);
   const std::vector<b200feat_reverb_rir> rirs = load<b200feat_reverb_rir>(argv[2]);
   const std::vector<b200feat_reverb_cut> cuts = load<b200feat_reverb_cut>(argv[3]);
   const std::vector<float> in = load<float>(argv[4]);
+  const std::vector<float> s32 = argc == 7 ? load<float>(argv[6]) : std::vector<float>();
   std::vector<rv_c> tw(RV_B), a(RV_F);
   for (int k = 0; k < RV_B; ++k) tw[k] = rv_twiddle(k);
   // the RIR kernel: spectra and shifts
   std::vector<RvRir> rv(rirs.size());
-  std::vector<int16_t *> rir_mem(rirs.size());
+  std::vector<int16_t *> rir_mem(rirs.size(), nullptr);
+  std::vector<float *> rir32_mem(rirs.size(), nullptr);
   std::vector<std::vector<rv_c>> spectra(rirs.size());
   std::vector<int64_t> shift(rirs.size());
   for (size_t i = 0; i < rirs.size(); ++i) {
-    rir_mem[i] = exact_copy(s0, rirs[i].src_elem, rirs[i].num_samples);
-    rv[i] = RvRir{rir_mem[i], rirs[i].num_samples, 0, (int32_t)rv_parts(rirs[i].num_samples), 0};
+    if (rirs[i].source == B200FEAT_REVERB_RIR_F32)
+      rir32_mem[i] = exact_copy(s32, rirs[i].src_elem, rirs[i].num_samples);
+    else
+      rir_mem[i] = exact_copy(s0, rirs[i].src_elem, rirs[i].num_samples);
+    rv[i] = RvRir{rir_mem[i], rirs[i].num_samples, 0, (int32_t)rv_parts(rirs[i].num_samples), 0, rir32_mem[i]};
     spectra[i].resize((size_t)rv[i].nparts * RV_F);
     for (int p = 0; p < rv[i].nparts; ++p) {
       for (int m = 0; m < RV_F; ++m) a[rv_bitrev(m)] = rv_c{rv_rir_sample(rv[i], p, m), 0.0f};
       fft(a.data(), tw.data(), false);
       memcpy(&spectra[i][(size_t)p * RV_F], a.data(), sizeof(rv_c) * RV_F);
     }
-    int best = -32769;
-    for (int64_t k = 0; k < rv[i].len; ++k)
-      if (rv[i].src[k] > best) { best = rv[i].src[k]; shift[i] = k; }
+    // the first index of the maximum, on the widened samples
+    shift[i] = 0;
+    float best = rv_rir_value(rv[i], 0);
+    for (int64_t k = 1; k < rv[i].len; ++k)
+      if (rv_rir_value(rv[i], k) > best) { best = rv_rir_value(rv[i], k); shift[i] = k; }
   }
   FILE *fo = fopen(argv[5], "wb");
   if (!fo) { fprintf(stderr, "cannot write %s\n", argv[5]); return 2; }
@@ -109,6 +117,7 @@ int main(int argc, char **argv) {
   }
   fclose(fo);
   for (int16_t *p : rir_mem) free(p);
+  for (float *p : rir32_mem) free(p);
   printf("reverb: %zu cuts, %zu rirs, %lld ctas\n", cuts.size(), rirs.size(), (long long)ctas);
   return 0;
 }

@@ -31,14 +31,32 @@ def harness(tmp_path_factory):
     pytest.skip("no host C++ compiler")
 
 
-def run_harness(exe, tmp_path, rirs, cuts):
-    """rirs: [int16 array]; cuts: [(float32 x, rir index, normalize, target_len)] -> [float32 output per cut]."""
-    from lhotse_b200.engine import REVERB_CUT_DTYPE, REVERB_RIR_DTYPE
+def rir_records(rirs):
+    """The b200feat_reverb_rir table of `rirs` and its two sources: int16 arrays back to back in source 0, float32 arrays
+    (REVERB_RIR_F32) back to back in the float32 source."""
+    from lhotse_b200.engine import REVERB_RIR_DTYPE, REVERB_RIR_F32
 
     rt = np.zeros(len(rirs), REVERB_RIR_DTYPE)
     rt["struct_size"] = REVERB_RIR_DTYPE.itemsize
     rt["num_samples"] = [len(q) for q in rirs]
-    rt["src_elem"] = np.concatenate(([0], np.cumsum([len(q) for q in rirs])[:-1]))
+    f32 = np.asarray([q.dtype == np.float32 for q in rirs], bool)
+    rt["source"] = np.where(f32, REVERB_RIR_F32, 0)
+    for kind in (False, True):
+        lens = np.asarray([len(q) if f == kind else 0 for q, f in zip(rirs, f32)], np.int64)
+        at = np.concatenate(([0], np.cumsum(lens)[:-1]))
+        rt["src_elem"][f32 == kind] = at[f32 == kind]
+    s0 = [q.astype(np.int16) for q, f in zip(rirs, f32) if not f]
+    s32 = [q for q, f in zip(rirs, f32) if f]
+    return (rt, np.concatenate(s0) if s0 else np.zeros(0, np.int16),
+            np.concatenate(s32) if s32 else np.zeros(0, np.float32))
+
+
+def run_harness(exe, tmp_path, rirs, cuts):
+    """rirs: [int16 array, or float32 array for the float32 source]; cuts: [(float32 x, rir index, normalize, target_len)]
+    -> [float32 output per cut]."""
+    from lhotse_b200.engine import REVERB_CUT_DTYPE
+
+    rt, s0, s32 = rir_records(rirs)
     ct = np.zeros(len(cuts), REVERB_CUT_DTYPE)
     ct["struct_size"] = REVERB_CUT_DTYPE.itemsize
     ct["rir"] = [c[1] for c in cuts]
@@ -46,13 +64,16 @@ def run_harness(exe, tmp_path, rirs, cuts):
     ct["in_len"] = [len(c[0]) for c in cuts]
     ct["in_elem"] = np.concatenate(([0], np.cumsum([len(c[0]) for c in cuts])[:-1]))
     ct["target_len"] = [c[3] for c in cuts]
-    np.concatenate(rirs).astype(np.int16).tofile(tmp_path / "s0.i16")
+    s0.tofile(tmp_path / "s0.i16")
     rt.tofile(tmp_path / "rirs.bin")
     ct.tofile(tmp_path / "cuts.bin")
     np.concatenate([c[0] for c in cuts]).astype(np.float32).tofile(tmp_path / "in.f32")
+    files = ["s0.i16", "rirs.bin", "cuts.bin", "in.f32", "out.f32"]
+    if len(s32):
+        s32.tofile(tmp_path / "rir32.f32")
+        files.append("rir32.f32")
     env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:abort_on_error=0")
-    r = subprocess.run([exe, *(str(tmp_path / f) for f in ("s0.i16", "rirs.bin", "cuts.bin", "in.f32", "out.f32"))],
-                       capture_output=True, text=True, env=env)
+    r = subprocess.run([exe, *(str(tmp_path / f) for f in files)], capture_output=True, text=True, env=env)
     assert r.returncode == 0 and "AddressSanitizer" not in r.stderr, r.stdout[-2000:] + r.stderr[-4000:]
     out = np.fromfile(tmp_path / "out.f32", np.float32)
     ends = np.cumsum([c[3] for c in cuts])
