@@ -150,7 +150,8 @@ MIX_HD float sa_mean(const double *partial, int tiles, int64_t count) {
   return MIX_D2F(MIX_DDIV(s, (double)count));
 }
 
-// T * F < 2^31 (b200feat_specaug checks), so a rectangle's element count and offsets fit an int
+// T * F < 2^31 (b200feat_specaug checks), so a rectangle's element count and offsets, and a tile's unit count, fit an int;
+// the kernels' strided loop counters, which step past them, are 64-bit
 MIX_HD int sa_mask_elems(const SaMask &m, int T, int F) { return (m.end - m.start) * (m.axis == 0 ? F : T); }
 
 // element i of a rectangle, as an offset into its sequence
@@ -177,7 +178,8 @@ __global__ void __launch_bounds__(SA_THREADS) specaug_warp_kernel(const float *_
   float *dst = out + (int64_t)b * T * F;
   const int units = sa_tile_units(T, F, V, tile);
   double acc = 0.0;
-  for (int u = threadIdx.x; u < units; u += SA_THREADS) acc = sa_unit<V>(src, dst, F, warps, wb, we, row0, u, acc);
+  // a 64-bit counter: with T = 1 and F near 2^31 a CTA has up to 2^31 - 1 units, and u + SA_THREADS would wrap an int
+  for (int64_t u = threadIdx.x; u < units; u += SA_THREADS) acc = sa_unit<V>(src, dst, F, warps, wb, we, row0, (int)u, acc);
   red[threadIdx.x] = acc;
   __syncthreads();
   for (int w = SA_THREADS / 2; w > 0; w >>= 1) {
@@ -201,7 +203,8 @@ __global__ void __launch_bounds__(SA_FILL_THREADS) specaug_fill_kernel(float *__
   const float v = mean[m.seq];
   float *dst = out + (int64_t)m.seq * T * F;
   const int n = sa_mask_elems(m, T, F);
-  for (int i = blockIdx.y * SA_FILL_THREADS + threadIdx.x; i < n; i += gridDim.y * SA_FILL_THREADS)
-    dst[sa_mask_offset(m, F, i)] = v;
+  // a 64-bit counter: i < n < 2^31, but i + gridDim.y * SA_FILL_THREADS would wrap an int past 2^31 - 1
+  for (int64_t i = blockIdx.y * SA_FILL_THREADS + threadIdx.x; i < n; i += gridDim.y * SA_FILL_THREADS)
+    dst[sa_mask_offset(m, F, (int)i)] = v;
 }
 #endif
