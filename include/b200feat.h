@@ -529,6 +529,58 @@ int b200feat_specaug(b200feat_handle *h, const float *in_dev, float *out_dev, in
                      const b200feat_specaug_warp *warps, int32_t nwarps, const b200feat_specaug_mask *masks, int32_t nmasks,
                      void *work_dev, int64_t work_bytes, void *stream);
 
+/*
+ * Feature-domain mixing and right-padding collation of precomputed feature rows on the GPU: what lhotse's collate_features
+ * computes for cuts whose features are stored (MixedCut.load_features with its FeatureMixer, PaddingCut constants, the
+ * padding-only copy), within a float32 rounding of a float64 evaluation of the same tables (DESIGN.md §3.1m).  The stored
+ * rows are float32 elements of one device buffer (row-major, F per row); the output is a padded (B, T_max, F) float32 batch.
+ */
+#define B200FEAT_FEATMIX_LOG 0       /* mix law: log(max(EPSILON, e^a + g e^b)), energy sum e^x, scale x + log g (Fbank family) */
+#define B200FEAT_FEATMIX_LINEAR 1    /* mix law: a + g b, energy sum x, scale g x (Spectrogram) */
+#define B200FEAT_FEATMIX_COPY 0      /* cut mode: its one track's rows as they are, then pad_value up to num_rows */
+#define B200FEAT_FEATMIX_MIX 1       /* cut mode: FeatureMixer over its tracks, in track order */
+#define B200FEAT_FEATMIX_MIXED 1     /* track flag: the track is part of the mix (the cut's first track is the mixer's base) */
+#define B200FEAT_FEATMIX_ENERGY 2    /* track flag: the cut needs the track's energy (its SNR reference, a track with an SNR) */
+
+typedef struct b200feat_featmix_track {
+  int32_t struct_size;   /* sizeof(b200feat_featmix_track) — ABI guard, in every record */
+  int32_t cut;           /* index of the cut the track belongs to */
+  int32_t flags;         /* B200FEAT_FEATMIX_MIXED | B200FEAT_FEATMIX_ENERGY */
+  int32_t stored_rows;   /* rows in the source buffer; 0: a constant track (every element is `value`) */
+  int32_t num_rows;      /* rows the track has: stored_rows, or stored_rows + 1 (the last stored row repeated) */
+  int32_t offset;        /* first mix row of the track (0 for the cut's first track) */
+  float value;           /* the element value of a constant track (a PaddingCut's feat_value as float32) */
+  int32_t reserved;
+  int64_t src_elem;      /* first element of the stored rows in the source buffer */
+  double snr_factor;     /* 10 ** (-snr / 10) as the host evaluates it; NaN: the track has no SNR */
+} b200feat_featmix_track;
+
+typedef struct b200feat_featmix_cut {
+  int32_t struct_size;   /* sizeof(b200feat_featmix_cut) */
+  int32_t mode;          /* B200FEAT_FEATMIX_COPY | B200FEAT_FEATMIX_MIX */
+  int32_t law;           /* B200FEAT_FEATMIX_LOG | B200FEAT_FEATMIX_LINEAR (MIX cuts) */
+  int32_t num_rows;      /* the cut's rows in the output, at most T_max; rows past it are the call's pad_value */
+  int32_t mix_rows;      /* MIX: the mixer's rows (the base's, grown by every further track's offset + rows), within one
+                            row of num_rows: trimmed, or the last mix row repeated */
+  int32_t first_track;   /* the cut's tracks are [first_track, first_track + num_tracks) of the track table, in track order */
+  int32_t num_tracks;    /* COPY: 1 */
+  int32_t ref_track;     /* MIX: the SNR reference, relative to first_track */
+  float pad_value;       /* COPY: the value of rows [track rows, num_rows) */
+  int32_t reserved;
+} b200feat_featmix_cut;
+
+/* Device scratch b200feat_feature_mix needs for `ntracks` tracks and `ncuts` cuts (0 when a count is negative). */
+int64_t b200feat_feature_mix_work_bytes(int32_t ntracks, int32_t ncuts);
+
+/* Checks the host tables (every track inside the source buffer and linked to its cut, row counts, flags, law and mode codes,
+ * mix_rows the end of the cut's mixed tracks, at most 65535 cuts), copies them to `work_dev` and launches the energy, gain
+ * and output kernels, asynchronously on `stream`: three launches whatever the batch.  Every element of the
+ * (ncuts, T_max, F) output `out_dev` is written.  Results are identical from run to run.  Errors are reported through `h`
+ * (b200feat_last_error) when it is not NULL, and through b200feat_global_error. */
+int b200feat_feature_mix(b200feat_handle *h, const float *src_dev, int64_t src_elems, const b200feat_featmix_track *tracks,
+                         int32_t ntracks, const b200feat_featmix_cut *cuts, int32_t ncuts, int32_t F, float *out_dev,
+                         int32_t T_max, float pad_value, void *work_dev, int64_t work_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -31,6 +31,7 @@
 #include "reverb.cuh"
 #include "specaug.cuh"
 #include "rirgen.cuh"
+#include "featmix.cuh"
 
 #include <cub/device/device_segmented_radix_sort.cuh>
 
@@ -1376,6 +1377,99 @@ int b200feat_specaug(b200feat_handle *h, const float *in_dev, float *out_dev, in
   CU_TRY(h, cudaGetLastError());
   const int64_t gy = std::min<int64_t>(std::max<int64_t>((largest + 8 * SA_FILL_THREADS - 1) / (8 * SA_FILL_THREADS), 1), 64);
   specaug_fill_kernel<<<dim3((unsigned)nmasks, (unsigned)gy), SA_FILL_THREADS, 0, st>>>(out_dev, T, F, (const SaMask *)(w + l.masks), d_mean);
+  CU_TRY(h, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+int64_t b200feat_feature_mix_work_bytes(int32_t ntracks, int32_t ncuts) {
+  if (ntracks < 0 || ncuts < 0) return 0;
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  return up((int64_t)ntracks * (int64_t)sizeof(b200feat_featmix_track)) + up((int64_t)ncuts * (int64_t)sizeof(b200feat_featmix_cut)) +
+         up((int64_t)ntracks * FM_PARTS * 8) + up((int64_t)ntracks * 8);
+}
+
+int b200feat_feature_mix(b200feat_handle *h, const float *src_dev, int64_t src_elems, const b200feat_featmix_track *tracks,
+                         int32_t ntracks, const b200feat_featmix_cut *cuts, int32_t ncuts, int32_t F, float *out_dev,
+                         int32_t T_max, float pad_value, void *work_dev, int64_t work_bytes, void *stream) {
+  if (ntracks < 0 || ncuts < 0 || F < 1 || T_max < 0 || src_elems < 0 || (ncuts > 0 && (!cuts || !out_dev || !work_dev)) ||
+      (ntracks > 0 && !tracks))
+    return fail(h, B200FEAT_EINVAL, "feature_mix: bad arguments");
+  if (ncuts == 0 || T_max == 0) return B200FEAT_OK;
+  if (ncuts > 65535) return fail(h, B200FEAT_EINVAL, "feature_mix: more than 65535 cuts in one call");
+  if ((int64_t)ntracks * FM_PARTS > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "feature_mix: too many tracks in one call");
+  const int64_t tiles = ((int64_t)T_max * F + FM_TILE - 1) / FM_TILE;
+  if (tiles > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "feature_mix: T_max * F too large");
+  if (work_bytes < b200feat_feature_mix_work_bytes(ntracks, ncuts)) return fail(h, B200FEAT_EINVAL, "feature_mix: work buffer too small");
+  auto where = [](const char *what, int64_t i) { return std::string("feature_mix: ") + what + " " + std::to_string(i) + ": "; };
+  for (int32_t t = 0; t < ntracks; ++t) {
+    const b200feat_featmix_track &tr = tracks[t];
+    if (tr.struct_size != (int32_t)sizeof(b200feat_featmix_track))
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "b200feat_featmix_track size mismatch (ABI)");
+    if (tr.cut < 0 || tr.cut >= ncuts) return fail(h, B200FEAT_EINVAL, where("track", t) + "cut index out of range");
+    if (tr.flags & ~(B200FEAT_FEATMIX_MIXED | B200FEAT_FEATMIX_ENERGY)) return fail(h, B200FEAT_EINVAL, where("track", t) + "bad flags");
+    if (tr.num_rows < 0 || tr.offset < 0 || tr.stored_rows < 0 ||
+        (tr.stored_rows > 0 && tr.stored_rows != tr.num_rows && tr.stored_rows != tr.num_rows - 1))
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "bad row counts or offset (stored_rows is num_rows or num_rows - 1)");
+    if (tr.stored_rows > 0 && (!src_dev || tr.src_elem < 0 || tr.src_elem > src_elems - (int64_t)tr.stored_rows * F))
+      return fail(h, B200FEAT_EINVAL, where("track", t) + "rows outside the source buffer");
+  }
+  for (int32_t c = 0; c < ncuts; ++c) {
+    const b200feat_featmix_cut &cu = cuts[c];
+    if (cu.struct_size != (int32_t)sizeof(b200feat_featmix_cut))
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "b200feat_featmix_cut size mismatch (ABI)");
+    if (cu.mode != B200FEAT_FEATMIX_COPY && cu.mode != B200FEAT_FEATMIX_MIX) return fail(h, B200FEAT_EINVAL, where("cut", c) + "bad mode");
+    if (cu.num_tracks < 1 || cu.first_track < 0 || (int64_t)cu.first_track + cu.num_tracks > ntracks)
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "tracks outside the track table");
+    if (cu.num_rows < 0 || cu.num_rows > T_max) return fail(h, B200FEAT_EINVAL, where("cut", c) + "num_rows outside [0, T_max]");
+    for (int32_t k = 0; k < cu.num_tracks; ++k)
+      if (tracks[cu.first_track + k].cut != c) return fail(h, B200FEAT_EINVAL, where("cut", c) + "a track of another cut inside its range");
+    const b200feat_featmix_track &b = tracks[cu.first_track];
+    if (!(b.flags & B200FEAT_FEATMIX_MIXED) || b.offset != 0)
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "the first track must be mixed, at offset 0");
+    if (cu.mode == B200FEAT_FEATMIX_COPY) {
+      if (cu.num_tracks != 1 || b.num_rows > cu.num_rows) return fail(h, B200FEAT_EINVAL, where("cut", c) + "a copy is one track of at most num_rows rows");
+      continue;
+    }
+    if (cu.law != B200FEAT_FEATMIX_LOG && cu.law != B200FEAT_FEATMIX_LINEAR) return fail(h, B200FEAT_EINVAL, where("cut", c) + "bad law");
+    if (cu.ref_track < 0 || cu.ref_track >= cu.num_tracks) return fail(h, B200FEAT_EINVAL, where("cut", c) + "reference index outside the cut's tracks");
+    if (!(tracks[cu.first_track + cu.ref_track].flags & B200FEAT_FEATMIX_ENERGY))
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "the reference track needs the energy flag");
+    int64_t rows = b.num_rows;
+    for (int32_t k = 0; k < cu.num_tracks; ++k) {
+      const b200feat_featmix_track &tr = tracks[cu.first_track + k];
+      if (!(tr.flags & B200FEAT_FEATMIX_MIXED)) continue;
+      if (tr.snr_factor == tr.snr_factor && (k > 0 || cu.ref_track != 0) && !(tr.flags & B200FEAT_FEATMIX_ENERGY))
+        return fail(h, B200FEAT_EINVAL, where("cut", c) + "a mixed track with an SNR needs the energy flag");
+      if (k == 0) continue;
+      if (tr.num_rows < 1) return fail(h, B200FEAT_EINVAL, where("cut", c) + "a further mixed track without rows (the mixer skips those)");
+      rows = std::max(rows, (int64_t)tr.offset + tr.num_rows);
+    }
+    if (rows != cu.mix_rows) return fail(h, B200FEAT_EINVAL, where("cut", c) + "mix_rows is not the end of its mixed tracks");
+    if (cu.num_rows > 0 && (cu.mix_rows < 1 || cu.mix_rows < (int64_t)cu.num_rows - 1 || cu.mix_rows > (int64_t)cu.num_rows + 1))
+      return fail(h, B200FEAT_EINVAL, where("cut", c) + "mix_rows more than one row away from num_rows");
+  }
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  char *w = (char *)work_dev;
+  b200feat_featmix_track *d_tracks = (b200feat_featmix_track *)w;
+  w += up((int64_t)ntracks * (int64_t)sizeof(b200feat_featmix_track));
+  b200feat_featmix_cut *d_cuts = (b200feat_featmix_cut *)w;
+  w += up((int64_t)ncuts * (int64_t)sizeof(b200feat_featmix_cut));
+  double *partial = (double *)w;
+  w += up((int64_t)ntracks * FM_PARTS * 8);
+  double *gain = (double *)w;
+  const cudaStream_t st = (cudaStream_t)stream;
+  // pageable copies: each returns once its table has been staged, so the tables may go when this function returns
+  CU_TRY(h, cudaMemcpyAsync(d_tracks, tracks, (size_t)ntracks * sizeof(b200feat_featmix_track), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_cuts, cuts, (size_t)ncuts * sizeof(b200feat_featmix_cut), cudaMemcpyHostToDevice, st));
+  if (ntracks) {
+    featmix_energy_kernel<<<(unsigned)(ntracks * FM_PARTS), FM_THREADS, 0, st>>>(src_dev, d_tracks, d_cuts, F, partial);
+    CU_TRY(h, cudaGetLastError());
+  }
+  featmix_gain_kernel<<<(unsigned)((ncuts + FM_GAIN_THREADS - 1) / FM_GAIN_THREADS), FM_GAIN_THREADS, 0, st>>>(d_tracks, d_cuts, ncuts,
+                                                                                                               partial, gain);
+  CU_TRY(h, cudaGetLastError());
+  featmix_out_kernel<<<dim3((unsigned)tiles, (unsigned)ncuts), FM_THREADS, 0, st>>>(src_dev, d_tracks, d_cuts, gain, F, T_max, pad_value,
+                                                                                      out_dev);
   CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }
