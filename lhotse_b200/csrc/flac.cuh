@@ -1,8 +1,8 @@
 // FLAC (RFC 9639) decode of 16-bit streams: the host frame index and the per-frame decoder, one thread per frame.
 //
-// The per-frame decoder is __host__ __device__ code with no CUDA intrinsics outside FLAC_CLZ64, so that
-// scripts/micro/flac_host_check.cu runs exactly this code on the CPU (also under AddressSanitizer) against the oracle and on
-// truncated / bit-flipped frames.  The kernel at the end is the only device-only part.
+// The per-frame decoder and the per-job checks are __host__ __device__ code with no CUDA intrinsics outside FLAC_CLZ64, so that
+// scripts/micro/flac_host_check.cu runs exactly this code on the CPU (also under AddressSanitizer) against the oracle, on
+// truncated / bit-flipped frames and on job tables.  The kernel at the end is the only device-only part.
 //
 //   bit reader   a 64-bit MSB-first window refilled byte by byte; bytes at or past the frame's byte_length read as zero, and
 //                every loop that could spin on those zeros (unary codes) stops once the reader has passed the end.  The
@@ -342,6 +342,17 @@ FLAC_HD int flac_decode_frame(const uint8_t *p, const b200feat_flac_job &job, in
   return st;
 }
 
+// One job of a launch: the job's offsets checked against the launch's buffers (`out_elems` int16 of output, `scratch_elems`
+// int32 of scratch; a job whose scratch range does not fit gets none), then the frame.  The kernel and the host check both
+// run this, so they apply the same checks.
+FLAC_HD int flac_decode_job(const uint8_t *bytes, const b200feat_flac_job &job, int16_t *out, int64_t out_elems, int32_t *scratch,
+                            int64_t scratch_elems, int32_t *hist, int32_t *coef, int stride, const uint16_t *crc_tab) {
+  if (job.src_byte < 0 || job.dst_elem < 0 || job.count < 0 || job.dst_elem + job.count > out_elems) return B200FEAT_FLAC_EJOB;
+  int32_t *scr = nullptr;
+  if (job.scratch_elem >= 0 && job.scratch_elem + job.count <= scratch_elems) scr = scratch + job.scratch_elem;
+  return flac_decode_frame(bytes + job.src_byte, job, out + job.dst_elem, scr, hist, coef, stride, crc_tab, true);
+}
+
 // Host frame index (b200feat_flac_index).
 inline int64_t flac_index(const uint8_t *f, int64_t nbytes, b200feat_flac_stream *info, b200feat_flac_frame *frames,
                           int64_t capacity) {
@@ -429,17 +440,7 @@ __global__ void __launch_bounds__(FLAC_THREADS) flac_decode_kernel(const uint8_t
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= njobs) return;
   const b200feat_flac_job job = jobs[j];
-  int st;
-  if (job.src_byte < 0 || job.dst_elem < 0 || job.count < 0 || job.dst_elem + job.count > out_elems) {
-    st = B200FEAT_FLAC_EJOB;
-  } else {
-    int32_t *scr = nullptr;
-    if (job.scratch_elem >= 0) {
-      if (job.scratch_elem + job.count <= scratch_elems) scr = scratch + job.scratch_elem;
-    }
-    st = flac_decode_frame(bytes + job.src_byte, job, out + job.dst_elem, scr, hist + threadIdx.x, coef + threadIdx.x,
-                           FLAC_THREADS, tab, true);
-  }
-  status[j] = st;
+  status[j] = flac_decode_job(bytes, job, out, out_elems, scratch, scratch_elems, hist + threadIdx.x, coef + threadIdx.x,
+                              FLAC_THREADS, tab);
 }
 #endif

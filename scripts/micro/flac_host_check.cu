@@ -7,6 +7,12 @@
 //   ./flac_host_check in.flac - corrupt N    N rounds over every frame: truncated byte ranges and single bit flips must come
 //                                            back as a status (with the CRC-16 check), and the parser alone (check off) must
 //                                            stay inside the buffers whatever the bits say
+//   ./flac_host_check jobs data.bin jobs.bin OUT_ELEMS SCRATCH_ELEMS OUT_FILL SCRATCH_FILL out.bin scratch.bin
+//                                            one launch of a b200feat_flac_job table over the bytes of data.bin, as the kernel
+//                                            runs it (flac_decode_job): an int16 output of OUT_ELEMS and an int32 scratch of
+//                                            SCRATCH_ELEMS, filled with OUT_FILL / SCRATCH_FILL, each exactly sized; each job
+//                                            reads an exactly sized copy of its byte range.  Prints one status per job and
+//                                            writes both buffers.  A job whose byte range leaves data.bin refuses the table.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -35,7 +41,64 @@ static int run(const uint8_t *src, int nbytes, b200feat_flac_job job, std::vecto
   return st;
 }
 
+static bool read_file(const char *path, std::vector<uint8_t> &out) {
+  FILE *f = fopen(path, "rb");
+  if (!f) return false;
+  uint8_t buf[65536];
+  size_t k;
+  while ((k = fread(buf, 1, sizeof buf, f)) > 0) out.insert(out.end(), buf, buf + k);
+  fclose(f);
+  return true;
+}
+
+static int jobs_main(int argc, char **argv) {
+  if (argc != 10) {
+    fprintf(stderr, "usage: %s jobs data.bin jobs.bin OUT_ELEMS SCRATCH_ELEMS OUT_FILL SCRATCH_FILL out.bin scratch.bin\n", argv[0]);
+    return 2;
+  }
+  std::vector<uint8_t> data, table;
+  if (!read_file(argv[2], data) || !read_file(argv[3], table) || table.size() % sizeof(b200feat_flac_job)) return 2;
+  const int64_t out_elems = atoll(argv[4]), scratch_elems = atoll(argv[5]);
+  const int16_t out_fill = (int16_t)atoi(argv[6]);
+  const int32_t scratch_fill = (int32_t)strtol(argv[7], nullptr, 0);
+  const size_t njobs = table.size() / sizeof(b200feat_flac_job);
+  std::vector<b200feat_flac_job> jobs(njobs);
+  memcpy(jobs.data(), table.data(), table.size());
+  int16_t *out = (int16_t *)malloc(sizeof(int16_t) * (out_elems > 0 ? out_elems : 1));
+  int32_t *scratch = scratch_elems > 0 ? (int32_t *)malloc(sizeof(int32_t) * scratch_elems) : nullptr;
+  for (int64_t i = 0; i < out_elems; ++i) out[i] = out_fill;
+  for (int64_t i = 0; i < scratch_elems; ++i) scratch[i] = scratch_fill;
+  int32_t *hist = (int32_t *)malloc(sizeof(int32_t) * FLAC_MAX_ORDER), *coef = (int32_t *)malloc(sizeof(int32_t) * FLAC_MAX_ORDER);
+  printf("statuses");
+  for (size_t j = 0; j < njobs; ++j) {
+    b200feat_flac_job job = jobs[j];
+    const int64_t len = job.byte_length > 0 ? job.byte_length : 0;
+    if (job.src_byte >= 0 && job.src_byte + len > (int64_t)data.size()) {
+      fprintf(stderr, "job %zu: bytes [%lld, +%lld) outside the %zu bytes of data\n", j, (long long)job.src_byte,
+              (long long)len, data.size());
+      return 2;
+    }
+    uint8_t *bytes = (uint8_t *)malloc(len > 0 ? len : 1);
+    if (job.src_byte >= 0) {
+      memcpy(bytes, data.data() + job.src_byte, len);
+      job.src_byte = 0;
+    }
+    printf(" %d", flac_decode_job(bytes, job, out, out_elems, scratch, scratch_elems, hist, coef, 1, nullptr));
+    free(bytes);
+  }
+  printf("\n");
+  FILE *o = fopen(argv[8], "wb"), *s = fopen(argv[9], "wb");
+  if (!o || !s) return 2;
+  fwrite(out, sizeof(int16_t), out_elems, o);
+  if (scratch_elems > 0) fwrite(scratch, sizeof(int32_t), scratch_elems, s);
+  fclose(o);
+  fclose(s);
+  free(out); free(scratch); free(hist); free(coef);
+  return 0;
+}
+
 int main(int argc, char **argv) {
+  if (argc >= 2 && !strcmp(argv[1], "jobs")) return jobs_main(argc, argv);
   if (argc < 3) {
     fprintf(stderr, "usage: %s in.flac out.raw|- [corrupt N]\n", argv[0]);
     return 2;

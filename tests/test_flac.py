@@ -4,12 +4,12 @@ test writer; the library's host frame index (`b200feat_flac_index`) against the 
 exact per-frame decoder of csrc/flac.cuh run on the host (scripts/micro/flac_host_check.cu), under AddressSanitizer
 where the toolchain has it, on whole streams and on truncated and bit-flipped frames."""
 import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
+import flac_cases as C
 import flac_oracle as F
 import flac_writer as W
 import refshim
@@ -115,25 +115,8 @@ def test_ring_job_table_decodes_to_the_requested_samples(streams, stream_dir):
         assert np.array_equal(out[o:o + n], w)
 
 
-def _host_check_binary(tmp_path):
-    src = os.path.join(ROOT, "scripts", "micro", "flac_host_check.cu")
-    exe = str(tmp_path / "flac_host_check")
-    gxx = shutil.which("g++")
-    if gxx:
-        for flags in (["-fsanitize=address", "-fno-omit-frame-pointer"], []):
-            res = subprocess.run([gxx, "-x", "c++", "-std=c++17", "-O1", "-g", *flags, "-o", exe, src], capture_output=True, text=True)
-            if res.returncode == 0:
-                return exe, bool(flags)
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("no host compiler")
-    res = subprocess.run([nvcc, "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe, src], capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-2000:]
-    return exe, False
-
-
 def test_kernel_frame_decoder_on_the_host(stream_dir, tmp_path):
-    exe, asan = _host_check_binary(tmp_path)
+    exe, asan = C.host_check_binary(tmp_path)
     env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:abort_on_error=0")
     files = sorted(str(p) for p in stream_dir.glob("*.flac")) + GOLDEN
     for path in files:
