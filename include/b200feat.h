@@ -581,6 +581,26 @@ int b200feat_feature_mix(b200feat_handle *h, const float *src_dev, int64_t src_e
                          int32_t ntracks, const b200feat_featmix_cut *cuts, int32_t ncuts, int32_t F, float *out_dev,
                          int32_t T_max, float pad_value, void *work_dev, int64_t work_bytes, void *stream);
 
+/*
+ * Backward of the Kaldi-family kinds (B200FEAT_FBANK, _MFCC, _SPECTROGRAM, _LOG_SPECTROGRAM, Kaldi framing): the gradient of
+ * a scalar loss with respect to the float32 samples, given its gradient with respect to the packed (sum T_i, F) rows that
+ * b200feat_extract produced from the same samples (DESIGN.md §3.1n).  The frames are recomputed from the samples; nothing
+ * of the forward is kept.
+ */
+/* Device scratch b200feat_backward needs for cuts of `num_samples` (host array of B), or a negative B200FEAT_E* code
+ * (B200FEAT_ESHORT for a cut too short to be framed, B200FEAT_EINVAL for a kind without a backward). */
+int64_t b200feat_backward_work_bytes(b200feat_handle *h, const int64_t *num_samples, int32_t B);
+
+/* `samples_dev` (B200FEAT_F32 only) holds cut i at element offsets[i] with num_samples[i] samples (host arrays); `grad_out_dev`
+ * the (row_off[B], F) gradient of the features, cut i's rows at [row_off[i], row_off[i + 1]) (host array of B + 1 with
+ * row_off[0] = 0 and each cut's frame count).  Writes the gradient of every sample [offsets[i], offsets[i] + num_samples[i])
+ * of `grad_in_dev` (same layout as the samples; elements outside the cuts are not touched), asynchronously on `stream`: two
+ * launches.  No atomics: results are identical from run to run, and a cut's gradient does not depend on the other cuts of the
+ * call.  Errors are reported through `h` (b200feat_last_error). */
+int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples, const int64_t *offsets,
+                      int32_t B, const float *grad_out_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
+                      int64_t work_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

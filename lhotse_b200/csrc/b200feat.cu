@@ -32,6 +32,7 @@
 #include "specaug.cuh"
 #include "rirgen.cuh"
 #include "featmix.cuh"
+#include "backward.cuh"
 
 #include <cub/device/device_segmented_radix_sort.cuh>
 
@@ -1618,6 +1619,117 @@ int b200feat_rir_generate(b200feat_handle *h, const double *draws_dev, int64_t d
   }
   rirgen_biquad_kernel<<<(unsigned)((nrirs + 31) / 32), 32, 0, st>>>(d_rirs, nrirs);
   CU_TRY(h, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The backward's view of the handle's plan; false for a plan without a backward (whisper / log10 kinds, centre padding).
+bool bwd_plan(const b200feat_handle *h, BwdPlan *out) {
+  const DevPlan &p = h->plan;
+  const int f = p.feature;
+  if ((f != B200FEAT_FBANK && f != B200FEAT_MFCC && f != B200FEAT_SPECTROGRAM && f != B200FEAT_LOG_SPECTROGRAM) || p.whisper ||
+      p.log10_mel || p.pad_mode != B200FEAT_PAD_KALDI)
+    return false;
+  BwdPlan b;
+  memset(&b, 0, sizeof(b));
+  b.feature = f; b.L = p.L; b.S = p.S; b.N = p.N; b.K = p.K; b.M = p.M; b.C = p.C; b.F = p.F; b.Nc = p.Nc; b.packed = p.packed;
+  b.pad = p.pad_left; b.snip_edges = p.snip_edges; b.remove_dc = p.remove_dc; b.use_energy = p.use_energy;
+  b.raw_energy = p.raw_energy; b.use_mag = p.use_mag; b.energy_style = p.energy_style; b.use_lifter = p.use_lifter;
+  b.ecol = p.energy_last ? p.F - 1 : 0;
+  b.shift = (f == B200FEAT_FBANK && p.use_energy && !p.energy_last) ? 1 : 0;
+  b.preemph = p.preemph; b.energy_floor_log = p.energy_floor_log; b.has_energy_floor = p.has_energy_floor;
+  b.mel_floor = p.mel_floor; b.log_spec_eps = p.log_spec_eps; b.log_spec_floor = p.log_spec_floor;
+  b.window = p.window; b.tws = reinterpret_cast<const BwdC *>(p.tws);
+  b.mel_start = p.mel_start; b.mel_len = p.mel_len; b.mel_woff = p.mel_woff; b.mel_w = p.mel_w;
+  b.dct = p.dct; b.lifter = p.lifter; b.post_scale = p.post_scale;
+  *out = b;
+  return true;
+}
+
+// Tiles of every cut (tile_off, B + 1 entries) and the work buffer size; a negative code for a cut too short to be framed
+int64_t bwd_layout(b200feat_handle *h, const BwdPlan &p, int ft, const int64_t *num_samples, int32_t B,
+                   std::vector<int64_t> *tile_off) {
+  int64_t tiles = 0;
+  if (tile_off) tile_off->assign((size_t)B + 1, 0);
+  for (int i = 0; i < B; ++i) {
+    const int64_t T = cut_frames(h, i, num_samples[i]);
+    if (T < 0) return T;
+    tiles += (T + ft - 1) / ft;
+    if (tile_off) (*tile_off)[i + 1] = tiles;
+  }
+  return bwd_meta_bytes(B) + tiles * bwd_span(p, ft) * (int64_t)sizeof(float);
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t b200feat_backward_work_bytes(b200feat_handle *h, const int64_t *num_samples, int32_t B) {
+  if (!h || !num_samples || B <= 0) return fail(h, B200FEAT_EINVAL, "backward_work_bytes: bad arguments");
+  BwdPlan p;
+  if (!bwd_plan(h, &p)) return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram and log-spectrogram kinds have one");
+  int warps, ft;
+  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, "backward: frame too long for shared memory");
+  return bwd_layout(h, p, ft, num_samples, B, nullptr);
+}
+
+int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples, const int64_t *offsets,
+                      int32_t B, const float *grad_out_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
+                      int64_t work_bytes, void *stream) {
+  if (!h) return fail(nullptr, B200FEAT_EINVAL, "backward: null handle");
+  if (!samples_dev || !num_samples || !offsets || B <= 0 || !grad_out_dev || !row_off || !grad_in_dev || !work_dev)
+    return fail(h, B200FEAT_EINVAL, "backward: bad arguments");
+  if (dt != B200FEAT_F32) return fail(h, B200FEAT_EINVAL, "backward: float32 samples only");
+  BwdPlan p;
+  if (!bwd_plan(h, &p)) return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram and log-spectrogram kinds have one");
+  int warps, ft;
+  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, "backward: frame too long for shared memory");
+  std::vector<int64_t> tile_off;
+  const int64_t need = bwd_layout(h, p, ft, num_samples, B, &tile_off);
+  if (need < 0) return (int)need;
+  if (work_bytes < need) return fail(h, B200FEAT_EINVAL, "backward: work buffer too small");
+  if (row_off[0] != 0) return fail(h, B200FEAT_EINVAL, "backward: row_off[0] must be 0");
+  for (int i = 0; i < B; ++i) {
+    if (offsets[i] < 0 || num_samples[i] < 0) return fail(h, B200FEAT_EINVAL, "backward: negative offset or length");
+    if (row_off[i + 1] - row_off[i] != frames_for(h->desc, num_samples[i]))
+      return fail(h, B200FEAT_EINVAL, "backward: row_off does not match cut " + std::to_string(i) + "'s frame count");
+  }
+  // the int64 tables in one host block: samp_off, nsamp, row_off, tile_off
+  std::vector<int64_t> meta(4 * (size_t)B + 2);
+  std::copy(offsets, offsets + B, meta.begin());
+  std::copy(num_samples, num_samples + B, meta.begin() + B);
+  std::copy(row_off, row_off + B + 1, meta.begin() + 2 * (size_t)B);
+  std::copy(tile_off.begin(), tile_off.end(), meta.begin() + 3 * (size_t)B + 1);
+  DeviceGuard on(h->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  unsigned char *w = (unsigned char *)work_dev;
+  // a pageable copy: the call returns once the block has been staged, so the vector may go when this function returns
+  CU_TRY(h, cudaMemcpyAsync(w, meta.data(), meta.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  const int64_t *dm = (const int64_t *)w;
+  BwdBatch bb;
+  bb.samples = samples_dev; bb.grad_out = grad_out_dev; bb.grad_in = grad_in_dev;
+  bb.samp_off = dm; bb.nsamp = dm + B; bb.row_off = dm + 2 * (int64_t)B; bb.tile_off = dm + 3 * (int64_t)B + 1;
+  bb.spans = (float *)(w + bwd_meta_bytes(B));
+  bb.B = B; bb.ft = ft;
+  const int64_t ntiles = tile_off[B];
+  if (ntiles > 0) {
+    const size_t smem = bwd_smem(p, warps, ft);
+    CU_TRY(h, cudaFuncSetAttribute(b200feat_backward_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const unsigned grid = (unsigned)std::min<int64_t>(ntiles, (int64_t)h->sm_count * 64);
+    b200feat_backward_frames_kernel<<<grid, warps * 32, smem, st>>>(p, h->plan, bb, ntiles);
+    CU_TRY(h, cudaGetLastError());
+  }
+  int64_t nmax = 0;
+  for (int i = 0; i < B; ++i) nmax = std::max(nmax, num_samples[i]);
+  if (nmax > 0) {
+    const int64_t gx = std::min<int64_t>((nmax + BWD_COMBINE_THREADS - 1) / BWD_COMBINE_THREADS, 4096);
+    const dim3 grid((unsigned)gx, (unsigned)std::min<int32_t>(B, 65535));
+    b200feat_backward_combine_kernel<<<grid, BWD_COMBINE_THREADS, 0, st>>>(p, bb);
+    CU_TRY(h, cudaGetLastError());
+  }
   return B200FEAT_OK;
 }
 

@@ -130,7 +130,7 @@ EXPORTS = [
     "b200feat_resample_table", "b200feat_resample_work_bytes", "b200feat_resample", "b200feat_mix_ex",
     "b200feat_reverb_work_bytes", "b200feat_reverb", "b200feat_specaug_work_bytes", "b200feat_specaug",
     "b200feat_reverb_ex", "b200feat_rir_generate_work_bytes", "b200feat_rir_generate",
-    "b200feat_feature_mix_work_bytes", "b200feat_feature_mix",
+    "b200feat_feature_mix_work_bytes", "b200feat_feature_mix", "b200feat_backward_work_bytes", "b200feat_backward",
 ]
 
 
@@ -224,6 +224,10 @@ def load_library():
         lib.b200feat_feature_mix_work_bytes.argtypes = [i32, i32]
         lib.b200feat_feature_mix.restype = C.c_int
         lib.b200feat_feature_mix.argtypes = [vp, vp, i64, vp, i32, vp, i32, i32, vp, i32, C.c_float, vp, i64, vp]
+        lib.b200feat_backward_work_bytes.restype = i64
+        lib.b200feat_backward_work_bytes.argtypes = [vp, vp, i32]
+        lib.b200feat_backward.restype = C.c_int
+        lib.b200feat_backward.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -550,6 +554,28 @@ class Engine:
         if out is None:
             out = flat[: shape[0] * shape[1] * (shape[2] if len(shape) == 3 else 1)].view(shape)
         return out, row_prefix
+
+    def backward_device(self, samples: torch.Tensor, num_samples: Sequence[int], offsets: Sequence[int],
+                        grad_out: torch.Tensor, row_prefix: Sequence[int]) -> torch.Tensor:
+        """Gradient with respect to `samples` (1-D float32 CUDA tensor, cut i at offsets[i] with num_samples[i] samples) of a
+        loss whose gradient with respect to the packed (sum T_i, F) features `extract_device` gave for them is `grad_out`
+        (`row_prefix`: that call's row prefix).  Returns a float32 tensor shaped like `samples`: zero outside the cuts."""
+        assert samples.is_cuda and samples.dim() == 1 and samples.is_contiguous() and samples.dtype == torch.float32
+        B = len(num_samples)
+        ns = np.ascontiguousarray(num_samples, dtype=np.int64)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        rows = np.ascontiguousarray(row_prefix, dtype=np.int64)
+        g = grad_out.to(device=samples.device, dtype=torch.float32).contiguous()
+        assert g.shape == (int(rows[-1]), self.feature_dim), (tuple(g.shape), int(rows[-1]), self.feature_dim)
+        nbytes = int(self.lib.b200feat_backward_work_bytes(self._h, _ptr(ns), B))
+        if nbytes < 0:
+            self._check_cuts(nbytes)
+        work = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=samples.device)
+        grad_in = torch.zeros_like(samples)
+        stream = torch.cuda.current_stream(samples.device).cuda_stream
+        self._check_cuts(self.lib.b200feat_backward(self._h, samples.data_ptr(), DT_F32, _ptr(ns), _ptr(off), B, g.data_ptr(),
+                                                    _ptr(rows), grad_in.data_ptr(), work.data_ptr(), work.numel(), stream))
+        return grad_in
 
     # ------------------------------------------------------------------ host-to-host path
     def extract_host(self, samples: Union[np.ndarray, torch.Tensor], num_samples: Sequence[int],

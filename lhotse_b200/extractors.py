@@ -21,6 +21,9 @@ Deliberate differences, all documented in DESIGN.md:
     framing, drawn from torch's global generator — here the CUDA generator of the extractor's device, so the noise
     values differ from a CPU run (they also differ between any two reference runs that do not share a seed).
   * ``device`` must be a CUDA device; there is no CPU fallback.
+  * A float tensor input that requires grad (with grad mode on) gives features with a graph back to it, as the reference's
+    ``nn.Module`` chain does, for the Fbank / Mfcc / Spectrogram / LogSpectrogram classes through ``extract`` and
+    ``extract_batch``: the gradient is the sm_90a backward kernel's (csrc/backward.cuh, DESIGN.md §3.1n).
 """
 from __future__ import annotations
 
@@ -184,9 +187,49 @@ def _to_float32(x: ArrayLike) -> ArrayLike:
     return x.astype(np.float32) * np.float32(1.0 / 32768.0) if x.dtype == np.int16 else x.astype(np.float32, copy=False)
 
 
+_GRAD_KINDS = ("fbank", "mfcc", "spectrogram", "log-spectrogram")
+
+
+class _KaldiFeatures(torch.autograd.Function):
+    """Features of flat float32 waveforms with the backward kernel as their gradient.  `items` are the cuts' tensors (on
+    the host or a device); one item may hold several cuts at `offs` (the rows of a (B, n) batch), several items are one cut
+    each and are packed here.  The (dithered) packed device buffer is saved; the backward recomputes everything else."""
+
+    @staticmethod
+    def forward(ctx, ext, eng, lens, offs, info, *items):
+        if len(items) == 1:
+            buf = items[0].detach().reshape(-1).to(eng.device, non_blocking=True)
+        else:
+            buf, lens, offs = pack_device([x.detach().reshape(-1) for x in items], eng.device)
+        buf = ext._dithered(buf).contiguous()
+        if buf.data_ptr() % 16:
+            buf = buf.clone()  # extract_device would copy an unaligned view; the backward must read the same buffer
+        out, prefix = eng.extract_device(buf, list(lens), offsets=list(offs))
+        info["prefix"] = prefix
+        ctx.eng, ctx.lens, ctx.offs, ctx.prefix = eng, list(lens), list(offs), prefix
+        ctx.items = [(x.shape, x.device, x.numel()) for x in items]
+        ctx.save_for_backward(buf)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        if torch.is_grad_enabled():
+            raise RuntimeError("the b200 extractors' backward is not differentiable: double backward (create_graph=True) is "
+                               "not supported")
+        (buf,) = ctx.saved_tensors
+        g = ctx.eng.backward_device(buf, ctx.lens, ctx.offs, grad_out, ctx.prefix)
+        if len(ctx.items) == 1:
+            shape, dev, numel = ctx.items[0]
+            grads = [g[:numel].view(shape).to(dev)]
+        else:
+            grads = [g[o:o + numel].view(shape).to(dev) for o, (shape, dev, numel) in zip(ctx.offs, ctx.items)]
+        return (None, None, None, None, None, *grads)
+
+
 class _B200Extractor(FeatureExtractor):
     feature_kind: str = None
     _returns_cpu_tensor = False  # Spectrogram/LogSpectrogram `.cpu()` their tensor outputs (:343, :453)
+    _grad = True  # the families' inner extractors keep detached outputs
 
     def __init__(self, config: Optional[Any] = None):
         super().__init__(config=config)
@@ -258,10 +301,24 @@ class _B200Extractor(FeatureExtractor):
         x = buf.to(torch.float32) * (1.0 / 32768.0) if buf.dtype == torch.int16 else buf
         return x + d * torch.randn(x.shape, device=x.device, dtype=torch.float32)
 
+    def _wants_grad(self, items: Sequence[ArrayLike]) -> bool:
+        """True when the features must carry a graph back to the float tensors `items` (the backward kernel's path)."""
+        return (self._grad and self.feature_kind in _GRAD_KINDS and torch.is_grad_enabled()
+                and any(isinstance(x, torch.Tensor) and x.requires_grad for x in items))
+
+    def _extract_grad(self, items: Sequence[torch.Tensor], lens: Sequence[int], offsets: Sequence[int]):
+        """`_extract_on_device` / `_extract_list_on_device` with a graph: (features, row prefix)."""
+        info = {}
+        out = _KaldiFeatures.apply(self, self.engine, list(lens), list(offsets), info, *items)
+        return out, info["prefix"]
+
     def extract(self, samples: ArrayLike, sampling_rate: int) -> ArrayLike:
         self._check_sr(sampling_rate)
         (x,), _ = _kernel_input([_first_channel_1d(samples)])
         if isinstance(x, torch.Tensor):
+            if self._wants_grad([x]):
+                feats, _ = self._extract_grad([x], [x.numel()], [0])
+                return feats.cpu() if self._returns_cpu_tensor else feats
             feats, _ = self._extract_on_device(x.contiguous(), [x.numel()], [0])
             return feats.cpu() if self._returns_cpu_tensor else feats
         if self.config.dither != 0.0:  # noise is generated on the device: take the tensor route
@@ -287,6 +344,9 @@ class _B200Extractor(FeatureExtractor):
         """A list of waveforms (numpy arrays or tensors, on the host or the device), packed into one device buffer."""
         eng = engine or self.engine
         flat, pcm16 = _kernel_input(samples)
+        if engine is None and not kw and not pcm16 and self._wants_grad(flat):
+            items = [torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x for x in flat]
+            return self._extract_grad(items, [int(x.numel()) for x in items], [0] * len(items))
         tensors = [torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x for x in flat]
         buf, lens, offs = pack_device(tensors, eng.device, dtype=torch.int16 if pcm16 else torch.float32)
         return self._extract_on_device(buf, lens, offs, eng, **kw)
@@ -300,7 +360,10 @@ class _B200Extractor(FeatureExtractor):
             lens = [int(l) for l in lengths]
             assert len(lens) == B and max(lens) <= n
         (buf,), _ = _kernel_input([samples])
-        out, prefix = self._extract_on_device(buf, lens, [i * n for i in range(B)])
+        if self._wants_grad([buf]):
+            out, prefix = self._extract_grad([buf], lens, [i * n for i in range(B)])
+        else:
+            out, prefix = self._extract_on_device(buf, lens, [i * n for i in range(B)])
         return out, [out[prefix[i]: prefix[i + 1]] for i in range(B)]
 
     def extract_batch(

@@ -235,6 +235,7 @@ class _FamilyExtractor(FeatureExtractor):
         if inner is None:
             inner = from_reference_config(self.config, device=str(self.config.device), sampling_rate=sr)
             inner.config.kernel = self.config.kernel
+            inner._grad = False  # the torchaudio and kaldifeat families return detached features
             self._inner_by_sr[sr] = inner
         return inner
 
@@ -335,6 +336,7 @@ class B200TorchaudioSpectrogram(_TorchaudioFamily):
                 preemph_coeff=c.preemphasis_coefficient, window_type=c.window_type, dither=c.dither,
                 energy_floor=c.energy_floor, raw_energy=c.raw_energy, use_energy=True,  # kaldi.py: bin 0 <- log-energy, always
                 device=str(c.device), kernel=c.kernel, compat="torchaudio"))
+            inner._grad = False
             self._inner_by_sr[sr] = inner
         return inner
 
