@@ -1663,6 +1663,13 @@ int64_t bwd_layout(b200feat_handle *h, const BwdPlan &p, int ft, const int64_t *
   return bwd_meta_bytes(B) + tiles * bwd_span(p, ft) * (int64_t)sizeof(float);
 }
 
+// The refusal of a frame whose backward does not fit shared memory, with the numbers that decide it
+std::string bwd_too_long(const BwdPlan &p) {
+  return "backward: frame too long for shared memory: L = " + std::to_string(p.L) + ", N = " + std::to_string(p.N) + " needs " +
+         std::to_string(bwd_smem(p, 1, 1)) + " bytes for one warp and one frame, over the backward's limit of " +
+         std::to_string(BWD_SMEM_LIMIT) + " bytes (at 16 kHz, N = 8192 with frames up to about 0.4 s is the largest supported)";
+}
+
 }  // namespace
 
 extern "C" {
@@ -1672,7 +1679,7 @@ int64_t b200feat_backward_work_bytes(b200feat_handle *h, const int64_t *num_samp
   BwdPlan p;
   if (!bwd_plan(h, &p)) return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram and log-spectrogram kinds have one");
   int warps, ft;
-  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, "backward: frame too long for shared memory");
+  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, bwd_too_long(p));
   return bwd_layout(h, p, ft, num_samples, B, nullptr);
 }
 
@@ -1686,7 +1693,7 @@ int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, 
   BwdPlan p;
   if (!bwd_plan(h, &p)) return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram and log-spectrogram kinds have one");
   int warps, ft;
-  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, "backward: frame too long for shared memory");
+  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, bwd_too_long(p));
   std::vector<int64_t> tile_off;
   const int64_t need = bwd_layout(h, p, ft, num_samples, B, &tile_off);
   if (need < 0) return (int)need;

@@ -7,7 +7,8 @@
 // in.bin: int32 header [feature L S N M C F snip_edges remove_dc use_energy raw_energy use_mag energy_style use_lifter
 // ecol shift n T pad 0], float32 [preemph energy_floor_log has_energy_floor mel_floor log_spec_eps log_spec_floor], then
 // float32 window [L], mel bank [K][M] (M > 0), dct [M][C] (C > 0), lifter [C] (use_lifter), samples [n], row gradient [T][F].
-// out.f32: the gradient of the n samples.
+// out.f32: the gradient of the n samples.  Prints the launch shape (frames per tile, warps per CTA); exits with 3, writing
+// nothing, for a frame the backward refuses.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -105,7 +106,12 @@ int main(int argc, char **argv) {
   p.mel_start = mstart.data(); p.mel_len = mlen.data(); p.mel_woff = mwoff.data(); p.mel_w = mw.data();
 
   int warps, ft;
-  if (!bwd_launch_shape(p, &warps, &ft)) { fprintf(stderr, "frame too long\n"); return 2; }
+  if (!bwd_launch_shape(p, &warps, &ft)) {
+    printf("backward: frame too long, %zu bytes of shared memory for one warp and one frame, limit %d\n", bwd_smem(p, 1, 1),
+           BWD_SMEM_LIMIT);
+    free(h); free(sc); free(window); free(bank); free(dct); free(lifter); free(x); free(g); free(tws);
+    return 3;
+  }
   const bool mel = p.feature == B200FEAT_FBANK || p.feature == B200FEAT_MFCC;
   int *flo = (int *)malloc(sizeof(int) * p.K), *fhi = (int *)malloc(sizeof(int) * p.K);
   if (mel)
@@ -168,7 +174,8 @@ int main(int argc, char **argv) {
   FILE *fo = fopen(argv[2], "wb");
   if (!fo || fwrite(gx, sizeof(float), (size_t)n, fo) != (size_t)n) { fprintf(stderr, "cannot write %s\n", argv[2]); return 2; }
   fclose(fo);
-  printf("backward: n %lld, T %lld, %lld tiles of %d frames\n", (long long)n, (long long)T, (long long)ntiles, ft);
+  printf("backward: n %lld, T %lld, %lld tiles of %d frames, %d warps\n", (long long)n, (long long)T, (long long)ntiles, ft,
+         warps);
   free(h); free(sc); free(window); free(bank); free(dct); free(lifter); free(x); free(g); free(tws); free(flo); free(fhi);
   free(spans); free(G); free(raw); free(v); free(gm); free(xs); free(fa); free(fb); free(gx);
   return 0;

@@ -1,7 +1,8 @@
 """Shared pieces of the backward tests (csrc/backward.cuh, DESIGN.md §3.1n): the configs and lengths they sweep, the float64
-autograd twin of the oracle's `extract` (a tensor out instead of a numpy array, so that autograd can run it), a float64
-NumPy restatement of the adjoint chain written the way the kernel computes it, and the host harness
-(scripts/micro/backward_host_check.cu) with its input file."""
+autograd twin of the oracle's `extract` (a tensor out instead of a numpy array, so that autograd can run it), a twin driven
+by a FeaturePlan that also follows the torchaudio and HTK conventions (common.cuh), a float64 NumPy restatement of the
+adjoint chain written the way the kernel computes it, and the host harness (scripts/micro/backward_host_check.cu) with its
+input file."""
 from __future__ import annotations
 
 import dataclasses
@@ -14,6 +15,7 @@ from dataclasses import astuple
 import numpy as np
 import torch
 
+from lhotse_b200.plan import ENERGY_KALDI, FeaturePlan
 from oracle import kaldi_oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -135,54 +137,150 @@ def autograd_grad(x: np.ndarray, cfg, G: np.ndarray, dtype=torch.float64, device
     return xt.grad.double().cpu().numpy()
 
 
+# ----------------------------------------------------------------------------- the plan's conventions (common.cuh)
+def oracle_plan(cfg: O.OracleConfig, dtype=torch.float64) -> FeaturePlan:
+    """The oracle config as a FeaturePlan (lhotse's conventions) holding the oracle's tables in `dtype`, as float64 arrays."""
+    L, S, N = O.layer_sizes(cfg)
+    win, fb, dct, lifter = (None if t is None else t.numpy().astype(np.float64) for t in O._cached_tables(astuple(cfg), dtype))
+    return FeaturePlan(feature=cfg.feature, sampling_rate=cfg.sampling_rate, L=L, S=S, N=N,
+                       num_filters=0 if fb is None else fb.shape[1], num_ceps=0 if dct is None else dct.shape[1],
+                       snip_edges=cfg.snip_edges, remove_dc_offset=cfg.remove_dc_offset, use_energy=cfg.use_energy,
+                       raw_energy=cfg.raw_energy, use_fft_mag=cfg.use_fft_mag, preemph_coeff=cfg.preemph_coeff,
+                       energy_floor=cfg.energy_floor, window=win, mel_bank=fb, dct=dct, lifter=lifter)
+
+
+def energy_floor_binds(plan: FeaturePlan) -> bool:
+    """Whether the log-energy is floored: Kaldi's rule is `energy_floor != 0`, lhotse's `energy_floor > 0` (b200feat.cu)."""
+    return plan.energy_floor != 0.0 if plan.energy_style == ENERGY_KALDI else plan.energy_floor > 0.0
+
+
+def energy_col(plan: FeaturePlan, F: int) -> int:
+    """Column of the log-energy in a row of F features: last under htk_compat, else first."""
+    return F - 1 if plan.energy_last else 0
+
+
+def _log_energy_t(e: torch.Tensor, plan: FeaturePlan) -> torch.Tensor:
+    """common.cuh log_energy_value: Kaldi log(max(e, eps32)) or lhotse log(e + 1e-15), then the floor."""
+    if plan.energy_style == ENERGY_KALDI:
+        le = torch.max(e, torch.tensor(EPS32, dtype=e.dtype, device=e.device)).log()
+    else:
+        le = (e + 1e-15).log()
+    if energy_floor_binds(plan):
+        le = torch.max(le, torch.tensor(math.log(plan.energy_floor), dtype=e.dtype, device=e.device))
+    return le
+
+
+def plan_features_t(x: torch.Tensor, plan: FeaturePlan) -> torch.Tensor:
+    """The forward of `plan` on a tensor (in the dtype of x, on its device), with the plan's own tables and conventions:
+    lhotse's or Kaldi's log-energy, the floor-form log-spectrogram, the energy column first or last, and the permuted HTK
+    DCT and lifter.  autograd runs it."""
+    dt, dev = x.dtype, x.device
+
+    def tab(a):
+        return torch.as_tensor(np.asarray(a, dtype=np.float64)).to(dtype=dt, device=dev)
+
+    f = O._frames_view(x.reshape(-1), plan.L, plan.S, plan.snip_edges)
+    if plan.remove_dc_offset:
+        f = f - torch.mean(f, dim=1, keepdim=True)
+    le = None
+    if plan.use_energy and plan.raw_energy:
+        le = _log_energy_t(f.pow(2).sum(1), plan)
+    if plan.preemph_coeff != 0.0:
+        f = f - plan.preemph_coeff * torch.cat((f[:, :1], f[:, :-1]), dim=1)
+    f = f * tab(plan.window)
+    if plan.use_energy and not plan.raw_energy:
+        le = _log_energy_t(f.pow(2).sum(1), plan)
+    X = torch.fft.rfft(f, n=plan.N, dim=-1)
+    spec = X.abs() if plan.use_fft_mag else X.abs() ** 2
+    if plan.feature == "spectrogram":
+        out = spec
+    elif plan.feature == "log-spectrogram":
+        out = torch.max(spec, tab(-plan.log_spec_eps)).log() if plan.log_spec_eps < 0 else (spec + plan.log_spec_eps).log()
+    else:
+        mel = torch.max(torch.matmul(spec, tab(plan.mel_bank)), tab(plan.mel_floor)).log()
+        if plan.feature == "fbank":
+            if le is None:
+                return mel
+            return torch.cat((mel, le[:, None]), 1) if plan.energy_last else torch.cat((le[:, None], mel), 1)
+        out = torch.matmul(mel, tab(plan.dct))
+        if plan.lifter is not None:
+            out = out * tab(plan.lifter)
+        if le is not None:
+            c = energy_col(plan, out.shape[1])
+            out = torch.cat((out[:, :c], le[:, None], out[:, c + 1:]), 1)
+        return out
+    if le is not None:  # bin 0 <- log-energy
+        out = torch.cat((le[:, None], out[:, 1:]), dim=1)
+    return out
+
+
+def plan_autograd_grad(x: np.ndarray, plan: FeaturePlan, G: np.ndarray, dtype=torch.float64, device="cpu") -> np.ndarray:
+    """d sum(features * G) / dx through `plan_features_t`."""
+    xt = torch.tensor(np.asarray(x, dtype=np.float64), dtype=dtype, device=device, requires_grad=True)
+    out = plan_features_t(xt, plan)
+    (out * torch.as_tensor(G, dtype=dtype, device=device)).sum().backward()
+    return xt.grad.double().cpu().numpy()
+
+
 # ----------------------------------------------------------------------------- float64 restatement of the adjoint chain
 def _dlog_max(v, floor):
     return np.where(v > floor, 1.0 / np.where(v > 0, v, 1.0), np.where(v == floor, 0.5 / floor, 0.0))
 
 
 def restated_grad(x: np.ndarray, cfg, G: np.ndarray) -> np.ndarray:
-    """The kernel's adjoint chain in float64: recompute the frame, then log, mel / DCT, spectrum, frame preprocessing and
-    overlap-add, in that order."""
-    L, S, N = O.layer_sizes(cfg)
+    """The kernel's adjoint chain in float64 for an oracle config, with the oracle's float64 tables."""
+    return restated_grad_plan(x, oracle_plan(cfg), G)
+
+
+def restated_grad_plan(x: np.ndarray, plan: FeaturePlan, G: np.ndarray) -> np.ndarray:
+    """The kernel's adjoint chain in float64 with the plan's tables and conventions: recompute the frame, then log, mel /
+    DCT, spectrum, frame preprocessing and overlap-add, in that order."""
+    L, S, N = plan.L, plan.S, plan.N
     n = x.shape[0]
-    idx = O.frame_index_matrix(n, L, S, cfg.snip_edges)
-    win, fb, dct, lifter = (None if t is None else t.numpy().astype(np.float64) for t in O._cached_tables(astuple(cfg), torch.float64))
+    idx = O.frame_index_matrix(n, L, S, plan.snip_edges)
+    win, fb, dct, lifter = (None if t is None else np.asarray(t, dtype=np.float64)
+                            for t in (plan.window, plan.mel_bank, plan.dct, plan.lifter))
     f = x[idx]
-    mu = f.mean(1, keepdims=True) if cfg.remove_dc_offset else 0.0
+    mu = f.mean(1, keepdims=True) if plan.remove_dc_offset else 0.0
     d = f - mu
-    a = cfg.preemph_coeff
+    a = plan.preemph_coeff
     pre = d - a * np.concatenate((d[:, :1], d[:, :-1]), 1) if a != 0.0 else d
     y = pre * win
-    e = (d * d).sum(1) if cfg.raw_energy else (y * y).sum(1)
+    e = (d * d).sum(1) if plan.raw_energy else (y * y).sum(1)
     X = np.fft.rfft(y, n=N)
     P = X.real ** 2 + X.imag ** 2
-    v = np.sqrt(P) if cfg.use_fft_mag else P
+    v = np.sqrt(P) if plan.use_fft_mag else P
     G = np.asarray(G, dtype=np.float64)
-    g_le = G[:, 0] if cfg.use_energy else np.zeros(G.shape[0])
-    if cfg.feature in ("fbank", "mfcc"):
+    ecol = energy_col(plan, G.shape[1])
+    g_le = G[:, ecol] if plan.use_energy else np.zeros(G.shape[0])
+    if plan.feature in ("fbank", "mfcc"):
         mel = v @ fb
-        if cfg.feature == "fbank":
-            gml = G[:, 1:] if cfg.use_energy else G
+        if plan.feature == "fbank":
+            gml = np.delete(G, ecol, 1) if plan.use_energy else G
         else:
             gc = G.copy()
-            if cfg.use_energy:
-                gc[:, 0] = 0.0
+            if plan.use_energy:
+                gc[:, ecol] = 0.0
             if lifter is not None:
                 gc = gc * lifter
             gml = gc @ dct.T
-        gv = (gml * _dlog_max(mel, EPS32)) @ fb.T
+        gv = (gml * _dlog_max(mel, plan.mel_floor)) @ fb.T
     else:
         gv = G.copy()
-        if cfg.feature == "log-spectrogram":
-            gv = gv / (v + 1e-15)
-        if cfg.use_energy:
+        if plan.feature == "log-spectrogram":
+            gv = gv * (_dlog_max(v, -plan.log_spec_eps) if plan.log_spec_eps < 0 else 1.0 / (v + plan.log_spec_eps))
+        if plan.use_energy:
             gv[:, 0] = 0.0
-    ge = g_le / (e + 1e-15)
-    if cfg.energy_floor > 0.0:
+    if plan.energy_style == ENERGY_KALDI:
+        lv = np.log(np.maximum(e, EPS32))
+        ge = g_le * _dlog_max(e, EPS32)
+    else:
         lv = np.log(e + 1e-15)
-        fl = math.log(cfg.energy_floor)
+        ge = g_le / (e + 1e-15)
+    if energy_floor_binds(plan):
+        fl = math.log(plan.energy_floor)
         ge = ge * np.where(lv > fl, 1.0, np.where(lv == fl, 0.5, 0.0))
-    if cfg.use_fft_mag:
+    if plan.use_fft_mag:
         A = v
         Z = np.where(A > 0, 0.5 * gv / np.where(A > 0, A, 1.0), 0.0) * X
     else:
@@ -192,16 +290,16 @@ def restated_grad(x: np.ndarray, cfg, G: np.ndarray) -> np.ndarray:
     if N % 2 == 0:
         H[:, N // 2] = 2.0 * Z[:, N // 2].real
     gy = N * np.fft.irfft(H, n=N)[:, :L]
-    if cfg.use_energy and not cfg.raw_energy:
+    if plan.use_energy and not plan.raw_energy:
         gy = gy + 2.0 * ge[:, None] * y
     gpre = gy * win
     gd = gpre.copy()
     if a != 0.0:
         gd[:, :-1] -= a * gpre[:, 1:]
         gd[:, 0] -= a * gpre[:, 0]
-    if cfg.use_energy and cfg.raw_energy:
+    if plan.use_energy and plan.raw_energy:
         gd = gd + 2.0 * ge[:, None] * d
-    if cfg.remove_dc_offset:
+    if plan.remove_dc_offset:
         gd = gd - gd.mean(1, keepdims=True)
     gx = np.zeros(n)
     np.add.at(gx, idx, gd)
@@ -267,28 +365,33 @@ def host_check_binary(tmp_dir):
 
 
 def host_check_input(path, cfg, x: np.ndarray, G: np.ndarray):
-    """The harness's input file: int32 header, float32 scalars, then the float32 tables, the waveform and the row gradient."""
-    L, S, N = O.layer_sizes(cfg)
-    win, fb, dct, lifter = O._cached_tables(astuple(cfg), torch.float32)
-    feat = {"fbank": 0, "mfcc": 1, "spectrogram": 2, "log-spectrogram": 3}[cfg.feature]
-    M = cfg.num_filters if feat in (0, 1) else 0
-    C = cfg.num_ceps if feat == 1 else 0
+    """The harness's input file: int32 header, float32 scalars, then the float32 tables, the waveform and the row gradient.
+    `cfg` is an oracle config (its float32 tables) or a FeaturePlan, whose energy style, energy column, mel shift and
+    log-spectrogram floor the header then carries (b200feat.cu bwd_plan)."""
+    plan = oracle_plan(cfg, torch.float32) if isinstance(cfg, O.OracleConfig) else cfg
+    L, S, N = plan.L, plan.S, plan.N
+    feat = {"fbank": 0, "mfcc": 1, "spectrogram": 2, "log-spectrogram": 3}[plan.feature]
+    M = plan.num_filters if feat in (0, 1) else 0
+    C = plan.num_ceps if feat == 1 else 0
     T, F = G.shape
-    use_lifter = int(feat == 1 and lifter is not None)
-    shift = 1 if (feat == 0 and cfg.use_energy) else 0
-    hdr = np.asarray([feat, L, S, N, M, C, F, int(cfg.snip_edges), int(cfg.remove_dc_offset), int(cfg.use_energy),
-                      int(cfg.raw_energy), int(cfg.use_fft_mag), 0, use_lifter, 0, shift, x.shape[0], T, (L - S) // 2, 0],
-                     dtype=np.int32)
-    has_floor = cfg.energy_floor > 0.0
-    sc = np.asarray([cfg.preemph_coeff, math.log(cfg.energy_floor) if has_floor else 0.0, 1.0 if has_floor else 0.0, EPS32,
-                     1e-15, 0.0], dtype=np.float32)
-    parts = [hdr.tobytes(), sc.tobytes(), win.numpy().astype(np.float32).tobytes()]
+    use_lifter = int(feat == 1 and plan.lifter is not None)
+    ecol = energy_col(plan, F) if plan.use_energy else 0
+    shift = 1 if (feat == 0 and plan.use_energy and not plan.energy_last) else 0
+    hdr = np.asarray([feat, L, S, N, M, C, F, int(plan.snip_edges), int(plan.remove_dc_offset), int(plan.use_energy),
+                      int(plan.raw_energy), int(plan.use_fft_mag), int(plan.energy_style), use_lifter, ecol, shift, x.shape[0], T,
+                      (L - S) // 2, 0], dtype=np.int32)
+    has_floor = energy_floor_binds(plan)
+    floor_form = plan.log_spec_eps < 0
+    sc = np.asarray([plan.preemph_coeff, math.log(plan.energy_floor) if has_floor else 0.0, 1.0 if has_floor else 0.0,
+                     plan.mel_floor, 0.0 if floor_form else plan.log_spec_eps, -plan.log_spec_eps if floor_form else 0.0],
+                    dtype=np.float32)
+    parts = [hdr.tobytes(), sc.tobytes(), np.asarray(plan.window, dtype=np.float32).tobytes()]
     if M:
-        parts.append(np.ascontiguousarray(fb.numpy(), dtype=np.float32).tobytes())
+        parts.append(np.ascontiguousarray(plan.mel_bank, dtype=np.float32).tobytes())
     if C:
-        parts.append(np.ascontiguousarray(dct.numpy(), dtype=np.float32).tobytes())
+        parts.append(np.ascontiguousarray(plan.dct, dtype=np.float32).tobytes())
     if use_lifter:
-        parts.append(lifter.numpy().astype(np.float32).tobytes())
+        parts.append(np.asarray(plan.lifter, dtype=np.float32).tobytes())
     parts += [x.astype(np.float32).tobytes(), np.ascontiguousarray(G, dtype=np.float32).tobytes()]
     with open(path, "wb") as fh:
         fh.write(b"".join(parts))
