@@ -1396,7 +1396,6 @@ int b200feat_feature_mix(b200feat_handle *h, const float *src_dev, int64_t src_e
       (ntracks > 0 && !tracks))
     return fail(h, B200FEAT_EINVAL, "feature_mix: bad arguments");
   if (ncuts == 0 || T_max == 0) return B200FEAT_OK;
-  if (ncuts > 65535) return fail(h, B200FEAT_EINVAL, "feature_mix: more than 65535 cuts in one call");
   if ((int64_t)ntracks * FM_PARTS > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "feature_mix: too many tracks in one call");
   const int64_t tiles = ((int64_t)T_max * F + FM_TILE - 1) / FM_TILE;
   if (tiles > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "feature_mix: T_max * F too large");
@@ -1469,8 +1468,8 @@ int b200feat_feature_mix(b200feat_handle *h, const float *src_dev, int64_t src_e
   featmix_gain_kernel<<<(unsigned)((ncuts + FM_GAIN_THREADS - 1) / FM_GAIN_THREADS), FM_GAIN_THREADS, 0, st>>>(d_tracks, d_cuts, ncuts,
                                                                                                                partial, gain);
   CU_TRY(h, cudaGetLastError());
-  featmix_out_kernel<<<dim3((unsigned)tiles, (unsigned)ncuts), FM_THREADS, 0, st>>>(src_dev, d_tracks, d_cuts, gain, F, T_max, pad_value,
-                                                                                      out_dev);
+  featmix_out_kernel<<<dim3((unsigned)tiles, (unsigned)std::min(ncuts, 65535)), FM_THREADS, 0, st>>>(src_dev, d_tracks, d_cuts, ncuts, gain,
+                                                                                                     F, T_max, pad_value, out_dev);
   CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }

@@ -6,14 +6,18 @@
 //   energy   E_t = the float64 sum of e^x (log law) or x (linear law) over track t's rows: FM_PARTS CTAs per track, CTA p
 //            summing chunks p, p + FM_PARTS, ... of FM_CHUNK elements, each thread in element order, then a fixed tree per
 //            CTA; the gains fold the parts in order
-//   gains    a track with an SNR and every later mixed track: g = E_ref * factor / E_t when E_ref > 0 and E_t > 0, else 1;
-//            the first track only when the reference is another track (_scale_features_for_snr), stored as log g for the
-//            log law (x + log g) and g for the linear law (g x)
+//   gains    a later mixed track with an SNR: g = E_ref * factor / E_t when E_ref > 0 and E_t > 0, else 1 (FeatureMixer);
+//            the first track with an SNR, only when the reference is another track: the same g unless E_ref <= 0 or E_t <= 0
+//            (_scale_features_for_snr's rejections, so a NaN energy gives a NaN gain), stored as log g for the log law
+//            (x + log g) and g for the linear law (g x)
 //   output   per element in float64, rounded once: the base (the scaled first track, -1000 past its rows), then every further
 //            mixed track folded in track order with -1000 outside its rows: s = max(EPSILON, s + g e^b) over s = e^base and a
 //            final log (log law), or s + g b (linear law); a cut with no further track is its base.  Mix row m = min(r,
 //            mix_rows - 1) (trimmed, or the last row repeated).  COPY cuts are their track's rows and then pad_value; rows
 //            past a cut's num_rows are the call's pad value.
+//   non-finite values  NaN and +-inf follow lhotse's float64 code element by element: the clamp keeps a NaN (np.maximum),
+//            inf * 0 is NaN, and a COPY cut is its rows bit for bit.
+//   cuts     any number: the output kernel's grid y is min(cuts, 65535) and strides over the rest.
 //
 // The per-element, per-thread and per-cut arithmetic is __host__ __device__, so that scripts/micro/featmix_host_check.cu runs
 // exactly this code on the CPU.  Kernels at the end.
@@ -64,17 +68,19 @@ MIX_HD double fm_energy(const double *partial, int64_t t) {
 
 MIX_HD bool fm_has_snr(const b200feat_featmix_track &t) { return t.snr_factor == t.snr_factor; }
 
-// gain[t] of every track of a MIX cut (the first track's as log g under the log law); COPY cuts leave 1
+// gain[t] of every track of a MIX cut (the first track's as log g under the log law); COPY cuts leave 1.  The first track
+// takes _scale_features_for_snr's rejections (E <= 0 keeps 1, so a NaN energy scales by NaN), later tracks FeatureMixer's
+// acceptance (E > 0 scales, so a NaN energy keeps 1)
 MIX_HD void fm_gains(const b200feat_featmix_cut &cu, const b200feat_featmix_track *tracks, const double *partial, double *gain) {
   const int64_t t0 = cu.first_track;
   const double e_ref = cu.mode == B200FEAT_FEATMIX_MIX ? fm_energy(partial, t0 + cu.ref_track) : 0.0;
   for (int k = 0; k < cu.num_tracks; ++k) {
     const b200feat_featmix_track &t = tracks[t0 + k];
     double g = 1.0;
-    if (cu.mode == B200FEAT_FEATMIX_MIX && (t.flags & B200FEAT_FEATMIX_MIXED) && fm_has_snr(t) && (k > 0 || cu.ref_track != 0) &&
-        e_ref > 0.0) {
+    if (cu.mode == B200FEAT_FEATMIX_MIX && (t.flags & B200FEAT_FEATMIX_MIXED) && fm_has_snr(t) && (k > 0 || cu.ref_track != 0)) {
       const double e = fm_energy(partial, t0 + k);
-      if (e > 0.0) g = MIX_DDIV(MIX_DMUL(e_ref, t.snr_factor), e);
+      const bool scale = k == 0 ? !(e_ref <= 0.0) && !(e <= 0.0) : e_ref > 0.0 && e > 0.0;
+      if (scale) g = MIX_DDIV(MIX_DMUL(e_ref, t.snr_factor), e);
     }
     gain[t0 + k] = (k == 0 && cu.law == B200FEAT_FEATMIX_LOG) ? FM_DLOG(g) : g;
   }
@@ -104,7 +110,7 @@ MIX_HD float fm_output(const float *src, const b200feat_featmix_track *tracks, c
     const double v = inside ? (double)fm_track_x(src, t, F, m - t.offset, c) : FM_DUMMY;
     if (log_law) {
       const double y = MIX_DADD(s, MIX_DMUL(gain[t0 + k], FM_DEXP(v)));
-      s = y > FM_EPSILON ? y : FM_EPSILON;
+      s = y < FM_EPSILON ? FM_EPSILON : y;  // np.maximum: a NaN stays NaN
     } else {
       s = MIX_DADD(s, MIX_DMUL(gain[t0 + k], v));
     }
@@ -142,17 +148,20 @@ __global__ void __launch_bounds__(FM_GAIN_THREADS) featmix_gain_kernel(const b20
   if (c < ncuts) fm_gains(cuts[c], tracks, partial, gain);
 }
 
-// grid (tiles, cuts): CTA (x, y) writes elements [x * FM_TILE, (x + 1) * FM_TILE) of cut y's (T_max, F) output
+// grid (tiles, min(cuts, 65535)): CTA (x, y) writes elements [x * FM_TILE, (x + 1) * FM_TILE) of cuts y, y + gridDim.y, ...
+// of the (T_max, F) outputs
 __global__ void __launch_bounds__(FM_THREADS) featmix_out_kernel(const float *__restrict__ src,
                                                                  const b200feat_featmix_track *__restrict__ tracks,
-                                                                 const b200feat_featmix_cut *__restrict__ cuts,
+                                                                 const b200feat_featmix_cut *__restrict__ cuts, int ncuts,
                                                                  const double *__restrict__ gain, int F, int T_max, float pad_value,
                                                                  float *__restrict__ out) {
-  const b200feat_featmix_cut cu = cuts[blockIdx.y];
   const int64_t n = (int64_t)T_max * F;
-  float *dst = out + (int64_t)blockIdx.y * n;
   const int64_t e1 = min(n, ((int64_t)blockIdx.x + 1) * FM_TILE);
-  for (int64_t e = (int64_t)blockIdx.x * FM_TILE + threadIdx.x; e < e1; e += FM_THREADS)
-    dst[e] = fm_output(src, tracks, cu, gain, F, e / F, (int)(e % F), pad_value);
+  for (int c = blockIdx.y; c < ncuts; c += gridDim.y) {
+    const b200feat_featmix_cut cu = cuts[c];
+    float *dst = out + (int64_t)c * n;
+    for (int64_t e = (int64_t)blockIdx.x * FM_TILE + threadIdx.x; e < e1; e += FM_THREADS)
+      dst[e] = fm_output(src, tracks, cu, gain, F, e / F, (int)(e % F), pad_value);
+  }
 }
 #endif

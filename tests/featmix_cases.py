@@ -40,7 +40,14 @@ def track_rows(src, t, F):
 
 
 def evaluate(src, tracks, cuts, F, T, pad_value):
-    """The tables evaluated in float64 the way lhotse's FeatureMixer folds them: (B, T, F) float64."""
+    """The tables evaluated in float64 the way lhotse's FeatureMixer folds them: (B, T, F) float64.  The first track is scaled
+    by _scale_features_for_snr's rejections (`<= 0` keeps it, so a NaN energy scales by NaN), later tracks by FeatureMixer's
+    acceptance (`> 0` scales, so a NaN energy keeps gain 1)."""
+    with np.errstate(all="ignore"):
+        return _evaluate(src, tracks, cuts, F, T, pad_value)
+
+
+def _evaluate(src, tracks, cuts, F, T, pad_value):
     out = np.full((len(cuts), T, F), np.float64(np.float32(pad_value)))
     for c, cu in enumerate(cuts):
         t0, nt, nr = int(cu["first_track"]), int(cu["num_tracks"]), int(cu["num_rows"])
@@ -54,9 +61,9 @@ def evaluate(src, tracks, cuts, F, T, pad_value):
         law = int(cu["law"])
         ref = t0 + int(cu["ref_track"])
         e_ref = law_energy(law, track_rows(src, tracks[ref], F))
-        if int(cu["ref_track"]) != 0 and not math.isnan(base["snr_factor"]) and e_ref > 0:
+        if int(cu["ref_track"]) != 0 and not math.isnan(base["snr_factor"]) and not e_ref <= 0:
             e0 = law_energy(law, brow)
-            if e0 > 0:
+            if not e0 <= 0:
                 brow = law_scale(law, brow, e_ref * float(base["snr_factor"]) / e0)
         mix_rows = int(cu["mix_rows"])
         mix = np.full((mix_rows, F), DUMMY)
@@ -98,19 +105,22 @@ def check_gate(ours, lhotse32, truth64, what=""):
 
 # ---- archive-backed cut sets ----------------------------------------------------------------------------------------------
 
-def write_features(writer, rs, frames, F, kind="log"):
-    """Seeded log-mel-like rows (log law) or non-negative power-like rows (linear law)."""
+def write_features(writer, rs, frames, F, kind="log", cells=()):
+    """Seeded log-mel-like rows (log law) or non-negative power-like rows (linear law), then the (row, col, value) `cells`."""
     x = rs.randn(frames, F).astype(np.float32)
     if kind == "log":
         x = (x * 2.0 - 6.0 + np.linspace(0, 3, F, dtype=np.float32)).astype(np.float32)
     else:
         x = np.abs(x * 3.0).astype(np.float32)
+    for r, c, v in cells:
+        x[r, c] = v
     return writer.write("k", x), x
 
 
 def make_cuts(storage, frames_list, F=80, seed=0, prefix="c", ftype="b200-fbank", kind="log", frame_shift=0.01, sr=16000,
-              supervisions=True):
-    """One feature-only MonoCut per entry of `frames_list`, its rows appended to the archive at `storage`."""
+              supervisions=True, cells=None):
+    """One feature-only MonoCut per entry of `frames_list`, its rows appended to the archive at `storage`; `cells[i]` are
+    (row, col, value) cells written over cut i's rows."""
     from lhotse import CutSet, MonoCut, SupervisionSegment
     from lhotse.features.base import Features
 
@@ -120,7 +130,7 @@ def make_cuts(storage, frames_list, F=80, seed=0, prefix="c", ftype="b200-fbank"
     cuts = []
     with B200ArchiveWriter(storage, mode="a") as w:
         for i, n in enumerate(frames_list):
-            key, _ = write_features(w, rs, n, F, kind)
+            key, _ = write_features(w, rs, n, F, kind, (cells or {}).get(i, ()))
             dur = round(n * frame_shift, 6)
             fm = Features(type=ftype, num_frames=n, num_features=F, frame_shift=frame_shift, sampling_rate=sr, start=0.0,
                           duration=dur, storage_type="b200_archive", storage_path=str(w.storage_path), storage_key=key,

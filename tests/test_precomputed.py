@@ -240,7 +240,7 @@ def _call(tr, cu, F=4, T=10, src_elems=100, work=None):
 
 @pytest.mark.parametrize("name", ["track_size", "cut_size", "cut_link", "flags", "rows", "stored_rows", "source", "mode", "law",
                                   "ref", "ref_energy", "snr_energy", "first_offset", "mix_rows", "adjust", "copy_tracks",
-                                  "num_rows", "empty_further", "work", "cuts_limit"])
+                                  "num_rows", "empty_further", "work"])
 def test_abi_refuses_malformed_tables(name):
     tr, cu = _tables()
     kw = {}
@@ -283,11 +283,22 @@ def test_abi_refuses_malformed_tables(name):
         tr["num_rows"][1] = tr["stored_rows"][1] = 0
     elif name == "work":
         kw["work"] = 16
-    elif name == "cuts_limit":
-        tr, cu = _tables(65536)
-        tr["src_elem"] = np.tile([0, 40], 65536)
     rc, msg = _call(tr, cu, **kw)
     assert rc == -1 and msg.startswith("feature_mix"), (name, rc, msg)
+
+
+def test_abi_checks_every_cut_past_65535():
+    """No limit on the number of cuts in one call (the output kernel strides over grid y): a table of 65536 cuts gets past
+    the count, and its last cut and last track are checked like the first.  The accepted call runs on the GPU in
+    test_featmix_kernel_edges.py::test_batch_shapes."""
+    tr, cu = _tables(65536)
+    cu["mode"][65535] = 2
+    rc, msg = _call(tr, cu)
+    assert rc == -1 and msg.startswith("feature_mix: cut 65535: bad mode"), (rc, msg)
+    tr, cu = _tables(65536)
+    tr["src_elem"][131071] = 90
+    rc, msg = _call(tr, cu)
+    assert rc == -1 and msg.startswith("feature_mix: track 131071: rows outside the source buffer"), (rc, msg)
 
 
 @needs_ref
