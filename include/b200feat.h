@@ -601,6 +601,24 @@ int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, 
                       int32_t B, const float *grad_out_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
                       int64_t work_bytes, void *stream);
 
+/*
+ * Right-padding collation of a ragged waveform buffer into a (B, T) float32 batch on the GPU: what lhotse's collate_audio
+ * returns for mono cuts (DESIGN.md §3.1o).  Row b holds cut b's samples (int16 sources widened as q / 32768, exactly as
+ * B200FEAT_I16 is widened for the feature kernels; float32 sources as they are), then zeros up to T.
+ */
+/* Device scratch b200feat_collate_audio needs for B cuts (0 when B is negative). */
+int64_t b200feat_collate_audio_work_bytes(int32_t B);
+
+/* `src_dev` (B200FEAT_F32 or B200FEAT_I16, `src_elems` elements; 16-byte aligned for F32, 8-byte for I16) holds cut b's
+ * `lens[b]` samples from element `offsets[b]` (host arrays of B).  Checks the tables on the host before anything touches the
+ * device (a negative offset or length, a length above T, samples outside the source buffer, an unknown dtype: each its own
+ * message), copies them to `work_dev` and launches one kernel, asynchronously on `stream`.  Every element of the (B, T)
+ * output `out_dev` is written exactly once, zeros included; elements outside it are not touched.  Errors are reported
+ * through `h` (b200feat_last_error) when it is not NULL, and through b200feat_global_error. */
+int b200feat_collate_audio(b200feat_handle *h, const void *src_dev, int32_t dt, int64_t src_elems, const int64_t *offsets,
+                           const int64_t *lens, int32_t B, int64_t T, float *out_dev, void *work_dev, int64_t work_bytes,
+                           void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -37,6 +37,7 @@ from .pcm_staging import MixRequest, mix_cuts, mix_request_for_cut  # noqa: F401
 from .pcm_staging import ReverbRequest, TransformRequest, transform_cuts, transform_request_for_cut  # noqa: F401
 from .spec_augment import B200SpecAugment, spec_augment_plan  # noqa: F401
 from .precomputed import FusedPrecomputedFeatures, precomputed_plan  # noqa: F401
+from .input_strategies import FusedAudioSamples  # noqa: F401
 
 __version__ = "0.1.0"
 

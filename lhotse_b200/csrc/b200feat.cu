@@ -33,6 +33,7 @@
 #include "rirgen.cuh"
 #include "featmix.cuh"
 #include "backward.cuh"
+#include "collate.cuh"
 
 #include <cub/device/device_segmented_radix_sort.cuh>
 
@@ -1470,6 +1471,50 @@ int b200feat_feature_mix(b200feat_handle *h, const float *src_dev, int64_t src_e
   CU_TRY(h, cudaGetLastError());
   featmix_out_kernel<<<dim3((unsigned)tiles, (unsigned)std::min(ncuts, 65535)), FM_THREADS, 0, st>>>(src_dev, d_tracks, d_cuts, ncuts, gain,
                                                                                                      F, T_max, pad_value, out_dev);
+  CU_TRY(h, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+int64_t b200feat_collate_audio_work_bytes(int32_t B) { return B < 0 ? 0 : (int64_t)B * 2 * (int64_t)sizeof(int64_t); }
+
+int b200feat_collate_audio(b200feat_handle *h, const void *src_dev, int32_t dt, int64_t src_elems, const int64_t *offsets,
+                           const int64_t *lens, int32_t B, int64_t T, float *out_dev, void *work_dev, int64_t work_bytes,
+                           void *stream) {
+  if (dt != B200FEAT_F32 && dt != B200FEAT_I16) return fail(h, B200FEAT_EINVAL, "collate_audio: unknown dtype " + std::to_string(dt));
+  if (B < 0 || T < 0 || src_elems < 0) return fail(h, B200FEAT_EINVAL, "collate_audio: negative B, T or source size");
+  if (B > 0 && (!offsets || !lens)) return fail(h, B200FEAT_EINVAL, "collate_audio: missing offset or length table");
+  auto where = [](int64_t b) { return std::string("collate_audio: cut ") + std::to_string(b) + ": "; };
+  for (int32_t b = 0; b < B; ++b) {
+    if (offsets[b] < 0) return fail(h, B200FEAT_EINVAL, where(b) + "negative offset " + std::to_string(offsets[b]));
+    if (lens[b] < 0) return fail(h, B200FEAT_EINVAL, where(b) + "negative length " + std::to_string(lens[b]));
+    if (lens[b] > T)
+      return fail(h, B200FEAT_EINVAL, where(b) + "length " + std::to_string(lens[b]) + " above T = " + std::to_string(T));
+    if (offsets[b] > src_elems - lens[b])
+      return fail(h, B200FEAT_EINVAL, where(b) + "samples [" + std::to_string(offsets[b]) + ", " + std::to_string(offsets[b] + lens[b]) +
+                                           ") outside the source buffer of " + std::to_string(src_elems) + " elements");
+  }
+  if (B == 0 || T == 0) return B200FEAT_OK;
+  if (!out_dev || !work_dev) return fail(h, B200FEAT_EINVAL, "collate_audio: missing output or work buffer");
+  if (src_elems > 0 && !src_dev) return fail(h, B200FEAT_EINVAL, "collate_audio: missing source buffer");
+  if ((uintptr_t)src_dev % (dt == B200FEAT_F32 ? 16 : 8))
+    return fail(h, B200FEAT_EINVAL, "collate_audio: source buffer not 16-byte (float32) / 8-byte (int16) aligned");
+  if ((uintptr_t)out_dev % 4) return fail(h, B200FEAT_EINVAL, "collate_audio: output not 4-byte aligned");
+  if (work_bytes < b200feat_collate_audio_work_bytes(B)) return fail(h, B200FEAT_EINVAL, "collate_audio: work buffer too small");
+  // the units of the longest row (the head and tail units of every row included) over CTAs of CO_THREADS * CO_UNITS_PER_THREAD
+  const int64_t tiles = (co_units(T / 4) + CO_THREADS * CO_UNITS_PER_THREAD - 1) / (CO_THREADS * CO_UNITS_PER_THREAD);
+  if (tiles > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "collate_audio: T too large");
+  std::vector<int64_t> tab((size_t)B * 2);
+  std::copy(offsets, offsets + B, tab.begin());
+  std::copy(lens, lens + B, tab.begin() + B);
+  const cudaStream_t st = (cudaStream_t)stream;
+  // a pageable copy: it returns once the table has been staged, so the table may go when this function returns
+  CU_TRY(h, cudaMemcpyAsync(work_dev, tab.data(), tab.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  const dim3 grid((unsigned)tiles, (unsigned)std::min(B, 65535));
+  const int base_mod4 = (int)(((uintptr_t)out_dev / 4) % 4);
+  if (dt == B200FEAT_F32)
+    collate_audio_kernel<float><<<grid, CO_THREADS, 0, st>>>((const float *)src_dev, (const int64_t *)work_dev, B, T, base_mod4, out_dev);
+  else
+    collate_audio_kernel<int16_t><<<grid, CO_THREADS, 0, st>>>((const int16_t *)src_dev, (const int64_t *)work_dev, B, T, base_mod4, out_dev);
   CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }

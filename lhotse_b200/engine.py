@@ -131,6 +131,7 @@ EXPORTS = [
     "b200feat_reverb_work_bytes", "b200feat_reverb", "b200feat_specaug_work_bytes", "b200feat_specaug",
     "b200feat_reverb_ex", "b200feat_rir_generate_work_bytes", "b200feat_rir_generate",
     "b200feat_feature_mix_work_bytes", "b200feat_feature_mix", "b200feat_backward_work_bytes", "b200feat_backward",
+    "b200feat_collate_audio_work_bytes", "b200feat_collate_audio",
 ]
 
 
@@ -228,6 +229,10 @@ def load_library():
         lib.b200feat_backward_work_bytes.argtypes = [vp, vp, i32]
         lib.b200feat_backward.restype = C.c_int
         lib.b200feat_backward.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, vp, i64, vp]
+        lib.b200feat_collate_audio_work_bytes.restype = i64
+        lib.b200feat_collate_audio_work_bytes.argtypes = [i32]
+        lib.b200feat_collate_audio.restype = C.c_int
+        lib.b200feat_collate_audio.argtypes = [vp, vp, i32, i64, vp, vp, i32, i64, vp, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -441,6 +446,29 @@ def feature_mix(src: Optional[torch.Tensor], tracks: np.ndarray, cuts: np.ndarra
     with torch.cuda.device(out.device):
         rc = lib.b200feat_feature_mix(handle, p, n, tracks.ctypes.data, len(tracks), cuts.ctypes.data, len(cuts), F,
                                       out.data_ptr(), T, float(pad_value), work.data_ptr(), work.numel(), stream)
+    if rc != 0:
+        _raise(lib, rc, handle)
+
+
+def collate_audio(src: Optional[torch.Tensor], offsets: Sequence[int], lens: Sequence[int], out: torch.Tensor,
+                  handle=None) -> None:
+    """Launches `b200feat_collate_audio` on the current stream of `out`'s device (asynchronous, no synchronisation): row b of
+    the contiguous float32 (B, T) output `out` is cut b's `lens[b]` samples from element `offsets[b]` of the 1-D int16 or
+    float32 device buffer `src` (None = empty; int16 widened as q / 32768), then zeros.  Raises B200FeatError when the library
+    refuses the tables."""
+    lib = load_library()
+    assert out.dtype == torch.float32 and out.dim() == 2 and out.is_contiguous() and out.shape[0] == len(lens) == len(offsets)
+    assert src is None or (src.dim() == 1 and src.is_contiguous() and src.device == out.device)
+    dt = DT_F32 if src is None else {torch.float32: DT_F32, torch.int16: DT_I16}[src.dtype]
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    ln = np.ascontiguousarray(lens, dtype=np.int64)
+    B, T = out.shape
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    work = torch.empty(max(int(lib.b200feat_collate_audio_work_bytes(B)), 1), dtype=torch.uint8, device=out.device)
+    p, n = (None, 0) if src is None or src.numel() == 0 else (src.data_ptr(), src.numel())
+    with torch.cuda.device(out.device):
+        rc = lib.b200feat_collate_audio(handle, p, dt, n, off.ctypes.data, ln.ctypes.data, B, T, out.data_ptr(), work.data_ptr(),
+                                        work.numel(), stream)
     if rc != 0:
         _raise(lib, rc, handle)
 

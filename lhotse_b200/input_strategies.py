@@ -1,5 +1,6 @@
 """
-"Next" row §8f-1 of the scope contract: the caller right after the hot path.
+"Next" row §8f-1 of the scope contract: the caller right after the hot path.  ``FusedAudioSamples`` (below) is the same for
+lhotse's ``AudioSamples``: the padded waveform batch of models that hold their front end, built on the GPU.
 
 ``FusedOnTheFlyFeatures`` is a drop-in for ``lhotse.dataset.input_strategies.OnTheFlyFeatures``
 (input_strategies.py:351-476) for the B200 extractors: same constructor arguments, same return tuple
@@ -199,3 +200,134 @@ class FusedOnTheFlyFeatures:
         from lhotse.dataset.input_strategies import OnTheFlyFeatures
 
         return OnTheFlyFeatures.supervision_masks(self, cuts, use_alignment_if_exists)
+
+
+class FusedAudioSamples:
+    """lhotse's ``AudioSamples`` (same constructor and call) with the waveform batch built on the GPU.  A batch that a staged
+    route takes (``pcm_staging.staged_route``: PCM16 WAV or FLAC slices, MixedCuts of them, speed / volume / resample
+    transforms, reverb with ``reverb`` / ``generated_rir``) is staged without padding cuts, made on the device by that route
+    and collated by one kernel (csrc/collate.cuh): ``(audio, audio_lens)`` equal to ``collate_audio``'s, audio (B, T) float32
+    on the current CUDA device (``audio_on_device=False``: on the CPU), (B, 1, T) with ``mono_downmix=False``, audio_lens int32
+    on the CPU (DESIGN.md §3.1o).  Other batches go to lhotse's ``collate_audio`` with the same arguments
+    (``last_batch_route == "reference"``, the reason in ``last_decline``); the staged ones name their route in
+    ``last_batch_route``."""
+
+    def __init__(
+        self,
+        num_workers: int = 0,
+        fault_tolerant: bool = False,
+        executor_type: Type = ThreadPoolExecutor,
+        use_batch_loader: bool = False,
+        ais_force_individual: bool = False,
+        mono_downmix: Optional[bool] = None,
+        audio_on_device: bool = True,
+        perturbed_tracks: bool = False,
+        reverb: bool = False,
+        generated_rir: bool = False,
+    ) -> None:
+        self.num_workers = num_workers
+        self.fault_tolerant = fault_tolerant
+        self._executor_type = executor_type
+        self._executor = None
+        self.mono_downmix = mono_downmix
+        self.use_batch_loader = use_batch_loader
+        self.ais_batch_loader = None
+        if use_batch_loader:  # as AudioSamples: AIStore fetches the whole batch, which then takes lhotse's collate_audio
+            from lhotse.ais import AISBatchLoader
+
+            self.ais_batch_loader = AISBatchLoader(force_individual=ais_force_individual, skip_failed_fetches=fault_tolerant)
+        self.audio_on_device = audio_on_device
+        # the staged routes' options, as in FusedOnTheFlyFeatures (off by default for the same reasons)
+        self.perturbed_tracks = perturbed_tracks
+        self.reverb = reverb
+        self.generated_rir = generated_rir
+        self._rings = {}  # route -> its staging ring, made when a batch first takes the route
+        self.last_batch_route = None  # one of pcm_staging.STAGED_ROUTES | "reference"
+        self.last_decline = None
+
+    def _get_executor(self):
+        if self.num_workers <= 0:
+            return None
+        if self._executor is None:
+            self._executor = self._executor_type(max_workers=self.num_workers)
+        return self._executor
+
+    def _decline_reason(self, cuts, recording_field) -> Optional[str]:
+        if recording_field is not None:
+            return "recording_field is set"
+        if self.use_batch_loader:
+            return "use_batch_loader is set"
+        if any(type(c).__name__ == "MultiCut" or (getattr(c, "num_channels", 1) or 1) > 1 for c in cuts):
+            return "a MultiCut or multi-channel cut"
+        if len({c.sampling_rate for c in cuts}) > 1:
+            return "more than one sampling rate"
+        return None
+
+    def _try_staged(self, cuts):
+        """(route, (B, T) audio on the current CUDA device) of a staged route, or a str: why lhotse takes the batch."""
+        from .pcm_staging import collate_staged, new_ring, staged_route, undo_draws
+
+        chosen = staged_route(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb,
+                              generated_rir=self.generated_rir)
+        if chosen is None:
+            return "a cut that no staged route takes"
+        route, reqs = chosen
+        ring = self._rings.get(route)
+        if ring is None:
+            ring = self._rings[route] = new_ring(route)
+        staged = None
+        try:  # a read or a FLAC frame that fails raises before any audio is handed back
+            staged, lens, offs, sr = ring.stage(reqs, executor=self._get_executor())
+            if sr != cuts[0].sampling_rate:
+                undo_draws(staged)  # lhotse draws the generated RIRs again
+                return "the staged sampling rate is not the cuts'"
+            audio = collate_staged(staged, lens, offs, torch.device("cuda", torch.cuda.current_device()), ring)
+        except (OSError, ValueError) as e:
+            undo_draws(staged)  # lhotse draws the generated RIRs again
+            if self.fault_tolerant:
+                return f"a staged read or decode failed: {e}"
+            raise
+        return route, audio
+
+    def __call__(self, cuts, recording_field: Optional[str] = None):
+        reason = self._decline_reason(cuts, recording_field)
+        fast = reason or self._try_staged(cuts)
+        if isinstance(fast, str):
+            return self._reference(cuts, recording_field, fast)
+        self.last_batch_route, audio = fast
+        self.last_decline = None
+        if self.mono_downmix is False:  # mono cuts in channel 0 of a (B, 1, T) batch, as collate_audio expands them
+            audio = audio.unsqueeze(1)
+        if not self.audio_on_device:
+            audio = audio.cpu()
+        audio_lens = torch.tensor([c.num_samples for c in cuts], dtype=torch.int32)
+        if not self.fault_tolerant:
+            return audio, audio_lens
+        # collate_audio hands back the cuts it read: the batch padded to its longest duration
+        from lhotse import CutSet
+
+        padded = CutSet.from_cuts(cuts).pad(duration=max(c.duration for c in cuts), direction="right", preserve_id=True)
+        return audio, audio_lens, padded
+
+    def _reference(self, cuts, recording_field, reason: str):
+        from lhotse.dataset.collation import collate_audio
+
+        self.last_batch_route, self.last_decline = "reference", reason
+        if self.use_batch_loader and self.ais_batch_loader is not None:
+            cuts = self.ais_batch_loader(cuts)
+        out = collate_audio(cuts, executor=self._get_executor(), fault_tolerant=self.fault_tolerant,
+                            recording_field=recording_field, mono_downmix=self.mono_downmix)
+        if self.audio_on_device:
+            out = (out[0].to(torch.device("cuda", torch.cuda.current_device())),) + tuple(out[1:])
+        return out
+
+    # lhotse's BatchIO protocol (input_strategies.py): used by K2SpeechRecognitionDataset for supervisions
+    def supervision_intervals(self, cuts):
+        from lhotse.dataset.input_strategies import AudioSamples
+
+        return AudioSamples.supervision_intervals(self, cuts)
+
+    def supervision_masks(self, cuts, use_alignment_if_exists: Optional[str] = None):
+        from lhotse.dataset.input_strategies import AudioSamples
+
+        return AudioSamples.supervision_masks(self, cuts, use_alignment_if_exists)

@@ -21,7 +21,8 @@ ragged buffer (no float copy on the host), cross PCIe as 2 bytes per sample and 
                                  transforms run by csrc/resample.cuh
 The mix and transform rings stage their int16 sources (WAV and FLAC slices, RIRs) through one `_SourceRing`.
 `staged_route(cuts)` picks the route of a batch (one of `STAGED_ROUTES`) with its requests, `new_ring(route)` makes the ring
-that stages them, and `staged_to_device` runs the device half of any staged batch.
+that stages them, and `staged_to_device` runs the device half of any staged batch; `collate_staged` turns it into lhotse's
+padded (B, T) waveform batch (csrc/collate.cuh).
 Everything here is host-side I/O; the arithmetic stays in the CUDA kernels.
 """
 from __future__ import annotations
@@ -1605,3 +1606,24 @@ def staged_to_device(staged, device, ring: Optional[_PinnedRing] = None,
     if ring is not None:
         ring.mark_in_flight(device)
     return buf, None, None
+
+
+def collate_staged(staged, lens: Sequence[int], offsets: Sequence[int], device, ring: Optional[_PinnedRing] = None,
+                   handle=None) -> torch.Tensor:
+    """`staged_to_device` and then the collation kernel (csrc/collate.cuh), on `device`'s current stream: the (B, T) float32
+    batch whose row b is cut b's samples and then zeros, T the longest cut, what lhotse's `collate_audio` returns for the same
+    cuts (DESIGN.md §3.1o).  `lens` / `offsets` are those the ring's `stage` returned (a raw int16 buffer's; a FLAC, mix or
+    transform batch brings its own)."""
+    from . import engine as E
+
+    device = torch.device(device)
+    with torch.cuda.device(device):
+        buf, staged_lens, staged_offsets = staged_to_device(staged, device, ring, handle=handle)
+        if staged_lens is not None:
+            lens, offsets = staged_lens, staged_offsets
+        if buf.data_ptr() % 16:  # a view with a storage offset: the kernel reads whole vectors from the buffer's start
+            buf = buf.clone()
+        lens, offsets = [int(n) for n in lens], [int(o) for o in offsets]
+        out = torch.empty((len(lens), max(lens, default=0)), dtype=torch.float32, device=device)
+        E.collate_audio(buf, offsets, lens, out, handle=handle)
+    return out
