@@ -357,14 +357,8 @@ int setup_handle(b200feat_handle *h, const float *window, const float *mel_bank,
   else if (desc->kernel == B200FEAT_KERNEL_GENERIC || !fast_ok) h->kernel = B200FEAT_KERNEL_GENERIC;
   else h->kernel = B200FEAT_KERNEL_FAST;
 
-  {  // generic launch shape: as many warps per CTA as fit ~100 KB, CTA <= 8 warps
-    const size_t per_warp = generic_smem_per_warp(p.N, p.Nc);
-    int w = (int)((100 * 1024) / per_warp);
-    if (w > 8) w = 8;
-    if (w < 1) w = 1;
-    h->generic_warps = w;
-    h->generic_smem = per_warp * w;
-    if (h->generic_smem > 227 * 1024)
+  {  // generic launch shape (generic.cuh)
+    if (!generic_launch_shape(p, &h->generic_warps, &h->generic_smem))
       return fail(nullptr, B200FEAT_EUNSUPPORTED, "fft_length too large for shared memory");
     if (h->generic_smem > 48 * 1024) {
       cudaError_t e1 = cudaFuncSetAttribute(b200feat_generic_kernel<B200FEAT_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->generic_smem);

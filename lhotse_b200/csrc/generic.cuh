@@ -75,10 +75,41 @@ __device__ __forceinline__ void stockham_pass(const float2 *__restrict__ src, fl
   }
 }
 
-// dynamic smem per warp (floats): raw[Nr] + 2 complex buffers of Nc
-__host__ __device__ inline int generic_raw_floats(int N) { return (N + 3) & ~3; }
-__host__ __device__ inline size_t generic_smem_per_warp(int N, int Nc) {
-  return (size_t)generic_raw_floats(N) * 4 + (size_t)Nc * 8 * 2;
+// Per-warp region of the dynamic shared memory, in floats from the warp's base (the host sizes the launch from the same
+// function, so the two cannot disagree):
+//   raw   [0, bufA)              the frame's L samples, then its K <= N spectrum values
+//   bufA  [bufA, bufA + 2 Nc)    the FFT's ping-pong buffers, Nc complex values each
+//   bufB  [bufB, bufB + 2 Nc)
+//   mlog  [bufA, bufA + M)       the MFCC epilogue's M log-mel values.  Both FFT buffers are dead once the spectrum is in
+//                                raw, so mlog reuses them from bufA on, and the region grows past bufB only when M > 4 Nc
+//                                (N = 16 with 40 filters, say).  Other features keep no scratch.
+// Every region starts on 8 bytes and every warp's base on 16.
+struct GenericLayout {
+  int bufA, bufB, mlog, floats;
+};
+__host__ __device__ inline GenericLayout generic_layout(const DevPlan &p) {
+  GenericLayout l;
+  l.bufA = (p.N + 3) & ~3;
+  l.bufB = l.bufA + 2 * p.Nc;
+  l.mlog = l.bufA;
+  const int scratch = p.feature == B200FEAT_MFCC ? (p.M + 3) & ~3 : 0;
+  l.floats = l.bufA + (4 * p.Nc > scratch ? 4 * p.Nc : scratch);
+  return l;
+}
+
+// The opt-in limit of dynamic shared memory per CTA on sm_90
+#define GENERIC_SMEM_OPTIN_MAX (227 * 1024)
+
+// Launch shape: as many warps per CTA as fit ~100 KB, at least 1 and at most 8.  False if one warp's region is over the
+// opt-in limit: N > 16384 for even N, N > 11621 for odd N (20 N bytes per warp).
+inline bool generic_launch_shape(const DevPlan &p, int *warps, size_t *smem) {
+  const size_t per_warp = (size_t)generic_layout(p).floats * sizeof(float);
+  int w = (int)((100 * 1024) / per_warp);
+  if (w > 8) w = 8;
+  if (w < 1) w = 1;
+  *warps = w;
+  *smem = per_warp * w;
+  return *smem <= GENERIC_SMEM_OPTIN_MAX;
 }
 
 template <int DT>
@@ -87,10 +118,11 @@ __global__ void __launch_bounds__(256) b200feat_generic_kernel(const DevPlan p, 
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int nwarps = blockDim.x >> 5;
-  unsigned char *mine = smem_raw + (size_t)warp * generic_smem_per_warp(p.N, p.Nc);
-  float *raw = reinterpret_cast<float *>(mine);
-  float2 *bufA = reinterpret_cast<float2 *>(mine + (size_t)generic_raw_floats(p.N) * 4);
-  float2 *bufB = bufA + p.Nc;
+  const GenericLayout lay = generic_layout(p);
+  float *raw = reinterpret_cast<float *>(smem_raw) + (size_t)warp * lay.floats;
+  float2 *bufA = reinterpret_cast<float2 *>(raw + lay.bufA);
+  float2 *bufB = reinterpret_cast<float2 *>(raw + lay.bufB);
+  float *mlog = raw + lay.mlog;
 
   // generic kernel: one tile == one output row
   for (int64_t g = (int64_t)blockIdx.x * nwarps + warp; g < b.num_tiles; g += (int64_t)gridDim.x * nwarps) {
@@ -190,7 +222,6 @@ __global__ void __launch_bounds__(256) b200feat_generic_kernel(const DevPlan p, 
       for (int k = lane; k < p.K; k += 32)
         out[k] = post_affine(p, k, (k == 0 && p.use_energy) ? le : log_spec_value(p, raw[k]));
     } else {
-      float *mlog = reinterpret_cast<float *>(dst);  // scratch (FFT buffer not holding the result)
       const int shift = mel_shift(p), ecol = energy_col(p);
       float vmax = __int_as_float(0xff800000);  // -inf
       for (int m = lane; m < p.M; m += 32) {
