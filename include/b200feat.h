@@ -587,8 +587,9 @@ int b200feat_feature_mix(b200feat_handle *h, const float *src_dev, int64_t src_e
  * b200feat_extract produced from the same samples (DESIGN.md §3.1n).  The frames are recomputed from the samples; nothing
  * of the forward is kept.
  */
-/* Device scratch b200feat_backward needs for cuts of `num_samples` (host array of B), or a negative B200FEAT_E* code
- * (B200FEAT_ESHORT for a cut too short to be framed, B200FEAT_EINVAL for a kind without a backward). */
+/* Device scratch b200feat_backward (b200feat_whisper_backward for a whisper-fbank handle) needs for cuts of `num_samples`
+ * (host array of B), or a negative B200FEAT_E* code (B200FEAT_ESHORT for a cut too short to be framed, B200FEAT_EINVAL for a
+ * kind without a backward). */
 int64_t b200feat_backward_work_bytes(b200feat_handle *h, const int64_t *num_samples, int32_t B);
 
 /* `samples_dev` (B200FEAT_F32 only) holds cut i at element offsets[i] with num_samples[i] samples (host arrays); `grad_out_dev`
@@ -600,6 +601,29 @@ int64_t b200feat_backward_work_bytes(b200feat_handle *h, const int64_t *num_samp
 int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples, const int64_t *offsets,
                       int32_t B, const float *grad_out_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
                       int64_t work_bytes, void *stream);
+
+/*
+ * Backward of whisper-fbank (DESIGN.md §3.1p).  Its forward clamps every log-mel value to its cut's maximum - 8, a cut-wide
+ * decision a recomputation by another FFT cannot repeat bit for bit, so the backward reads the forward's own un-normalised
+ * log-mel rows and maxima, which b200feat_extract_keep_raw keeps.
+ */
+/* b200feat_extract for a whisper-fbank handle and a batch planned with B200FEAT_OUT_PACKED, keeping what the backward
+ * needs: the fused kernel writes the (total_rows, F) log-mel rows to `raw_dev`, followed by the B per-cut maxima
+ * (`tot->out_floats` floats in all), and the normalise pass writes the features to `out_dev` ((total_rows, F) floats),
+ * bitwise equal to b200feat_extract's.  Both buffers 16-byte aligned.  Two launches, asynchronous on `stream`. */
+int b200feat_extract_keep_raw(b200feat_handle *h, const void *samples_dev, int32_t dt, const int64_t *meta_dev, int32_t B,
+                              const b200feat_batch_totals *tot, float *out_dev, float *raw_dev, void *stream);
+
+/* b200feat_backward for a whisper-fbank handle (whose b200feat_backward refuses and names this entry), with the forward's
+ * log-mel rows `raw_dev` (laid out as grad_out_dev) and per-cut maxima `cut_max_dev` [B] from b200feat_extract_keep_raw.
+ * b200feat_backward_work_bytes gives the scratch it needs.  The same argument checks (a cut of n <= fft_length / 2
+ * samples: B200FEAT_ESHORT, as the forward; a row_off that does not match a cut's rows; samples other than
+ * B200FEAT_F32), then three launches: a per-cut reduction, frames, combine.  No atomics: results are identical from run to
+ * run, and a cut's gradient does not depend on the other cuts of the call.  The gradient of the extra zero row is ignored. */
+int b200feat_whisper_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples,
+                              const int64_t *offsets, int32_t B, const float *grad_out_dev, const float *raw_dev,
+                              const float *cut_max_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
+                              int64_t work_bytes, void *stream);
 
 /*
  * Right-padding collation of a ragged waveform buffer into a (B, T) float32 batch on the GPU: what lhotse's collate_audio

@@ -397,7 +397,8 @@ int setup_handle(b200feat_handle *h, const float *window, const float *mel_bank,
 int launch_range(b200feat_handle *h, const void *samples_dev, int32_t dt, const int64_t *meta_dev,
                         int32_t B, int32_t b0, int32_t b1, int64_t tile0, int64_t tile1,
                         int64_t max_frames, float *out_dev, int32_t out_mode, float pad_value,
-                        cudaStream_t stream, float *cut_max_dev = nullptr, int64_t norm_rows = 0) {
+                        cudaStream_t stream, float *cut_max_dev = nullptr, int64_t norm_rows = 0,
+                        float *norm_out = nullptr) {
   DevBatch db;
   db.samples = samples_dev;
   db.samp_off = meta_dev + b0;
@@ -441,12 +442,15 @@ int launch_range(b200feat_handle *h, const void *samples_dev, int32_t dt, const 
     if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("generic launch: ") + cudaGetErrorString(e));
   }
   if (h->plan.whisper && norm_rows > 0) {  // second launch: clamp to the cut's maximum - 8, (x + 4) / 4, zero rows
+    // norm_out: the fused kernel's log-mel rows stay where it wrote them, the normalised rows go to norm_out
+    const float *src = out_dev;
+    if (norm_out) db.out = norm_out;
     if (h->frames_per_tile > 1) {
       const unsigned blocks = persistent_grid(db.num_tiles, h->sm_count, 8);
-      b200feat_whisper_normalize_tiled_kernel<<<blocks, 256, 0, stream>>>(h->plan, db, h->frames_per_tile);
+      b200feat_whisper_normalize_tiled_kernel<<<blocks, 256, 0, stream>>>(h->plan, db, src, h->frames_per_tile);
     } else {
       const unsigned blocks = persistent_grid((norm_rows + 7) / 8, h->sm_count, 16);
-      b200feat_whisper_normalize_kernel<<<blocks, 256, 0, stream>>>(h->plan, db, norm_rows);
+      b200feat_whisper_normalize_kernel<<<blocks, 256, 0, stream>>>(h->plan, db, src, norm_rows);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(h, B200FEAT_ECUDA, std::string("whisper normalise launch: ") + cudaGetErrorString(e));
@@ -754,6 +758,27 @@ int b200feat_extract(b200feat_handle *h, const void *samples_dev, int32_t dt, co
     std::lock_guard<std::mutex> g(h->stats_mu);
     h->stats.calls++; h->stats.cuts += B; h->stats.frames += tot->total_rows;
     h->stats.kernel_launches += h->plan.whisper ? 2 : 1;
+  }
+  return B200FEAT_OK;
+}
+
+
+int b200feat_extract_keep_raw(b200feat_handle *h, const void *samples_dev, int32_t dt, const int64_t *meta_dev, int32_t B,
+                              const b200feat_batch_totals *tot, float *out_dev, float *raw_dev, void *stream) {
+  if (!h || !samples_dev || !meta_dev || !tot || !out_dev || !raw_dev || B <= 0)
+    return fail(h, B200FEAT_EINVAL, "extract_keep_raw: bad arguments");
+  if (!h->plan.whisper) return fail(h, B200FEAT_EINVAL, "extract_keep_raw: whisper-fbank handles only");
+  if (dt != B200FEAT_F32 && dt != B200FEAT_I16) return fail(h, B200FEAT_EINVAL, "bad sample dtype");
+  if (((uintptr_t)out_dev | (uintptr_t)raw_dev) & 15) return fail(h, B200FEAT_EINVAL, "extract_keep_raw: out and raw must be 16-byte aligned");
+  DeviceGuard on(h->device);
+  float *scratch = raw_dev + tot->total_rows * h->plan.F;
+  int rc = launch_range(h, samples_dev, dt, meta_dev, B, 0, B, 0, tot->total_tiles, tot->max_frames, raw_dev,
+                        B200FEAT_OUT_PACKED, 0.f, (cudaStream_t)stream, scratch, tot->total_rows, out_dev);
+  if (rc) return rc;
+  {
+    std::lock_guard<std::mutex> g(h->stats_mu);
+    h->stats.calls++; h->stats.cuts += B; h->stats.frames += tot->total_rows;
+    h->stats.kernel_launches += 2;
   }
   return B200FEAT_OK;
 }
@@ -1664,12 +1689,14 @@ int b200feat_rir_generate(b200feat_handle *h, const double *draws_dev, int64_t d
 
 namespace {
 
-// The backward's view of the handle's plan; false for a plan without a backward (whisper / log10 kinds, centre padding).
-bool bwd_plan(const b200feat_handle *h, BwdPlan *out) {
+// The backward's view of the handle's plan; false for a plan without a backward (log10-fbank).  whisper-fbank has one
+// through b200feat_whisper_backward only, which asks for it with `whisper`.
+bool bwd_plan(const b200feat_handle *h, BwdPlan *out, bool whisper = false) {
   const DevPlan &p = h->plan;
   const int f = p.feature;
-  if ((f != B200FEAT_FBANK && f != B200FEAT_MFCC && f != B200FEAT_SPECTROGRAM && f != B200FEAT_LOG_SPECTROGRAM) || p.whisper ||
-      p.log10_mel || p.pad_mode != B200FEAT_PAD_KALDI)
+  if (whisper != (p.whisper != 0)) return false;
+  if (!whisper && ((f != B200FEAT_FBANK && f != B200FEAT_MFCC && f != B200FEAT_SPECTROGRAM && f != B200FEAT_LOG_SPECTROGRAM) ||
+                   p.log10_mel || p.pad_mode != B200FEAT_PAD_KALDI))
     return false;
   BwdPlan b;
   memset(&b, 0, sizeof(b));
@@ -1683,6 +1710,7 @@ bool bwd_plan(const b200feat_handle *h, BwdPlan *out) {
   b.window = p.window; b.tws = reinterpret_cast<const BwdC *>(p.tws);
   b.mel_start = p.mel_start; b.mel_len = p.mel_len; b.mel_woff = p.mel_woff; b.mel_w = p.mel_w;
   b.dct = p.dct; b.lifter = p.lifter; b.post_scale = p.post_scale;
+  b.whisper = p.whisper; b.reflect = p.pad_mode == B200FEAT_PAD_CENTER ? 1 : 0;
   *out = b;
   return true;
 }
@@ -1695,10 +1723,11 @@ int64_t bwd_layout(b200feat_handle *h, const BwdPlan &p, int ft, const int64_t *
   for (int i = 0; i < B; ++i) {
     const int64_t T = cut_frames(h, i, num_samples[i]);
     if (T < 0) return T;
-    tiles += (T + ft - 1) / ft;
+    const int64_t frames = bwd_frames(p, num_samples[i], T);
+    tiles += (frames + ft - 1) / ft;
     if (tile_off) (*tile_off)[i + 1] = tiles;
   }
-  return bwd_meta_bytes(B) + tiles * bwd_span(p, ft) * (int64_t)sizeof(float);
+  return bwd_meta_bytes(B) + bwd_reduce_bytes(p, B) + tiles * bwd_span(p, ft) * (int64_t)sizeof(float);
 }
 
 // The refusal of a frame whose backward does not fit shared memory, with the numbers that decide it
@@ -1708,28 +1737,17 @@ std::string bwd_too_long(const BwdPlan &p) {
          std::to_string(BWD_SMEM_LIMIT) + " bytes (at 16 kHz, N = 8192 with frames up to about 0.4 s is the largest supported)";
 }
 
-}  // namespace
-
-extern "C" {
-
-int64_t b200feat_backward_work_bytes(b200feat_handle *h, const int64_t *num_samples, int32_t B) {
-  if (!h || !num_samples || B <= 0) return fail(h, B200FEAT_EINVAL, "backward_work_bytes: bad arguments");
-  BwdPlan p;
-  if (!bwd_plan(h, &p)) return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram and log-spectrogram kinds have one");
-  int warps, ft;
-  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, bwd_too_long(p));
-  return bwd_layout(h, p, ft, num_samples, B, nullptr);
-}
-
-int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples, const int64_t *offsets,
-                      int32_t B, const float *grad_out_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
-                      int64_t work_bytes, void *stream) {
-  if (!h) return fail(nullptr, B200FEAT_EINVAL, "backward: null handle");
+// b200feat_backward / b200feat_whisper_backward after their kind checks: the argument and per-cut checks, the tables, and
+// the launches (whisper-fbank: the per-cut reduction, then the frames and combine kernels of every kind)
+int run_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples, const int64_t *offsets,
+                 int32_t B, const float *grad_out_dev, const float *raw_dev, const float *cut_max_dev, const int64_t *row_off,
+                 float *grad_in_dev, void *work_dev, int64_t work_bytes, void *stream) {
   if (!samples_dev || !num_samples || !offsets || B <= 0 || !grad_out_dev || !row_off || !grad_in_dev || !work_dev)
     return fail(h, B200FEAT_EINVAL, "backward: bad arguments");
   if (dt != B200FEAT_F32) return fail(h, B200FEAT_EINVAL, "backward: float32 samples only");
   BwdPlan p;
-  if (!bwd_plan(h, &p)) return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram and log-spectrogram kinds have one");
+  if (!bwd_plan(h, &p, raw_dev != nullptr))
+    return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram, log-spectrogram and whisper-fbank kinds have one");
   int warps, ft;
   if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, bwd_too_long(p));
   std::vector<int64_t> tile_off;
@@ -1755,10 +1773,19 @@ int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, 
   CU_TRY(h, cudaMemcpyAsync(w, meta.data(), meta.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   const int64_t *dm = (const int64_t *)w;
   BwdBatch bb;
+  memset(&bb, 0, sizeof(bb));
   bb.samples = samples_dev; bb.grad_out = grad_out_dev; bb.grad_in = grad_in_dev;
   bb.samp_off = dm; bb.nsamp = dm + B; bb.row_off = dm + 2 * (int64_t)B; bb.tile_off = dm + 3 * (int64_t)B + 1;
-  bb.spans = (float *)(w + bwd_meta_bytes(B));
+  bb.spans = (float *)(w + bwd_meta_bytes(B) + bwd_reduce_bytes(p, B));
   bb.B = B; bb.ft = ft;
+  if (p.whisper) {
+    bb.xrows = raw_dev; bb.cut_max = cut_max_dev;
+    bb.routed = (float *)(w + bwd_meta_bytes(B));
+    bb.ties = (int *)(bb.routed + B);
+    const unsigned grid = (unsigned)std::min<int64_t>(B, (int64_t)h->sm_count * 8);
+    b200feat_whisper_backward_reduce_kernel<<<grid, BWD_REDUCE_THREADS, 0, st>>>(p, bb);
+    CU_TRY(h, cudaGetLastError());
+  }
   const int64_t ntiles = tile_off[B];
   if (ntiles > 0) {
     const size_t smem = bwd_smem(p, warps, ft);
@@ -1776,6 +1803,41 @@ int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, 
     CU_TRY(h, cudaGetLastError());
   }
   return B200FEAT_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t b200feat_backward_work_bytes(b200feat_handle *h, const int64_t *num_samples, int32_t B) {
+  if (!h || !num_samples || B <= 0) return fail(h, B200FEAT_EINVAL, "backward_work_bytes: bad arguments");
+  BwdPlan p;
+  if (!bwd_plan(h, &p, h->plan.whisper != 0))
+    return fail(h, B200FEAT_EINVAL, "backward: only the fbank, mfcc, spectrogram, log-spectrogram and whisper-fbank kinds have one");
+  int warps, ft;
+  if (!bwd_launch_shape(p, &warps, &ft)) return fail(h, B200FEAT_EUNSUPPORTED, bwd_too_long(p));
+  return bwd_layout(h, p, ft, num_samples, B, nullptr);
+}
+
+int b200feat_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples, const int64_t *offsets,
+                      int32_t B, const float *grad_out_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
+                      int64_t work_bytes, void *stream) {
+  if (!h) return fail(nullptr, B200FEAT_EINVAL, "backward: null handle");
+  if (h->plan.whisper)
+    return fail(h, B200FEAT_EINVAL, "backward: whisper-fbank's backward needs the forward's log-mel rows: use b200feat_whisper_backward");
+  return run_backward(h, samples_dev, dt, num_samples, offsets, B, grad_out_dev, nullptr, nullptr, row_off, grad_in_dev, work_dev,
+                      work_bytes, stream);
+}
+
+int b200feat_whisper_backward(b200feat_handle *h, const float *samples_dev, int32_t dt, const int64_t *num_samples,
+                              const int64_t *offsets, int32_t B, const float *grad_out_dev, const float *raw_dev,
+                              const float *cut_max_dev, const int64_t *row_off, float *grad_in_dev, void *work_dev,
+                              int64_t work_bytes, void *stream) {
+  if (!h) return fail(nullptr, B200FEAT_EINVAL, "whisper_backward: null handle");
+  if (!h->plan.whisper) return fail(h, B200FEAT_EINVAL, "whisper_backward: whisper-fbank handles only (b200feat_backward serves the others)");
+  if (!raw_dev || !cut_max_dev) return fail(h, B200FEAT_EINVAL, "whisper_backward: bad arguments");
+  return run_backward(h, samples_dev, dt, num_samples, offsets, B, grad_out_dev, raw_dev, cut_max_dev, row_off, grad_in_dev,
+                      work_dev, work_bytes, stream);
 }
 
 }  // extern "C"

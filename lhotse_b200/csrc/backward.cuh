@@ -18,8 +18,15 @@
 // for every sample, the spans of the tiles that cover it in tile order.  No atomics: the result is bitwise reproducible
 // and a cut's gradient does not depend on the other cuts of its batch.
 //
-// The per-frame and per-sample arithmetic is __host__ __device__, so that scripts/micro/backward_host_check.cu runs this
-// code on the CPU.  Kernels at the end.
+// whisper-fbank (DESIGN.md §3.1p) runs the same chain with three differences.  The row gradient comes from the saved
+// un-normalised log-mel rows x and the cut's maximum m: y = (maximum(x, m - 8) + 4) / 4 passes g / 4 to x above the
+// threshold, half of it on a tie, and the rest to m, which max() spreads evenly over the elements equal to m; a reduction
+// kernel sums that routed mass and counts the ties per cut before the frames kernel runs.  log10(clamp(v, 1e-10)) passes
+// g / (v ln 10) where v >= 1e-10 and nothing below.  The frames are torch.stft's centred frames over the stft's n / S rows
+// (the zero row gets no gradient), mirrored without repeating the edge sample.
+//
+// The per-frame and per-sample arithmetic is __host__ __device__, so that scripts/micro/backward_host_check.cu and
+// scripts/micro/whisper_backward_host_check.cu run this code on the CPU.  Kernels at the end.
 #pragma once
 #include <math.h>
 #include <stddef.h>
@@ -37,6 +44,7 @@
 #define BWD_MAX_TILE 16   // consecutive frames of one cut per CTA (fewer when a long frame does not fit)
 #define BWD_SMEM_LIMIT (200 * 1024)
 #define BWD_COMBINE_THREADS 256
+#define BWD_REDUCE_THREADS 256  // per-cut reduction of whisper-fbank: fixed, so that its summation order is fixed
 
 struct BwdC {  // same layout as float2
   float x, y;
@@ -48,6 +56,8 @@ struct BwdPlan {
   int pad, snip_edges, remove_dc, use_energy, raw_energy, use_mag, energy_style, use_lifter;
   int ecol;   // column of the log-energy (fbank / mfcc) when use_energy
   int shift;  // first mel column of an fbank row
+  int whisper;  // whisper-fbank: row gradient from the saved log-mel rows, log10 with its clamp, n / S frames
+  int reflect;  // mirror of the padded edges: 0 repeats the edge sample (Kaldi), 1 does not (torch's "reflect")
   float preemph, energy_floor_log, has_energy_floor, mel_floor, log_spec_eps, log_spec_floor;
   const float *window;     // [L]
   const BwdC *tws;         // [N/2 + 1] exp(-2 pi i k / N), even N
@@ -178,7 +188,7 @@ BWD_HD void bwd_bin_filters(const BwdPlan &p, int k, int *lo, int *hi) {
 
 // gradient reaching spectrum value k: the mel transpose over the filters [lo, hi), or the row's own column
 BWD_HD float bwd_gvalue(const BwdPlan &p, const float *g, const float *v, const float *gm, int lo, int hi, int k) {
-  if (p.feature == B200FEAT_FBANK || p.feature == B200FEAT_MFCC) {
+  if (p.feature == B200FEAT_FBANK || p.feature == B200FEAT_MFCC || p.whisper) {
     float acc = 0.f;
     for (int m = lo; m < hi; ++m) {
       const int i = k - p.mel_start[m];
@@ -248,6 +258,32 @@ BWD_HD float bwd_gd(const BwdPlan &p, const BwdC *out, const float *raw, float m
   return gd;
 }
 
+// ---- whisper-fbank -------------------------------------------------------------------------------------------------
+// frames of a cut of n samples the backward runs: the stft's n / S rows for whisper-fbank, else every row
+BWD_HD int64_t bwd_frames(const BwdPlan &p, int64_t n, int64_t rows) { return p.whisper ? n / p.S : rows; }
+
+// share of g / 4 that maximum(x, thr) passes to x: all above the threshold, half on a tie, none below (torch.maximum)
+BWD_HD float bwd_whisper_weight(float x, float thr) { return x > thr ? 1.f : (x == thr ? 0.5f : 0.f); }
+
+// what log-mel value x with row gradient g routes to the threshold m - 8, i.e. to the cut's maximum
+BWD_HD float bwd_whisper_routed(float g, float x, float m) { return 0.25f * g * (1.f - bwd_whisper_weight(x, m - 8.f)); }
+
+// gradient reaching log-mel value x: its own share of g / 4, plus the cut's routed mass over its `ties` maxima if x is one
+BWD_HD float bwd_whisper_glog(float g, float x, float m, float routed, int ties) {
+  float gx = 0.25f * g * bwd_whisper_weight(x, m - 8.f);
+  if (x == m) gx += routed / (float)ties;
+  return gx;
+}
+
+// d log10(clamp(v, min = floor)) / dv: torch.clamp passes the gradient where v >= floor, the tie included
+BWD_HD float bwd_dlog10_clamp(float v, float floor_) { return v >= floor_ ? 1.f / (v * 2.30258509299404568402f) : 0.f; }
+
+// gradient reaching mel energy m of a whisper-fbank row with gradient g and saved log-mel row x
+BWD_HD float bwd_whisper_gmel(const BwdPlan &p, const float *g, const float *x, int m, float mel, float cmax, float routed,
+                              int ties) {
+  return bwd_whisper_glog(g[m], x[m], cmax, routed, ties) * bwd_dlog10_clamp(mel, p.mel_floor);
+}
+
 // ---- overlap-add ---------------------------------------------------------------------------------------------------
 // position r of a tile's span: the sum, in frame order, of the gradients G[f][r - f S] of the tile's nf frames
 BWD_HD float bwd_span_value(const float *G, int ldg, int nf, int S, int L, int r) {
@@ -268,22 +304,26 @@ BWD_HD float bwd_position(const float *ws, int64_t ntiles, int64_t span, int64_t
 }
 
 // gradient of sample i of a cut of n samples and T frames: its own padded position, then its left and right mirror
-// images (layers.py:753-772 reflects once about either end, the edge sample repeated)
+// images.  layers.py:753-772 reflects once about either end, the edge sample repeated (reflect 0); torch.stft's "reflect"
+// padding does not repeat it (reflect 1), so the edge samples have no image there.
 BWD_HD float bwd_sample(const BwdPlan &p, const float *ws, int64_t ntiles, int ft, int64_t n, int64_t T, int64_t i) {
   const int64_t span = bwd_span(p, ft), stride = (int64_t)ft * p.S;
   const int64_t ext = (T - 1) * p.S + p.L, pad = p.snip_edges ? 0 : p.pad;
   float acc = 0.f;
   if (i + pad < ext) acc += bwd_position(ws, ntiles, span, stride, i + pad);
   if (!p.snip_edges) {
-    if (i < pad) acc += bwd_position(ws, ntiles, span, stride, pad - 1 - i);
-    const int64_t qr = 2 * n - 1 - i + pad;
-    if (qr < ext) acc += bwd_position(ws, ntiles, span, stride, qr);
+    const int64_t r = p.reflect;
+    if (i >= r && i < pad + r) acc += bwd_position(ws, ntiles, span, stride, pad - 1 - i + r);
+    const int64_t qr = 2 * n - 1 - r - i + pad;
+    if (i < n - r && qr < ext) acc += bwd_position(ws, ntiles, span, stride, qr);
   }
   return acc;
 }
 
-// the work buffer: int64 tables [samp_off B][nsamp B][row_off B + 1][tile_off B + 1], then the tiles' spans
+// the work buffer: int64 tables [samp_off B][nsamp B][row_off B + 1][tile_off B + 1], then (whisper-fbank) the per-cut
+// routed mass [B] and tie count [B], then the tiles' spans
 BWD_HD int64_t bwd_meta_bytes(int32_t B) { return ((4 * (int64_t)B + 2) * 8 + 255) / 256 * 256; }
+BWD_HD int64_t bwd_reduce_bytes(const BwdPlan &p, int32_t B) { return p.whisper ? (8 * (int64_t)B + 255) / 256 * 256 : 0; }
 
 #if defined(__CUDACC__)
 #include "generic.cuh"
@@ -295,6 +335,11 @@ struct BwdBatch {
   const int64_t *samp_off, *nsamp, *row_off, *tile_off;
   float *spans;
   int B, ft;
+  // whisper-fbank: the forward's un-normalised log-mel rows (laid out as grad_out) and per-cut maxima, and the reduction's
+  // per-cut routed mass and tie count
+  const float *xrows, *cut_max;
+  float *routed;
+  int *ties;
 };
 
 __device__ __forceinline__ int bwd_find(const int64_t *prefix, int B, int64_t g) {
@@ -324,7 +369,7 @@ __global__ void __launch_bounds__(BWD_MAX_WARPS * 32, 1) b200feat_backward_frame
   float *raw = reinterpret_cast<float *>(bufB + p.Nc);
   float *v = raw + bwd_round4(p.L);
   float *gm = v + bwd_round4(p.K);
-  const bool mel = p.feature == B200FEAT_FBANK || p.feature == B200FEAT_MFCC;
+  const bool mel = p.feature == B200FEAT_FBANK || p.feature == B200FEAT_MFCC || p.whisper;
   if (mel)
     for (int k = threadIdx.x; k < p.K; k += blockDim.x) bwd_bin_filters(p, k, flo + k, fhi + k);
   const int64_t span = bwd_span(p, b.ft);
@@ -333,9 +378,9 @@ __global__ void __launch_bounds__(BWD_MAX_WARPS * 32, 1) b200feat_backward_frame
     __syncthreads();  // the filter ranges are written; the previous tile's G has been read
     const int cut = bwd_find(b.tile_off, b.B, tile);
     const int64_t t0 = (tile - b.tile_off[cut]) * b.ft;
-    const int64_t T = b.row_off[cut + 1] - b.row_off[cut];
-    const int nf = (int)min((int64_t)b.ft, T - t0);
     const int64_t n = b.nsamp[cut];
+    const int64_t T = bwd_frames(p, n, b.row_off[cut + 1] - b.row_off[cut]);
+    const int nf = (int)min((int64_t)b.ft, T - t0);
     const float *x = b.samples + b.samp_off[cut];
     for (int f = warp; f < nf; f += nwarps) {
       const int64_t t = t0 + f;
@@ -344,7 +389,7 @@ __global__ void __launch_bounds__(BWD_MAX_WARPS * 32, 1) b200feat_backward_frame
       float s = 0.f;
       for (int j = lane; j < p.L; j += 32) {
         int64_t i = base + j;
-        if (!p.snip_edges) i = reflect_index(i, n, 0);
+        if (!p.snip_edges) i = reflect_index(i, n, p.reflect);
         const float r = __ldg(x + i);
         raw[j] = r;
         s += r;
@@ -379,7 +424,14 @@ __global__ void __launch_bounds__(BWD_MAX_WARPS * 32, 1) b200feat_backward_frame
       }
       __syncwarp();
       if (mel) {
-        for (int m = lane; m < p.M; m += 32) gm[m] = bwd_gmel(p, g, m, bwd_mel(p, v, m));
+        if (p.whisper) {
+          const float *xr = b.xrows + (b.row_off[cut] + t) * p.F;
+          const float cm = b.cut_max[cut], routed = b.routed[cut];
+          const int ties = b.ties[cut];
+          for (int m = lane; m < p.M; m += 32) gm[m] = bwd_whisper_gmel(p, g, xr, m, bwd_mel(p, v, m), cm, routed, ties);
+        } else {
+          for (int m = lane; m < p.M; m += 32) gm[m] = bwd_gmel(p, g, m, bwd_mel(p, v, m));
+        }
         __syncwarp();
       }
       for (int k = lane; k < p.K; k += 32) {
@@ -421,10 +473,45 @@ __global__ void __launch_bounds__(BWD_MAX_WARPS * 32, 1) b200feat_backward_frame
   }
 }
 
+// whisper-fbank, before the frames kernel: one CTA per cut sums what its stft rows route to the cut's maximum and counts
+// the elements equal to it.  Thread j takes elements j, j + 256, ... in order, then a fixed tree: the result depends on the
+// cut alone.
+__global__ void __launch_bounds__(BWD_REDUCE_THREADS) b200feat_whisper_backward_reduce_kernel(const BwdPlan p, const BwdBatch b) {
+  __shared__ float s_mass[BWD_REDUCE_THREADS];
+  __shared__ int s_ties[BWD_REDUCE_THREADS];
+  for (int cut = blockIdx.x; cut < b.B; cut += gridDim.x) {
+    const int64_t count = bwd_frames(p, b.nsamp[cut], 0) * p.F;
+    const float *g = b.grad_out + b.row_off[cut] * p.F, *x = b.xrows + b.row_off[cut] * p.F;
+    const float m = b.cut_max[cut];
+    float mass = 0.f;
+    int ties = 0;
+    for (int64_t e = threadIdx.x; e < count; e += BWD_REDUCE_THREADS) {
+      const float xv = x[e];
+      mass += bwd_whisper_routed(g[e], xv, m);
+      ties += xv == m;
+    }
+    s_mass[threadIdx.x] = mass;
+    s_ties[threadIdx.x] = ties;
+    __syncthreads();
+    for (int h = BWD_REDUCE_THREADS / 2; h > 0; h >>= 1) {
+      if (threadIdx.x < h) {
+        s_mass[threadIdx.x] += s_mass[threadIdx.x + h];
+        s_ties[threadIdx.x] += s_ties[threadIdx.x + h];
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+      b.routed[cut] = s_mass[0];
+      b.ties[cut] = s_ties[0];
+    }
+    __syncthreads();  // the next cut reuses the shared arrays
+  }
+}
+
 // One thread per sample: the tiles' spans summed back into the cut's samples.
 __global__ void __launch_bounds__(BWD_COMBINE_THREADS) b200feat_backward_combine_kernel(const BwdPlan p, const BwdBatch b) {
   for (int cut = blockIdx.y; cut < b.B; cut += gridDim.y) {
-    const int64_t n = b.nsamp[cut], T = b.row_off[cut + 1] - b.row_off[cut];
+    const int64_t n = b.nsamp[cut], T = bwd_frames(p, n, b.row_off[cut + 1] - b.row_off[cut]);
     const int64_t t0 = b.tile_off[cut], ntiles = b.tile_off[cut + 1] - t0;
     const float *ws = b.spans + t0 * bwd_span(p, b.ft);
     float *gx = b.grad_in + b.samp_off[cut];

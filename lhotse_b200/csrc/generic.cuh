@@ -260,8 +260,11 @@ __global__ void __launch_bounds__(256) b200feat_generic_kernel(const DevPlan p, 
 
 // Second launch of the whisper-fbank path (whisper_fbank.py:68-80): x -> (max(x, cut_max - 8) + 4) / 4 for the rows the
 // stft produced (t < n / S), 0 for the extra row `compute_num_frames_from_samples` asks for; padded rows keep pad_value.
+// The log-mel rows x are read from `src` and the result written to b.out at the same offsets: src is b.out itself, or the
+// rows the fused kernel wrote elsewhere when the caller keeps them (b200feat_extract_keep_raw, for the backward).
 // One warp per output row; reads and writes 4*F bytes per row.
-__global__ void __launch_bounds__(256) b200feat_whisper_normalize_kernel(const DevPlan p, const DevBatch b, int64_t nrows) {
+__global__ void __launch_bounds__(256) b200feat_whisper_normalize_kernel(const DevPlan p, const DevBatch b, const float *src,
+                                                                         int64_t nrows) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -280,11 +283,12 @@ __global__ void __launch_bounds__(256) b200feat_whisper_normalize_kernel(const D
       t = out_row - __ldg(b.row_off + cut);
     }
     float *o = b.out + out_row * p.F;
+    const float *x = src + out_row * p.F;
     if (t >= __ldg(b.nsamp + cut) / p.S) {
       for (int c = lane; c < p.F; c += 32) o[c] = 0.f;
     } else {
       const float thr = b.cut_max[cut] - 8.0f;
-      for (int c = lane; c < p.F; c += 32) o[c] = (nanmax(o[c], thr) + 4.0f) * 0.25f;
+      for (int c = lane; c < p.F; c += 32) o[c] = (nanmax(x[c], thr) + 4.0f) * 0.25f;
     }
   }
 }
@@ -293,7 +297,8 @@ __global__ void __launch_bounds__(256) b200feat_whisper_normalize_kernel(const D
 // The same pass for the tiled kernels (fast400): one CTA per tile of `ft` consecutive rows of one cut, located through the
 // host-built tile -> cut table exactly as the fused kernel does (no per-row search), rows processed as one contiguous run of
 // 128-bit accesses.
-__global__ void __launch_bounds__(256) b200feat_whisper_normalize_tiled_kernel(const DevPlan p, const DevBatch b, int ft) {
+__global__ void __launch_bounds__(256) b200feat_whisper_normalize_tiled_kernel(const DevPlan p, const DevBatch b, const float *src,
+                                                                               int ft) {
   for (int64_t tg = blockIdx.x; tg < b.num_tiles; tg += gridDim.x) {
     const int64_t tile = b.tile_base + tg;
     const int cut = __ldg(b.tile_cut + tile) - b.batch_first;
@@ -307,10 +312,12 @@ __global__ void __launch_bounds__(256) b200feat_whisper_normalize_tiled_kernel(c
     const int live = (int)max((int64_t)0, min(rows, __ldg(b.nsamp + cut) / p.S - t0)) * p.F;  // floats of stft rows
     const float thr = b.cut_max[cut] - 8.0f;
     float *o = b.out + row0 * p.F;
+    const float *x = src + row0 * p.F;
     if (((row0 * p.F) & 3) == 0 && (p.F & 3) == 0) {
       float4 *o4 = reinterpret_cast<float4 *>(o);
+      const float4 *x4 = reinterpret_cast<const float4 *>(x);
       for (int i = threadIdx.x; 4 * i < total; i += blockDim.x) {
-        float4 v = o4[i];
+        float4 v = x4[i];
         const bool on = 4 * i < live;  // F is a multiple of 4: a float4 never straddles the live / zero boundary
         v.x = on ? (nanmax(v.x, thr) + 4.0f) * 0.25f : 0.f;
         v.y = on ? (nanmax(v.y, thr) + 4.0f) * 0.25f : 0.f;
@@ -319,7 +326,7 @@ __global__ void __launch_bounds__(256) b200feat_whisper_normalize_tiled_kernel(c
         o4[i] = v;
       }
     } else {
-      for (int i = threadIdx.x; i < total; i += blockDim.x) o[i] = i < live ? (nanmax(o[i], thr) + 4.0f) * 0.25f : 0.f;
+      for (int i = threadIdx.x; i < total; i += blockDim.x) o[i] = i < live ? (nanmax(x[i], thr) + 4.0f) * 0.25f : 0.f;
     }
   }
 }

@@ -131,7 +131,7 @@ EXPORTS = [
     "b200feat_reverb_work_bytes", "b200feat_reverb", "b200feat_specaug_work_bytes", "b200feat_specaug",
     "b200feat_reverb_ex", "b200feat_rir_generate_work_bytes", "b200feat_rir_generate",
     "b200feat_feature_mix_work_bytes", "b200feat_feature_mix", "b200feat_backward_work_bytes", "b200feat_backward",
-    "b200feat_collate_audio_work_bytes", "b200feat_collate_audio",
+    "b200feat_collate_audio_work_bytes", "b200feat_collate_audio", "b200feat_extract_keep_raw", "b200feat_whisper_backward",
 ]
 
 
@@ -229,6 +229,10 @@ def load_library():
         lib.b200feat_backward_work_bytes.argtypes = [vp, vp, i32]
         lib.b200feat_backward.restype = C.c_int
         lib.b200feat_backward.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, vp, i64, vp]
+        lib.b200feat_extract_keep_raw.restype = C.c_int
+        lib.b200feat_extract_keep_raw.argtypes = [vp, vp, i32, vp, i32, C.POINTER(BatchTotals), vp, vp, vp]
+        lib.b200feat_whisper_backward.restype = C.c_int
+        lib.b200feat_whisper_backward.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp, i64, vp]
         lib.b200feat_collate_audio_work_bytes.restype = i64
         lib.b200feat_collate_audio_work_bytes.argtypes = [i32]
         lib.b200feat_collate_audio.restype = C.c_int
@@ -603,6 +607,51 @@ class Engine:
         stream = torch.cuda.current_stream(samples.device).cuda_stream
         self._check_cuts(self.lib.b200feat_backward(self._h, samples.data_ptr(), DT_F32, _ptr(ns), _ptr(off), B, g.data_ptr(),
                                                     _ptr(rows), grad_in.data_ptr(), work.data_ptr(), work.numel(), stream))
+        return grad_in
+
+    def extract_device_keep_raw(self, samples: torch.Tensor, num_samples: Sequence[int], offsets: Sequence[int]
+                                ) -> Tuple[torch.Tensor, torch.Tensor, np.ndarray]:
+        """`extract_device` (packed) for a whisper-fbank engine that also keeps what `whisper_backward_device` needs:
+        (features (sum R_i, F), raw, row prefix), `raw` a flat float32 tensor holding the forward's (sum R_i, F) log-mel rows
+        before the clamp and normalisation, then the B per-cut maxima.  The features are bitwise those of `extract_device`."""
+        assert samples.is_cuda and samples.dim() == 1 and samples.is_contiguous()
+        if samples.data_ptr() % 16:
+            samples = samples.clone()
+        dt = {torch.float32: DT_F32, torch.int16: DT_I16}[samples.dtype]
+        B = len(num_samples)
+        meta, totals = self.plan_batch(num_samples, offsets)
+        assert totals.span_samples <= samples.numel(), "sample buffer shorter than offsets + lengths"
+        meta_dev = torch.from_numpy(meta).to(samples.device, non_blocking=False)
+        rows = int(totals.total_rows)
+        out = torch.empty((rows, self.feature_dim), dtype=torch.float32, device=samples.device)
+        raw = torch.empty(int(totals.out_floats), dtype=torch.float32, device=samples.device)
+        stream = torch.cuda.current_stream(samples.device).cuda_stream
+        self._check(self.lib.b200feat_extract_keep_raw(self._h, samples.data_ptr(), dt, meta_dev.data_ptr(), B, C.byref(totals),
+                                                       out.data_ptr(), raw.data_ptr(), stream))
+        return out, raw, meta[2 * B: 3 * B + 1]
+
+    def whisper_backward_device(self, samples: torch.Tensor, num_samples: Sequence[int], offsets: Sequence[int],
+                                grad_out: torch.Tensor, raw: torch.Tensor, row_prefix: Sequence[int]) -> torch.Tensor:
+        """`backward_device` for a whisper-fbank engine: `raw` is the tensor `extract_device_keep_raw` returned for the same
+        samples, whose features the loss's gradient `grad_out` ((sum R_i, F)) is taken with respect to."""
+        assert samples.is_cuda and samples.dim() == 1 and samples.is_contiguous() and samples.dtype == torch.float32
+        B = len(num_samples)
+        ns = np.ascontiguousarray(num_samples, dtype=np.int64)
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        rows = np.ascontiguousarray(row_prefix, dtype=np.int64)
+        R = int(rows[-1])
+        g = grad_out.to(device=samples.device, dtype=torch.float32).contiguous()
+        assert g.shape == (R, self.feature_dim), (tuple(g.shape), R, self.feature_dim)
+        assert raw.is_cuda and raw.dtype == torch.float32 and raw.numel() == R * self.feature_dim + B
+        nbytes = int(self.lib.b200feat_backward_work_bytes(self._h, _ptr(ns), B))
+        if nbytes < 0:
+            self._check_cuts(nbytes)
+        work = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=samples.device)
+        grad_in = torch.zeros_like(samples)
+        stream = torch.cuda.current_stream(samples.device).cuda_stream
+        self._check_cuts(self.lib.b200feat_whisper_backward(
+            self._h, samples.data_ptr(), DT_F32, _ptr(ns), _ptr(off), B, g.data_ptr(), raw.data_ptr(),
+            raw.data_ptr() + 4 * R * self.feature_dim, _ptr(rows), grad_in.data_ptr(), work.data_ptr(), work.numel(), stream))
         return grad_in
 
     # ------------------------------------------------------------------ host-to-host path

@@ -23,7 +23,10 @@ Deliberate differences, all documented in DESIGN.md:
   * ``device`` must be a CUDA device; there is no CPU fallback.
   * A float tensor input that requires grad (with grad mode on) gives features with a graph back to it, as the reference's
     ``nn.Module`` chain does, for the Fbank / Mfcc / Spectrogram / LogSpectrogram classes through ``extract`` and
-    ``extract_batch``: the gradient is the sm_90a backward kernel's (csrc/backward.cuh, DESIGN.md §3.1n).
+    ``extract_batch``: the gradient is the sm_90a backward kernel's (csrc/backward.cuh, DESIGN.md §3.1n).  WhisperFbank
+    too, as the reference's torch-only ``log_mel_spectrogram`` is: its forward keeps its log-mel rows and per-cut maxima
+    for the backward (DESIGN.md §3.1p).  LibrosaFbank and the torchaudio and kaldifeat families stay detached, as the
+    reference's NumPy and C++ paths are.
 """
 from __future__ import annotations
 
@@ -187,7 +190,7 @@ def _to_float32(x: ArrayLike) -> ArrayLike:
     return x.astype(np.float32) * np.float32(1.0 / 32768.0) if x.dtype == np.int16 else x.astype(np.float32, copy=False)
 
 
-_GRAD_KINDS = ("fbank", "mfcc", "spectrogram", "log-spectrogram")
+_GRAD_KINDS = ("fbank", "mfcc", "spectrogram", "log-spectrogram", "whisper-fbank")
 
 
 class _KaldiFeatures(torch.autograd.Function):
@@ -196,7 +199,8 @@ class _KaldiFeatures(torch.autograd.Function):
     each and are packed here.  The (dithered) packed device buffer is saved; the backward recomputes everything else."""
 
     @staticmethod
-    def forward(ctx, ext, eng, lens, offs, info, *items):
+    def _pack(ctx, ext, eng, lens, offs, items):
+        """The cuts as one aligned float32 device buffer: (buffer, lens, offs); records the items' shapes in `ctx`."""
         if len(items) == 1:
             buf = items[0].detach().reshape(-1).to(eng.device, non_blocking=True)
         else:
@@ -204,26 +208,58 @@ class _KaldiFeatures(torch.autograd.Function):
         buf = ext._dithered(buf).contiguous()
         if buf.data_ptr() % 16:
             buf = buf.clone()  # extract_device would copy an unaligned view; the backward must read the same buffer
-        out, prefix = eng.extract_device(buf, list(lens), offsets=list(offs))
-        info["prefix"] = prefix
-        ctx.eng, ctx.lens, ctx.offs, ctx.prefix = eng, list(lens), list(offs), prefix
+        ctx.eng, ctx.lens, ctx.offs = eng, list(lens), list(offs)
         ctx.items = [(x.shape, x.device, x.numel()) for x in items]
-        ctx.save_for_backward(buf)
-        return out
+        return buf
 
     @staticmethod
-    def backward(ctx, grad_out):
-        if torch.is_grad_enabled():
-            raise RuntimeError("the b200 extractors' backward is not differentiable: double backward (create_graph=True) is "
-                               "not supported")
-        (buf,) = ctx.saved_tensors
-        g = ctx.eng.backward_device(buf, ctx.lens, ctx.offs, grad_out, ctx.prefix)
+    def _unpack(ctx, g):
+        """The gradient of the packed buffer cut back into the items' shapes and devices (autograd casts to their dtypes)."""
         if len(ctx.items) == 1:
             shape, dev, numel = ctx.items[0]
             grads = [g[:numel].view(shape).to(dev)]
         else:
             grads = [g[o:o + numel].view(shape).to(dev) for o, (shape, dev, numel) in zip(ctx.offs, ctx.items)]
         return (None, None, None, None, None, *grads)
+
+    @staticmethod
+    def forward(ctx, ext, eng, lens, offs, info, *items):
+        buf = _KaldiFeatures._pack(ctx, ext, eng, lens, offs, items)
+        out, prefix = eng.extract_device(buf, ctx.lens, offsets=ctx.offs)
+        info["prefix"] = ctx.prefix = prefix
+        ctx.save_for_backward(buf)
+        return out
+
+    @staticmethod
+    def _refuse_double_backward():
+        if torch.is_grad_enabled():
+            raise RuntimeError("the b200 extractors' backward is not differentiable: double backward (create_graph=True) is "
+                               "not supported")
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        _KaldiFeatures._refuse_double_backward()
+        (buf,) = ctx.saved_tensors
+        return _KaldiFeatures._unpack(ctx, ctx.eng.backward_device(buf, ctx.lens, ctx.offs, grad_out, ctx.prefix))
+
+
+class _WhisperFeatures(torch.autograd.Function):
+    """`_KaldiFeatures` for whisper-fbank: the forward also keeps its own log-mel rows and per-cut maxima (the clamp to the
+    cut's maximum - 8 is a cut-wide decision that a recomputation cannot repeat bit for bit), and the backward reads them."""
+
+    @staticmethod
+    def forward(ctx, ext, eng, lens, offs, info, *items):
+        buf = _KaldiFeatures._pack(ctx, ext, eng, lens, offs, items)
+        out, raw, prefix = eng.extract_device_keep_raw(buf, ctx.lens, ctx.offs)
+        info["prefix"] = ctx.prefix = prefix
+        ctx.save_for_backward(buf, raw)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        _KaldiFeatures._refuse_double_backward()
+        buf, raw = ctx.saved_tensors
+        return _KaldiFeatures._unpack(ctx, ctx.eng.whisper_backward_device(buf, ctx.lens, ctx.offs, grad_out, raw, ctx.prefix))
 
 
 class _B200Extractor(FeatureExtractor):
@@ -309,7 +345,8 @@ class _B200Extractor(FeatureExtractor):
     def _extract_grad(self, items: Sequence[torch.Tensor], lens: Sequence[int], offsets: Sequence[int]):
         """`_extract_on_device` / `_extract_list_on_device` with a graph: (features, row prefix)."""
         info = {}
-        out = _KaldiFeatures.apply(self, self.engine, list(lens), list(offsets), info, *items)
+        fn = _WhisperFeatures if self.feature_kind == "whisper-fbank" else _KaldiFeatures
+        out = fn.apply(self, self.engine, list(lens), list(offsets), info, *items)
         return out, info["prefix"]
 
     def extract(self, samples: ArrayLike, sampling_rate: int) -> ArrayLike:
