@@ -15,53 +15,16 @@ pytestmark = pytest.mark.gpu
 LENS = (201, 16000, 16079, 16080, 48159)
 
 
-def _ext(kernel="auto", M=80):
-    import lhotse_b200 as lb
-
-    return lb.B200WhisperFbank(lb.B200WhisperFbankConfig(num_filters=M, kernel=kernel))
-
-
-def _loss(feats, G):
-    return (feats * torch.as_tensor(G, dtype=feats.dtype, device=feats.device)).sum()
-
-
-def _grad(ext, x, G, dtype=torch.float32, device="cuda"):
-    xt = torch.tensor(np.asarray(x), dtype=dtype, device=device, requires_grad=True)
-    _loss(ext.extract(xt, 16000), G).backward()
-    return xt.grad.double().cpu().numpy()
-
-
-def _case(n, kind, M, seed=0):
-    """A waveform and a row gradient whose decisions agree across precisions: G is 0 on values within 1e-3 of m - 8 or of
-    the floor's log (-10), and the cut's maximum is unique by 1e-3 (asserted)."""
-    x = WB.waveform(n, kind, seed).astype(np.float32).astype(np.float64)
-    xr = WB.logmel_t(torch.tensor(x), M).numpy()
-    m = xr.max()
-    top = np.sort(xr.ravel())[-2:] if xr.size > 1 else np.asarray([-np.inf, m])
-    assert top[1] - top[0] > 1e-3, (n, kind, M)
-    G = np.random.RandomState(n + M + seed).randn(W.num_rows(n), M)
-    near = (np.abs(xr - (m - 8.0)) < 1e-3) | (np.abs(xr + 10.0) < 1e-3)
-    G[: xr.shape[0]][near] = 0.0
-    return x, G
-
-
-def _gate(x, G, M, g):
-    g64 = WB.autograd_grad(x, G, M)
-    g32 = WB.autograd_grad(x, G, M, dtype=torch.float32, device="cuda")
-    err, err32 = float(np.linalg.norm(g - g64)), float(np.linalg.norm(g32 - g64))
-    return err, 8.0 * err32 + 1e-7 * float(np.linalg.norm(g64)), err32
-
-
 @pytest.mark.parametrize("M", [80, 128])
 @pytest.mark.parametrize("kernel", ["auto", "generic"])
 def test_gpu_accuracy_per_cut(kernel, M):
-    ext = _ext(kernel, M)
+    ext = WB.extractor(kernel, M)
     worst = 0.0
     for kind in ("noise", "burst"):
         for n in LENS:
-            x, G = _case(n, kind, M)
-            g = _grad(ext, x, G)
-            err, bound, err32 = _gate(x, G, M, g)
+            x, G = WB.case(n, kind, M)
+            g = WB.b200_grad(ext, x, G)
+            err, bound, err32 = WB.gate(x, G, M, g)
             assert err <= bound, (kernel, M, kind, n, err, bound)
             worst = max(worst, err / max(err32, 1e-300))
     print(f"whisper backward {kernel} M={M}: worst ratio to the float32 chain's error {worst:.2f}")
@@ -71,7 +34,7 @@ def test_gpu_accuracy_per_cut(kernel, M):
 def test_gpu_tied_maximum_against_the_saved_rows(kernel):
     """A hop-periodic waveform ties its maximum across interior frames: the routed mass is split evenly over the ties the
     forward itself saw, so the reference is the restatement fed the forward's own rows and maximum."""
-    ext = _ext(kernel)
+    ext = WB.extractor(kernel)
     for n in (16000, 16080, 32080):
         x = WB.waveform(n, "periodic").astype(np.float32).astype(np.float64)
         xt = torch.tensor(x, dtype=torch.float32, device="cuda")
@@ -82,71 +45,71 @@ def test_gpu_tied_maximum_against_the_saved_rows(kernel):
         m = float(raw[R * 80].item())
         assert (xr == m).sum() > 10 and (xr < m - 8.0).any()  # ties and a binding clamp
         G = np.random.RandomState(n).randn(R, 80)
-        g = _grad(ext, x, G)
+        g = WB.b200_grad(ext, x, G)
         want = WB.restated_grad(x, G, 80, xr=xr, m=m)
         assert WB.rel_err(g, want) < 2e-3, (kernel, n, WB.rel_err(g, want))
 
 
 def test_gpu_exact_properties():
-    ext = _ext()
+    ext = WB.extractor()
     n = 48159
     G = np.random.RandomState(1).randn(W.num_rows(n), 80)
-    assert not _grad(ext, np.zeros(n), G).any()  # silence: every mel energy is clamped
+    assert not WB.b200_grad(ext, np.zeros(n), G).any()  # silence: every mel energy is clamped
     # a loud first second, then a tail 100 dB down whose log-mel values all sit below m - 8: the samples only the tail's
     # frames cover get exactly 0
     rs = np.random.RandomState(2)
     x = 1e-5 * rs.randn(n)
     x[:16000] = rs.randn(16000)
-    g = _grad(ext, x, G)
+    g = WB.b200_grad(ext, x, G)
     assert g[:15000].any() and not g[160 * 101 + 200:].any()  # frame 101 is the last to reach a loud sample
     # the zero row's gradient does not matter, two runs agree, and so does a cut batched with others
     x = WB.waveform(16080, "burst")
     G = np.random.RandomState(3).randn(W.num_rows(16080), 80)
-    g1 = _grad(ext, x, G)
+    g1 = WB.b200_grad(ext, x, G)
     G2 = G.copy()
     G2[-1] = 1e6
-    assert np.array_equal(_grad(ext, x, G2), g1)
-    assert np.array_equal(_grad(ext, x, G), g1)
+    assert np.array_equal(WB.b200_grad(ext, x, G2), g1)
+    assert np.array_equal(WB.b200_grad(ext, x, G), g1)
     others = [WB.waveform(n, "noise", 5) for n in (4000, 16080, 31999)]
     items = [torch.tensor(a, dtype=torch.float32, device="cuda", requires_grad=True) for a in others[:1] + [x] + others[1:]]
     feats = ext.extract_batch(items, 16000)
-    total = sum(_loss(f, np.random.RandomState(i).randn(*f.shape)) for i, f in enumerate(feats) if i != 1) + _loss(feats[1], G)
+    total = sum(WB.loss(f, np.random.RandomState(i).randn(*f.shape)) for i, f in enumerate(feats) if i != 1) + WB.loss(feats[1], G)
     total.backward()
     assert np.array_equal(items[1].grad.double().cpu().numpy(), g1)
 
 
 def test_gpu_lengths_and_padded_rows():
-    ext = _ext()
+    ext = WB.extractor()
     B, n = 3, 32000
     lengths = [32000, 16080, 20001]
     x = torch.tensor(np.stack([WB.waveform(n, "noise", i) for i in range(B)]), dtype=torch.float32, device="cuda",
                      requires_grad=True)
     feats = ext.extract_batch(x, 16000, lengths=lengths)
     Gs = [np.random.RandomState(i).randn(*f.shape) for i, f in enumerate(feats)]
-    sum(_loss(f, g) for f, g in zip(feats, Gs)).backward()
+    sum(WB.loss(f, g) for f, g in zip(feats, Gs)).backward()
     gx = x.grad.double().cpu().numpy()
     for i, L in enumerate(lengths):
         assert not gx[i, L:].any()
-        alone = _grad(ext, x.detach()[i, :L].double().cpu().numpy(), Gs[i])
+        alone = WB.b200_grad(ext, x.detach()[i, :L].double().cpu().numpy(), Gs[i])
         assert np.array_equal(gx[i, :L], alone), i
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
 @pytest.mark.parametrize("device", ["cpu", "cuda"])
 def test_gpu_containers(device, dtype):
-    ext = _ext()
+    ext = WB.extractor()
     xs = [WB.waveform(n, "noise", 7) for n in (16000, 16080)]
     G = [np.random.RandomState(i).randn(W.num_rows(len(a)), 80) for i, a in enumerate(xs)]
-    want = [_grad(ext, a, g) for a, g in zip(xs, G)]
+    want = [WB.b200_grad(ext, a, g) for a, g in zip(xs, G)]
     # extract on one tensor
     t = torch.tensor(xs[0], dtype=dtype, device=device, requires_grad=True)
-    _loss(ext.extract(t, 16000), G[0]).backward()
+    WB.loss(ext.extract(t, 16000), G[0]).backward()
     assert t.grad.dtype == dtype and t.grad.device == t.device
     assert np.allclose(t.grad.double().cpu().numpy(), want[0], rtol=0, atol=1e-6 * np.abs(want[0]).max())
     # extract_batch on a list
     ts = [torch.tensor(a, dtype=dtype, device=device, requires_grad=True) for a in xs]
     out = ext.extract_batch(ts, 16000)
-    sum(_loss(o, g) for o, g in zip(out, G)).backward()
+    sum(WB.loss(o, g) for o, g in zip(out, G)).backward()
     for tt, w in zip(ts, want):
         assert tt.grad.dtype == dtype and tt.grad.device == tt.device
         assert np.allclose(tt.grad.double().cpu().numpy(), w, rtol=0, atol=1e-6 * np.abs(w).max())
@@ -154,13 +117,13 @@ def test_gpu_containers(device, dtype):
     b = torch.tensor(np.stack([xs[0], xs[0][::-1].copy()]), dtype=dtype, device=device, requires_grad=True)
     out = ext.extract_batch(b, 16000)
     assert out.shape == (2, 100, 80) and out.requires_grad
-    _loss(out[0], G[0]).backward()
+    WB.loss(out[0], G[0]).backward()
     assert b.grad.dtype == dtype and b.grad.device == b.device and not b.grad[1].any()
     assert np.allclose(b.grad[0].double().cpu().numpy(), want[0], rtol=0, atol=1e-6 * np.abs(want[0]).max())
 
 
 def test_gpu_no_grad_path_untouched():
-    ext = _ext()
+    ext = WB.extractor()
     x = torch.tensor(WB.waveform(48159, "burst"), dtype=torch.float32, device="cuda")
     before = ext.engine.stats()["kernel_launches"]
     ref = ext.extract(x, 16000)
@@ -178,11 +141,11 @@ def test_gpu_no_grad_path_untouched():
 
 
 def test_gpu_failure_modes():
-    ext = _ext()
+    ext = WB.extractor()
     xg = torch.tensor(WB.waveform(16000, "noise"), dtype=torch.float32, device="cuda", requires_grad=True)
     og = ext.extract(xg, 16000)
     with pytest.raises(RuntimeError):
-        torch.autograd.grad(_loss(og, np.ones(og.shape)), xg, create_graph=True)
+        torch.autograd.grad(WB.loss(og, np.ones(og.shape)), xg, create_graph=True)
     with pytest.raises(ValueError):
         ext.extract(torch.zeros(200, device="cuda", requires_grad=True), 16000)
     with pytest.raises(NotImplementedError):
@@ -192,7 +155,7 @@ def test_gpu_failure_modes():
 def test_gpu_abi_refusals():
     from lhotse_b200 import engine
 
-    eng = _ext().engine
+    eng = WB.extractor().engine
     lib = eng.lib
     x = torch.zeros(32000, device="cuda")
     g = torch.zeros(200 * 80, device="cuda")
@@ -235,7 +198,7 @@ def test_gpu_conv1d_ahead_of_the_extractor_matches_lhotse():
     def weight_grad(front, conv, dtype, device):
         conv = conv.to(device=device, dtype=dtype)
         y = conv(x.to(device=device, dtype=dtype).view(1, 1, -1)).view(-1)
-        _loss(front(y), G).backward()
+        WB.loss(front(y), G).backward()
         return conv.weight.grad.double().cpu().numpy().ravel()
 
     torch.manual_seed(0)
@@ -249,7 +212,7 @@ def test_gpu_conv1d_ahead_of_the_extractor_matches_lhotse():
     ref64 = WhisperFbank(WhisperFbankConfig())
     ref64.filters, ref64.window = ref64.filters.double(), ref64.window.double()
     ref32 = WhisperFbank(WhisperFbankConfig(device="cuda"))
-    b200 = _ext()
+    b200 = WB.extractor()
     w64 = weight_grad(lambda y: ref64.extract(y, 16000), convs[0], torch.float64, "cpu")
     w32 = weight_grad(lambda y: ref32.extract(y, 16000), convs[1], torch.float32, "cuda")
     wb = weight_grad(lambda y: b200.extract(y, 16000), convs[2], torch.float32, "cuda")

@@ -8,6 +8,7 @@ import torch
 
 import refshim
 import whisper_backward_cases as WB
+import whisper_backward_edge_cases as E
 from oracle import whisper_oracle as W
 
 KINDS = ("noise", "burst", "periodic", "silence")
@@ -23,9 +24,25 @@ def test_twin_is_the_oracle_bit_for_bit(n, dtype):
         assert got.dtype == want.dtype and np.array_equal(got, want), (n, M, dtype)
 
 
-@pytest.mark.parametrize("M", [80, 128])
-@pytest.mark.parametrize("kind", KINDS)
-@pytest.mark.parametrize("n", WB.LENGTHS)
+def _with_edges(base, ident):
+    """`base` cases (n, kind, M), then those of every row of the edge table (whisper_backward_edge_cases.TABLE) not among
+    them, as pytest params with ids `ident(n, kind, M, is_edge_row)`.  The hop-periodic tone runs at M = 80 and 128 only:
+    its interior frames hold whole periods, so the filters between its harmonics see rounding-level leakage, and at other
+    filter counts some of it lands just above the 1e-10 floor, where the log's 1 / v turns rounding into gradient."""
+    seen = set(base)
+    cases = [pytest.param(*c, id=ident(*c, False)) for c in base]
+    for r in E.TABLE:
+        for kind in KINDS:
+            if kind == "periodic" and r.M not in (80, 128):
+                continue
+            if (r.n, kind, r.M) not in seen:
+                seen.add((r.n, kind, r.M))
+                cases.append(pytest.param(r.n, kind, r.M, id=ident(r.n, kind, r.M, True)))
+    return cases
+
+
+@pytest.mark.parametrize("n,kind,M", _with_edges([(n, kind, M) for n in WB.LENGTHS for kind in KINDS for M in (80, 128)],
+                                                 lambda n, kind, M, edge: f"{n}-{kind}-{M}"))
 def test_restatement_matches_float64_autograd(n, kind, M):
     x = WB.waveform(n, kind)
     G = np.random.RandomState(n + M).randn(W.num_rows(n), M)
@@ -112,16 +129,16 @@ def harness(tmp_path_factory):
     return exe
 
 
-@pytest.mark.parametrize("kind", ("noise", "burst", "periodic", "silence"))
-@pytest.mark.parametrize("n", (201, 16000, 16079, 16080, 16159))
-def test_host_harness_matches_restatement(n, kind, harness, tmp_path):
+@pytest.mark.parametrize("n,kind,M", _with_edges([(n, kind, 80) for n in (201, 16000, 16079, 16080, 16159) for kind in KINDS],
+                                                 lambda n, kind, M, edge: f"{n}-{kind}" + (f"-M{M}" if edge else "")))
+def test_host_harness_matches_restatement(n, kind, M, harness, tmp_path):
     """The header's per-cut, per-frame and per-sample code in float32 on the CPU, with every buffer at its exact size,
     against the restatement taking its decisions on the same saved rows."""
     x = WB.waveform(n, kind).astype(np.float32).astype(np.float64)
-    xr, m = WB.saved_rows(x)
-    G = np.random.RandomState(n).randn(W.num_rows(n), 80).astype(np.float32)
-    got = WB.run_host_check(harness, tmp_path, x, xr, m, G)
-    want = WB.restated_grad(x, G.astype(np.float64), 80, xr=xr.astype(np.float64), m=m)
+    xr, m = WB.saved_rows(x, M)
+    G = np.random.RandomState(n).randn(W.num_rows(n), M).astype(np.float32)
+    got = WB.run_host_check(harness, tmp_path, x, xr, m, G, M)
+    want = WB.restated_grad(x, G.astype(np.float64), M, xr=xr.astype(np.float64), m=m)
     assert got.shape == want.shape
     if kind == "silence":
         assert not got.any()
@@ -130,17 +147,29 @@ def test_host_harness_matches_restatement(n, kind, harness, tmp_path):
 
 
 def test_host_harness_folds_the_centre_mirror(harness, tmp_path):
-    """Rows of gradient on the first and last frames only: every sample those frames reach through torch's mirror gets its
-    share, the edge samples no mirror image, and the restatement's fold agrees."""
-    n = 1000
-    x = WB.waveform(n, "noise").astype(np.float32).astype(np.float64)
-    xr, m = WB.saved_rows(x)
-    G = np.zeros((W.num_rows(n), 80), dtype=np.float32)
-    G[0], G[n // 160 - 1] = 1.0, -1.0
-    got = WB.run_host_check(harness, tmp_path, x, xr, m, G)
-    want = WB.restated_grad(x, G.astype(np.float64), 80, xr=xr.astype(np.float64), m=m)
-    assert WB.rel_err(got, want) < 2e-4
-    assert not got[360:560].any()  # covered by neither edge frame (frame 0 ends at 199, the last starts at 760 - 200)
+    """Rows of gradient on the first and last frames only, at lengths whose last frame reaches 40, 39, 2, 1 and 0 positions
+    past the cut (n mod 160 = 0, 1, 38, 39, 40): every sample those frames reach through torch's mirror gets its share,
+    samples 0 and n - 1 no mirror image, nothing between the two frames, and the header's fold agrees with the
+    restatement's sample by sample at both ends."""
+    for n, reach in ((960, 40), (961, 39), (998, 2), (999, 1), (1000, 0)):
+        T = n // 160
+        assert E.right_reach(n) == reach
+        raw = np.arange(T)[:, None] * 160 - 200 + np.arange(400)[None, :]
+        idx = WB.frame_index(n)
+        assert int((raw[-1] >= n).sum()) == reach and int((raw >= n).sum()) == reach
+        assert sorted(idx[-1][raw[-1] >= n]) == list(range(n - 1 - reach, n - 1))  # n - 41 + n mod 160 .. n - 2
+        for i in (0, n - 1):  # each appears where its own padded position does, and nowhere else
+            assert np.array_equal(idx == i, raw == i), (n, i)
+        x = WB.waveform(n, "noise").astype(np.float32).astype(np.float64)
+        xr, m = WB.saved_rows(x)
+        G = np.zeros((W.num_rows(n), 80), dtype=np.float32)
+        G[0], G[T - 1] = 1.0, -1.0
+        got = WB.run_host_check(harness, tmp_path, x, xr, m, G)
+        want = WB.restated_grad(x, G.astype(np.float64), 80, xr=xr.astype(np.float64), m=m)
+        assert WB.rel_err(got, want) < 2e-4, (n, WB.rel_err(got, want))
+        ends = np.r_[0:202, (T - 1) * 160 - 200:n]
+        assert np.allclose(got[ends], want[ends], rtol=1e-3, atol=1e-4 * np.abs(want).max()), n
+        assert not got[201:(T - 1) * 160 - 200].any()  # frame 0 reaches 200 (its image of 200), the last starts at 160 (T - 1) - 200
 
 
 def test_abi_whisper_entries_refuse_bad_calls_without_a_gpu():

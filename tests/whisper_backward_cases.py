@@ -136,6 +136,54 @@ def saved_rows(x: np.ndarray, num_filters=80):
     return xr, float(xr.max())
 
 
+# ----------------------------------------------------------------------------- the B200 class on the GPU
+def extractor(kernel="auto", M=80):
+    import lhotse_b200 as lb
+
+    return lb.B200WhisperFbank(lb.B200WhisperFbankConfig(num_filters=M, kernel=kernel))
+
+
+def loss(feats, G):
+    return (feats * torch.as_tensor(G, dtype=feats.dtype, device=feats.device)).sum()
+
+
+def b200_grad(ext, x, G, dtype=torch.float32, device="cuda"):
+    """d sum(features * G) / dx of one cut through `extract`, as float64 NumPy."""
+    xt = torch.tensor(np.asarray(x), dtype=dtype, device=device, requires_grad=True)
+    loss(ext.extract(xt, 16000), G).backward()
+    return xt.grad.double().cpu().numpy()
+
+
+def b200_grads(ext, xs, Gs):
+    """float32 gradients (CUDA tensors) of sum_i <features(x_i), G_i> over one `extract_batch` call on the list `xs`."""
+    leaves = [torch.tensor(np.asarray(x), dtype=torch.float32, device="cuda", requires_grad=True) for x in xs]
+    outs = ext.extract_batch(leaves, 16000)
+    sum(loss(o, G) for o, G in zip(outs, Gs)).backward()
+    return [t.grad for t in leaves]
+
+
+def case(n, kind, M, seed=0):
+    """A waveform and a row gradient whose decisions agree across precisions: G is 0 on values within 1e-3 of m - 8 or of
+    the floor's log (-10), and the cut's maximum is unique by 1e-3 (asserted)."""
+    x = waveform(n, kind, seed).astype(np.float32).astype(np.float64)
+    xr = logmel_t(torch.tensor(x), M).numpy()
+    m = xr.max()
+    top = np.sort(xr.ravel())[-2:] if xr.size > 1 else np.asarray([-np.inf, m])
+    assert top[1] - top[0] > 1e-3, (n, kind, M)
+    G = np.random.RandomState(n + M + seed).randn(W.num_rows(n), M)
+    near = (np.abs(xr - (m - 8.0)) < 1e-3) | (np.abs(xr + 10.0) < 1e-3)
+    G[: xr.shape[0]][near] = 0.0
+    return x, G
+
+
+def gate(x, G, M, g):
+    """(||g - g64||, the bound 8 ||g32 - g64|| + 1e-7 ||g64||, ||g32 - g64||): g64 float64 autograd through the oracle's
+    chain, g32 the same chain in float32 on the GPU."""
+    g64 = autograd_grad(x, G, M)
+    g32 = autograd_grad(x, G, M, dtype=torch.float32, device="cuda")
+    err, err32 = float(np.linalg.norm(g - g64)), float(np.linalg.norm(g32 - g64))
+    return err, 8.0 * err32 + 1e-7 * float(np.linalg.norm(g64)), err32
+
 # ----------------------------------------------------------------------------- host harness
 def host_check_binary(tmp_dir):
     """scripts/micro/whisper_backward_host_check.cu compiled for the host (with AddressSanitizer where the toolchain has
