@@ -456,6 +456,56 @@ int b200feat_reverb_ex(b200feat_handle *h, const int16_t *src0_dev, int64_t src0
                        float *out_dev, int64_t out_elems, void *work_dev, int64_t work_bytes, void *stream);
 
 /*
+ * Single-channel WPE dereverberation on the GPU: lhotse's DereverbWPE (torch.stft with a centred, reflect-padded frame and
+ * the periodic Blackman window, nara_wpe's wpe_v8, torch.istft, then the cut's length fix), within a float32 tolerance of a
+ * float64 restatement (DESIGN.md §3.1q).  The inputs are float32 samples of one buffer (e.g. what b200feat_resample or
+ * b200feat_reverb wrote); every cut's result is written as float32 into a ragged output buffer that b200feat_extract takes
+ * as B200FEAT_F32.  A cut of L samples has T = 1 + L / 128 frames and dereverberates to 128 (T - 1) = 128 (L / 128) samples.
+ */
+#define B200FEAT_WPE_MAX_TAPS 16      /* the most filter taps */
+#define B200FEAT_WPE_MAX_FRAMES 8192  /* the most frames of one cut (L <= 1048575: 65.5 s at 16 kHz) */
+#define B200FEAT_WPE_FULL 0           /* b200feat_wpe_params.statistics_mode: statistics over every frame */
+#define B200FEAT_WPE_VALID 1          /* ... over the frames t >= delay + taps - 1 */
+
+typedef struct b200feat_wpe_params {
+  int32_t struct_size;      /* sizeof(b200feat_wpe_params) — ABI guard */
+  int32_t n_fft;            /* 512: the only transform size */
+  int32_t hop;              /* 128: the only hop */
+  int32_t taps;             /* 1 .. B200FEAT_WPE_MAX_TAPS (lhotse: 10) */
+  int32_t delay;            /* >= 0 (lhotse: 3) */
+  int32_t iterations;       /* 0 .. 64 (lhotse: 3; 0 leaves the spectra as they are) */
+  int32_t statistics_mode;  /* B200FEAT_WPE_FULL | B200FEAT_WPE_VALID */
+  int32_t reserved;
+} b200feat_wpe_params;
+
+typedef struct b200feat_wpe_cut {
+  int32_t struct_size;   /* sizeof(b200feat_wpe_cut) — ABI guard, in every record */
+  int32_t reserved;
+  int64_t in_elem;       /* first input sample in the input buffer */
+  int64_t in_len;        /* L: more than 256 (the reflect pad), 1 + L / 128 >= taps + delay, at most B200FEAT_WPE_MAX_FRAMES frames */
+  int64_t out_elem;      /* first output sample in the output buffer */
+  int64_t target_len;    /* samples written: 128 (L / 128), fewer (trimmed) or at most 128 (L / 128) - 1 more (np.pad(mode="reflect")) */
+} b200feat_wpe_cut;
+/* No cut's output window [out_elem, out_elem + target_len) may overlap any cut's input window [in_elem, in_elem + in_len)
+ * in memory: b200feat_wpe refuses such tables, and leaves the input as it was. */
+
+/* Device scratch b200feat_wpe needs for these cuts (0 when the count is negative): the cuts' spectra, 257 x T complex64 per
+ * cut (about 16 bytes per input sample), plus a few KB of tables. */
+int64_t b200feat_wpe_work_bytes(const b200feat_wpe_cut *cuts, int32_t ncuts);
+
+/* Checks the parameters (n_fft and hop other than 512 and 128: B200FEAT_EUNSUPPORTED; taps, delay, iterations and
+ * statistics_mode outside their ranges: B200FEAT_EINVAL) and the cut table (a cut too short for the reflect pad or with
+ * fewer than taps + delay frames: B200FEAT_ESHORT; more than B200FEAT_WPE_MAX_FRAMES frames, a read outside the input, a
+ * write outside the output, reflect padding longer than the signal, an output overlapping an input: B200FEAT_EINVAL), copies
+ * the tables and the host `window` (n_fft floats: torch.blackman_window(512)'s float32 values) to `work_dev` and launches
+ * the STFT, per-bin and iSTFT kernels, asynchronously on `stream`.  No atomics: results are identical from run to run, and
+ * a cut's output does not depend on the other cuts of the call.  Errors are reported through `h` (b200feat_last_error)
+ * when it is not NULL, and through b200feat_global_error. */
+int b200feat_wpe(b200feat_handle *h, const float *in_dev, int64_t in_elems, const b200feat_wpe_cut *cuts, int32_t ncuts,
+                 const b200feat_wpe_params *params, const float *window, float *out_dev, int64_t out_elems, void *work_dev,
+                 int64_t work_bytes, void *stream);
+
+/*
  * lhotse's FastRandomRIRGenerator (one source) on the GPU, from draws made on the host (DESIGN.md §3.1l): the Dirac comb at
  * 64 x sr, its 8 -> 1 resampling and torchaudio's 80 Hz highpass biquad, written as float32 at 8 x sr.  b200feat_resample
  * with the same 8 -> 1 table then gives the RIR at sr.  Results are identical from run to run.

@@ -35,7 +35,9 @@ from .engine import Engine, B200FeatError, load_library  # noqa: F401
 from .pcm_staging import FlacRequest, decode_flac, flac_request_for_cut  # noqa: F401
 from .pcm_staging import MixRequest, mix_cuts, mix_request_for_cut  # noqa: F401
 from .pcm_staging import ReverbRequest, TransformRequest, transform_cuts, transform_request_for_cut  # noqa: F401
+from .pcm_staging import WpeRequest  # noqa: F401
 from .spec_augment import B200SpecAugment, spec_augment_plan  # noqa: F401
+from .dereverb import B200DereverbWPE  # noqa: F401
 from .precomputed import FusedPrecomputedFeatures, precomputed_plan  # noqa: F401
 from .input_strategies import FusedAudioSamples  # noqa: F401
 

@@ -10,7 +10,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libb200feat.so")
 SOURCES = ["b200feat.cu"]
-HEADERS = ["common.cuh", "generic.cuh", "fast512.cuh", "tc512.cuh", "fast256.cuh", "fast2048.cuh", "fast1024.cuh", "fast400.cuh", "flac.cuh", "mix.cuh", "resample.cuh", "reverb.cuh", "specaug.cuh", "rirgen.cuh", "featmix.cuh", "backward.cuh", "collate.cuh", os.path.join("..", "..", "include", "b200feat.h")]
+HEADERS = ["common.cuh", "generic.cuh", "fast512.cuh", "tc512.cuh", "fast256.cuh", "fast2048.cuh", "fast1024.cuh", "fast400.cuh", "flac.cuh", "mix.cuh", "resample.cuh", "reverb.cuh", "specaug.cuh", "rirgen.cuh", "featmix.cuh", "backward.cuh", "collate.cuh", "wpe.cuh", os.path.join("..", "..", "include", "b200feat.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -34,6 +34,7 @@
 #include "featmix.cuh"
 #include "backward.cuh"
 #include "collate.cuh"
+#include "wpe.cuh"
 
 #include <cub/device/device_segmented_radix_sort.cuh>
 
@@ -1279,6 +1280,135 @@ int b200feat_reverb_ex(b200feat_handle *h, const int16_t *src0_dev, int64_t src0
   CU_TRY(h, cudaGetLastError());
   const int64_t gx = std::min<int64_t>((longest + 4 * RV_OUT_THREADS - 1) / (4 * RV_OUT_THREADS), 1024);
   reverb_out_kernel<<<dim3((unsigned)gx, (unsigned)ncuts), RV_OUT_THREADS, 0, st>>>(d_cuts, d_gain);
+  CU_TRY(h, cudaGetLastError());
+  return B200FEAT_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The WPE work buffer: the kernels' cut table, the window, the twiddles, then every cut's [bin][frame] spectra
+struct WpeLayout {
+  int64_t cuts, window, twiddles, spectra, total;
+  int64_t frames;
+};
+
+WpeLayout wpe_layout(const b200feat_wpe_cut *cuts, int32_t ncuts) {
+  auto up = [](int64_t b) { return (b + 255) / 256 * 256; };
+  WpeLayout l{};
+  for (int32_t i = 0; i < ncuts; ++i)
+    l.frames += wpe_frames(std::min<int64_t>(std::max<int64_t>(cuts[i].in_len, 0), (int64_t)1 << 40));
+  l.cuts = 0;
+  l.window = l.cuts + up((int64_t)ncuts * (int64_t)sizeof(WpeCut));
+  l.twiddles = l.window + up(WPE_NFFT * (int64_t)sizeof(float));
+  l.spectra = l.twiddles + up(WPE_NFFT / 2 * (int64_t)sizeof(wpe_c));
+  l.total = l.spectra + up(l.frames * WPE_BINS * (int64_t)sizeof(wpe_c));
+  return l;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t b200feat_wpe_work_bytes(const b200feat_wpe_cut *cuts, int32_t ncuts) {
+  if (ncuts < 0 || (ncuts > 0 && !cuts)) return 0;
+  return wpe_layout(cuts, ncuts).total;
+}
+
+int b200feat_wpe(b200feat_handle *h, const float *in_dev, int64_t in_elems, const b200feat_wpe_cut *cuts, int32_t ncuts,
+                 const b200feat_wpe_params *params, const float *window, float *out_dev, int64_t out_elems, void *work_dev,
+                 int64_t work_bytes, void *stream) {
+  if (ncuts < 0 || !params || in_elems < 0 || out_elems < 0 ||
+      (ncuts > 0 && (!cuts || !window || !in_dev || !out_dev || !work_dev)))
+    return fail(h, B200FEAT_EINVAL, "wpe: bad arguments");
+  const b200feat_wpe_params &pm = *params;
+  if (pm.struct_size != (int32_t)sizeof(b200feat_wpe_params))
+    return fail(h, B200FEAT_EINVAL, "wpe: b200feat_wpe_params size mismatch (ABI)");
+  if (pm.n_fft != WPE_NFFT || pm.hop != WPE_HOP)
+    return fail(h, B200FEAT_EUNSUPPORTED, "wpe: only n_fft = 512 and hop = 128 are supported");
+  if (pm.taps < 1 || pm.taps > B200FEAT_WPE_MAX_TAPS) return fail(h, B200FEAT_EINVAL, "wpe: taps outside 1 .. B200FEAT_WPE_MAX_TAPS");
+  if (pm.delay < 0 || pm.delay > B200FEAT_WPE_MAX_FRAMES) return fail(h, B200FEAT_EINVAL, "wpe: delay outside 0 .. B200FEAT_WPE_MAX_FRAMES");
+  if (pm.iterations < 0 || pm.iterations > 64) return fail(h, B200FEAT_EINVAL, "wpe: iterations outside 0 .. 64");
+  if (pm.statistics_mode != B200FEAT_WPE_FULL && pm.statistics_mode != B200FEAT_WPE_VALID)
+    return fail(h, B200FEAT_EINVAL, "wpe: statistics_mode must be B200FEAT_WPE_FULL or B200FEAT_WPE_VALID");
+  if (ncuts == 0) return B200FEAT_OK;
+  if ((int64_t)ncuts * WPE_BINS > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "wpe: too many cuts in one call");
+  auto where = [](int64_t i) { return std::string("wpe: cut ") + std::to_string(i) + ": "; };
+  for (int32_t c = 0; c < ncuts; ++c) {
+    const b200feat_wpe_cut &cu = cuts[c];
+    if (cu.struct_size != (int32_t)sizeof(b200feat_wpe_cut))
+      return fail(h, B200FEAT_EINVAL, where(c) + "b200feat_wpe_cut size mismatch (ABI)");
+    if (cu.in_len < 0 || cu.in_elem < 0 || cu.in_elem > in_elems - cu.in_len)
+      return fail(h, B200FEAT_EINVAL, where(c) + "input outside the input buffer");
+    if (cu.in_len <= WPE_NFFT / 2 || wpe_frames(cu.in_len) < (int64_t)pm.taps + pm.delay)
+      return fail(h, B200FEAT_ESHORT, where(c) + "too short: L > 256 and 1 + L / 128 >= taps + delay are needed");
+    if (wpe_frames(cu.in_len) > B200FEAT_WPE_MAX_FRAMES)
+      return fail(h, B200FEAT_EINVAL, where(c) + "longer than B200FEAT_WPE_MAX_FRAMES frames");
+    const int64_t lz = wpe_istft_len(cu.in_len);
+    if (cu.target_len < 0 || (cu.target_len > lz && cu.target_len - lz > lz - 1))
+      return fail(h, B200FEAT_EINVAL, where(c) + "bad target_len (reflect padding longer than the signal?)");
+    if (cu.out_elem < 0 || cu.out_elem > out_elems - cu.target_len)
+      return fail(h, B200FEAT_EINVAL, where(c) + "output outside the output buffer");
+  }
+  {  // no cut's output window may overlap any cut's input window (the header's contract: the input is left as it was)
+    std::vector<std::pair<uintptr_t, uintptr_t>> in(ncuts);
+    for (int32_t c = 0; c < ncuts; ++c) {
+      const uintptr_t a = (uintptr_t)(in_dev + cuts[c].in_elem);
+      in[c] = {a, a + (uintptr_t)cuts[c].in_len * sizeof(float)};
+    }
+    std::sort(in.begin(), in.end());
+    std::vector<uintptr_t> reach(ncuts);  // the furthest end among the first i + 1 windows
+    for (int32_t c = 0; c < ncuts; ++c) reach[c] = std::max(in[c].second, c ? reach[c - 1] : 0);
+    for (int32_t c = 0; c < ncuts; ++c) {
+      if (cuts[c].target_len == 0) continue;
+      const uintptr_t a = (uintptr_t)(out_dev + cuts[c].out_elem), b = a + (uintptr_t)cuts[c].target_len * sizeof(float);
+      const auto it = std::lower_bound(in.begin(), in.end(), std::make_pair(b, (uintptr_t)0));
+      if (it != in.begin() && reach[(it - in.begin()) - 1] > a)
+        return fail(h, B200FEAT_EINVAL, where(c) + "output overlaps an input window");
+    }
+  }
+  const WpeLayout l = wpe_layout(cuts, ncuts);
+  if (work_bytes < l.total) return fail(h, B200FEAT_EINVAL, "wpe: work buffer too small");
+  char *w = (char *)work_dev;
+  wpe_c *spectra = (wpe_c *)(w + l.spectra);
+  std::vector<WpeCut> cv((size_t)ncuts);
+  int64_t tiles = 0, outs = 0, frames = 0, longest = 1;
+  for (int32_t c = 0; c < ncuts; ++c) {
+    const b200feat_wpe_cut &cu = cuts[c];
+    const int64_t T = wpe_frames(cu.in_len);
+    cv[c] = WpeCut{in_dev + cu.in_elem, out_dev + cu.out_elem, spectra + frames * WPE_BINS, cu.in_len, cu.target_len, tiles,
+                   outs, (int32_t)T, 0};
+    tiles += wpe_stft_ctas(T);
+    outs += wpe_istft_ctas(T);
+    frames += T;
+    longest = std::max(longest, T);
+  }
+  if (tiles > 0x7fffffff || outs > 0x7fffffff) return fail(h, B200FEAT_EINVAL, "wpe: too many CTAs in one call");
+  // over the 48 KB a launch gets without asking; set on every call (the attribute belongs to the current device)
+  CU_TRY(h, cudaFuncSetAttribute(wpe_stft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WPE_STFT_SMEM));
+  CU_TRY(h, cudaFuncSetAttribute(wpe_istft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WPE_ISTFT_SMEM));
+  CU_TRY(h, cudaFuncSetAttribute(wpe_bin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 WPE_BIN_SMEM(B200FEAT_WPE_MAX_FRAMES)));
+  const cudaStream_t st = (cudaStream_t)stream;
+  WpeCut *d_cuts = (WpeCut *)(w + l.cuts);
+  float *d_window = (float *)(w + l.window);
+  wpe_c *d_twiddles = (wpe_c *)(w + l.twiddles);
+  static const std::vector<wpe_c> twiddles = [] {
+    std::vector<wpe_c> t(WPE_NFFT / 2);
+    for (int k = 0; k < WPE_NFFT / 2; ++k) t[k] = wpe_twiddle(k);
+    return t;
+  }();
+  // pageable copies: the call returns once the tables have been staged, so the caller's arrays may go when it returns
+  CU_TRY(h, cudaMemcpyAsync(d_twiddles, twiddles.data(), WPE_NFFT / 2 * sizeof(wpe_c), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_window, window, WPE_NFFT * sizeof(float), cudaMemcpyHostToDevice, st));
+  CU_TRY(h, cudaMemcpyAsync(d_cuts, cv.data(), cv.size() * sizeof(WpeCut), cudaMemcpyHostToDevice, st));
+  wpe_stft_kernel<<<(unsigned)tiles, WPE_THREADS, WPE_STFT_SMEM, st>>>(d_cuts, ncuts, d_window, d_twiddles);
+  CU_TRY(h, cudaGetLastError());
+  const WpeParams prm{pm.taps, pm.delay, pm.iterations, pm.statistics_mode == B200FEAT_WPE_VALID};
+  wpe_bin_kernel<<<(unsigned)(ncuts * WPE_BINS), WPE_THREADS, WPE_BIN_SMEM(longest), st>>>(d_cuts, prm);
+  CU_TRY(h, cudaGetLastError());
+  wpe_istft_kernel<<<(unsigned)outs, WPE_THREADS, WPE_ISTFT_SMEM, st>>>(d_cuts, ncuts, d_window, d_twiddles);
   CU_TRY(h, cudaGetLastError());
   return B200FEAT_OK;
 }

@@ -172,7 +172,7 @@ def compute_and_store_features_sharded(cuts, extractor, storage_path, rank: Opti
         from .storage import compute_and_store_features_fused
 
         allowed = {k: v for k, v in kwargs.items() if k in ("batch_duration", "num_workers", "overwrite", "pcm16_fast_path",
-                                                            "reverb", "generated_rir")}
+                                                            "reverb", "generated_rir", "wpe")}
         return compute_and_store_features_fused(mine, extractor, storage_path / f"feats-{rank}",
                                                 manifest_path=storage_path / f"{manifest_name}-{rank}.jsonl.gz", **allowed)
     return mine.compute_and_store_features_batch(

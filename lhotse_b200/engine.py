@@ -119,6 +119,18 @@ FEATMIX_LOG, FEATMIX_LINEAR = 0, 1
 FEATMIX_COPY, FEATMIX_MIX = 0, 1
 FEATMIX_MIXED, FEATMIX_ENERGY = 1, 2
 
+# b200feat_wpe_cut as a numpy record layout; b200feat_wpe_params
+WPE_CUT_DTYPE = np.dtype([("struct_size", "<i4"), ("reserved", "<i4"), ("in_elem", "<i8"), ("in_len", "<i8"), ("out_elem", "<i8"),
+                          ("target_len", "<i8")])
+WPE_MAX_TAPS = 16       # B200FEAT_WPE_MAX_TAPS
+WPE_MAX_FRAMES = 8192   # B200FEAT_WPE_MAX_FRAMES
+WPE_FULL, WPE_VALID = 0, 1
+
+
+class WpeParams(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("n_fft", C.c_int32), ("hop", C.c_int32), ("taps", C.c_int32), ("delay", C.c_int32),
+                ("iterations", C.c_int32), ("statistics_mode", C.c_int32), ("reserved", C.c_int32)]
+
 
 EXPORTS = [
     "b200feat_version", "b200feat_global_error", "b200feat_create", "b200feat_destroy",
@@ -132,6 +144,7 @@ EXPORTS = [
     "b200feat_reverb_ex", "b200feat_rir_generate_work_bytes", "b200feat_rir_generate",
     "b200feat_feature_mix_work_bytes", "b200feat_feature_mix", "b200feat_backward_work_bytes", "b200feat_backward",
     "b200feat_collate_audio_work_bytes", "b200feat_collate_audio", "b200feat_extract_keep_raw", "b200feat_whisper_backward",
+    "b200feat_wpe_work_bytes", "b200feat_wpe",
 ]
 
 
@@ -237,6 +250,10 @@ def load_library():
         lib.b200feat_collate_audio_work_bytes.argtypes = [i32]
         lib.b200feat_collate_audio.restype = C.c_int
         lib.b200feat_collate_audio.argtypes = [vp, vp, i32, i64, vp, vp, i32, i64, vp, vp, i64, vp]
+        lib.b200feat_wpe_work_bytes.restype = i64
+        lib.b200feat_wpe_work_bytes.argtypes = [vp, i32]
+        lib.b200feat_wpe.restype = C.c_int
+        lib.b200feat_wpe.argtypes = [vp, vp, i64, vp, i32, C.POINTER(WpeParams), vp, vp, i64, vp, i64, vp]
         if lib.b200feat_version() != 1:
             raise ImportError("libb200feat.so ABI version mismatch")
         _LIB = lib
@@ -473,6 +490,35 @@ def collate_audio(src: Optional[torch.Tensor], offsets: Sequence[int], lens: Seq
     with torch.cuda.device(out.device):
         rc = lib.b200feat_collate_audio(handle, p, dt, n, off.ctypes.data, ln.ctypes.data, B, T, out.data_ptr(), work.data_ptr(),
                                         work.numel(), stream)
+    if rc != 0:
+        _raise(lib, rc, handle)
+
+
+def wpe_window(n_fft: int = 512) -> np.ndarray:
+    """torch.blackman_window(n_fft) as float32: the window lhotse's DereverbWPE frames with (element 0 is -2.98e-8, not 0)."""
+    return torch.blackman_window(n_fft).numpy().astype(np.float32)
+
+
+def wpe(x: torch.Tensor, cuts: np.ndarray, out: torch.Tensor, taps: int = 10, delay: int = 3, iterations: int = 3,
+        statistics_mode: str = "full", n_fft: int = 512, hop_length: int = 128, handle=None) -> None:
+    """Launches `b200feat_wpe` on the current stream of `out`'s device (asynchronous): the float32 input `x`, the host cut
+    table (WPE_CUT_DTYPE; copied before this returns) and the float32 output, with lhotse's DereverbWPE parameters.  Raises
+    B200FeatError when the library refuses the parameters or the table (B200FEAT_ESHORT, -5, for a cut too short)."""
+    lib = load_library()
+    assert cuts.dtype == WPE_CUT_DTYPE and x.dtype == torch.float32 and out.dtype == torch.float32
+    if statistics_mode not in ("full", "valid"):
+        raise ValueError(f"statistics_mode must be 'full' or 'valid', got {statistics_mode!r}")
+    cuts = np.ascontiguousarray(cuts)
+    prm = WpeParams(C.sizeof(WpeParams), int(n_fft), int(hop_length), int(taps), int(delay), int(iterations),
+                    WPE_FULL if statistics_mode == "full" else WPE_VALID, 0)
+    window = wpe_window(n_fft)
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    work = torch.empty(max(int(lib.b200feat_wpe_work_bytes(cuts.ctypes.data, len(cuts))), 1), dtype=torch.uint8,
+                       device=out.device)
+    px, nx = (None, 0) if x.numel() == 0 else (x.data_ptr(), x.numel())
+    with torch.cuda.device(out.device):
+        rc = lib.b200feat_wpe(handle, px, nx, cuts.ctypes.data, len(cuts), C.byref(prm), window.ctypes.data, out.data_ptr(),
+                              out.numel(), work.data_ptr(), work.numel(), stream)
     if rc != 0:
         _raise(lib, rc, handle)
 

@@ -38,6 +38,7 @@ class FusedOnTheFlyFeatures:
         perturbed_tracks: bool = False,
         reverb: bool = False,
         generated_rir: bool = False,
+        wpe: bool = False,
     ) -> None:
         if not hasattr(extractor, "extract_batch_padded"):
             raise TypeError("FusedOnTheFlyFeatures needs a lhotse_b200 extractor (extract_batch_padded)")
@@ -70,12 +71,16 @@ class FusedOnTheFlyFeatures:
         # exactly their routes and features, and whether to turn it on by default is decided once H100 measurements of it
         # exist.  `generated_rir=True` does the same for cuts whose RIR lhotse generates (no RIR corpus): the generator's
         # random numbers are drawn on the host from the same generators in the same order, the RIRs are built on the GPU
-        # (DESIGN.md §3.1l); it is a separate flag so that `reverb=True` pipelines keep exactly their routes.
+        # (DESIGN.md §3.1l); it is a separate flag so that `reverb=True` pipelines keep exactly their routes.  `wpe=True`
+        # lets the "transform" route also take cuts whose chain ends in lhotse's DereverbWPE (`cuts.dereverb_wpe()`, after
+        # Speed / Volume / Resample and a reverb or not): the dereverberation runs on the GPU (DESIGN.md §3.1q) within a
+        # float32 tolerance of a float64 restatement, not bit for bit, so it is off by default too.
         # `pcm16_fast_path=False` turns all staged routes off.
         self.pcm16_fast_path = pcm16_fast_path and hasattr(extractor, "extract_staged_padded")
         self.perturbed_tracks = perturbed_tracks
         self.reverb = reverb
         self.generated_rir = generated_rir
+        self.wpe = wpe
         self._rings = {}  # route -> its staging ring, made when a batch first takes the route
         self.last_batch_route = None  # "pcm16" | "flac" | "mix" | "transform" | "float" (introspection for tests / logs)
         self._executor_type = executor_type
@@ -113,7 +118,7 @@ class FusedOnTheFlyFeatures:
         from .pcm_staging import new_ring, staged_route, undo_draws
 
         chosen = staged_route(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb,
-                              generated_rir=self.generated_rir)
+                              generated_rir=self.generated_rir, wpe=self.wpe)
         if chosen is None:
             return None  # mixed sampling rates (grouped by the float route) or a cut no staged route takes
         route, reqs = chosen
@@ -224,6 +229,7 @@ class FusedAudioSamples:
         perturbed_tracks: bool = False,
         reverb: bool = False,
         generated_rir: bool = False,
+        wpe: bool = False,
     ) -> None:
         self.num_workers = num_workers
         self.fault_tolerant = fault_tolerant
@@ -241,6 +247,7 @@ class FusedAudioSamples:
         self.perturbed_tracks = perturbed_tracks
         self.reverb = reverb
         self.generated_rir = generated_rir
+        self.wpe = wpe
         self._rings = {}  # route -> its staging ring, made when a batch first takes the route
         self.last_batch_route = None  # one of pcm_staging.STAGED_ROUTES | "reference"
         self.last_decline = None
@@ -268,7 +275,7 @@ class FusedAudioSamples:
         from .pcm_staging import collate_staged, new_ring, staged_route, undo_draws
 
         chosen = staged_route(cuts, perturbed_tracks=self.perturbed_tracks, reverb=self.reverb,
-                              generated_rir=self.generated_rir)
+                              generated_rir=self.generated_rir, wpe=self.wpe)
         if chosen is None:
             return "a cut that no staged route takes"
         route, reqs = chosen

@@ -32,7 +32,7 @@ import os
 import struct
 import threading
 from collections import OrderedDict
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -1097,12 +1097,49 @@ class GeneratedRirRequest:
 
 
 @dataclass(frozen=True)
+class WpeRequest:
+    """A DereverbWPE transform's parameters (its n_fft and hop are 512 and 128: `wpe_request` takes no others)."""
+    taps: int = 10
+    delay: int = 3
+    iterations: int = 3
+    statistics_mode: str = "full"
+
+
+@dataclass(frozen=True)
 class TransformRequest:
     source: object             # PcmRequest | FlacRequest: the slice of the file the chain starts from
     ops: Tuple[tuple, ...]     # in chain order: ("volume", float32 factor) | ("resample", orig, new)
     num_samples: int           # the cut's length: the chain's output is trimmed or reflect-padded to it
     sampling_rate: int         # the cut's (the recording's, after the chain)
     reverb: Optional[ReverbRequest] = None  # a last ReverbWithImpulseResponse, run on the chain's output before the length fix
+    wpe: Optional[WpeRequest] = None  # a last DereverbWPE, run on the chain's (or the reverb's) output before the length fix
+
+
+def wpe_request(t) -> Optional[WpeRequest]:
+    """The parameters of a DereverbWPE transform the GPU takes (csrc/wpe.cuh): n_fft 512, hop_length 128, 1 <= taps <=
+    WPE_MAX_TAPS, delay >= 0, 0 <= iterations <= 64, statistics_mode "full" or "valid", all plain ints.  None otherwise."""
+    from .engine import WPE_MAX_TAPS
+
+    ints = (t.n_fft, t.hop_length, t.taps, t.delay, t.iterations)
+    if any(type(v) is not int for v in ints) or (t.n_fft, t.hop_length) != (512, 128):
+        return None
+    if not 1 <= t.taps <= WPE_MAX_TAPS or t.delay < 0 or not 0 <= t.iterations <= 64:
+        return None
+    if t.statistics_mode not in ("full", "valid"):
+        return None
+    return WpeRequest(taps=t.taps, delay=t.delay, iterations=t.iterations, statistics_mode=t.statistics_mode)
+
+
+def wpe_output_len(L: int, w: WpeRequest) -> Optional[int]:
+    """The length DereverbWPE gives a signal of L samples, 128 (L // 128); None when the GPU does not take it: L <= 256
+    (torch.stft's reflect pad), fewer than taps + delay frames (R is singular in exact arithmetic), more than WPE_MAX_FRAMES
+    frames (a bin no longer fits in shared memory)."""
+    from .engine import WPE_MAX_FRAMES
+
+    T = 1 + L // 128
+    if L <= 256 or T < w.taps + w.delay or T > WPE_MAX_FRAMES:
+        return None
+    return 128 * (L // 128)
 
 
 def reverb_request(t, sampling_rate: int, reverb: bool = True, generated_rir: bool = False) -> Optional[ReverbRequest]:
@@ -1148,7 +1185,8 @@ def reverb_request(t, sampling_rate: int, reverb: bool = True, generated_rir: bo
     return ReverbRequest(rir=src, normalize=bool(t.normalize_output))
 
 
-def transform_request_for_cut(cut, reverb: bool = False, generated_rir: bool = False) -> Optional[TransformRequest]:
+def transform_request_for_cut(cut, reverb: bool = False, generated_rir: bool = False,
+                              wpe: bool = False) -> Optional[TransformRequest]:
     """What `cut.load_audio()` (audio/recording.py load_audio) amounts to for a MonoCut over a single-channel 16-bit WAV or
     FLAC file whose recording carries a non-empty chain of Speed, Volume and Resample transforms: the source slice (the
     transforms' own reverse_timestamps applied to the cut's range, a read to the end of the file when the cut's duration is
@@ -1161,9 +1199,16 @@ def transform_request_for_cut(cut, reverb: bool = False, generated_rir: bool = F
     reverb alone included): the stages before it write the pre-reverb signal, and the reverb kernel (csrc/reverb.cuh) writes
     the cut, within a float32 tolerance of a float64 convolution rather than bit for bit (DESIGN.md §3.1j).  Off by default
     so that existing callers keep exactly the routes and samples they have.  `generated_rir=True` takes such a last
-    reverb with an RIR that lhotse generates (see `reverb_request`; DESIGN.md §3.1l), also off by default."""
+    reverb with an RIR that lhotse generates (see `reverb_request`; DESIGN.md §3.1l), also off by default.
+
+    `wpe=True` also takes a chain whose last transform is a DereverbWPE that `wpe_request` accepts, after Speed / Volume /
+    Resample stages and an optional reverb (WPE alone on a plain slice included, what `cuts.dereverb_wpe()` makes): the
+    signal before it goes to an intermediate buffer at its natural length and the WPE kernels (csrc/wpe.cuh) write the cut,
+    within a float32 tolerance of a float64 restatement (DESIGN.md §3.1q).  The duration-mismatch check then applies to
+    DereverbWPE's output length, 128 (L // 128).  Off by default."""
     try:
         from lhotse.augmentation.rir import ReverbWithImpulseResponse
+        from lhotse.augmentation.wpe import DereverbWPE
         from lhotse.audio.resampling_backend import get_current_resampling_backend
         from lhotse.audio.utils import get_audio_duration_mismatch_tolerance
         from lhotse.augmentation import torchaudio as lta
@@ -1179,8 +1224,14 @@ def transform_request_for_cut(cut, reverb: bool = False, generated_rir: bool = F
     if torch.get_default_dtype() != torch.float32:
         return None  # lhotse's table phases and output lengths are evaluated in the default dtype
     tfs = [t if isinstance(t, AudioTransform) else AudioTransform.from_dict(t) for t in rec.transforms]
+    wr = None
+    if wpe and type(tfs[-1]) is DereverbWPE:
+        wr = wpe_request(tfs[-1])
+        if wr is None:
+            return None
+        tfs = tfs[:-1]
     rv = None
-    if (reverb or generated_rir) and type(tfs[-1]) is ReverbWithImpulseResponse:
+    if (reverb or generated_rir) and tfs and type(tfs[-1]) is ReverbWithImpulseResponse:
         rv = reverb_request(tfs[-1], rec.sampling_rate, reverb, generated_rir)
         if rv is None:
             return None
@@ -1226,32 +1277,38 @@ def transform_request_for_cut(cut, reverb: bool = False, generated_rir: bool = F
             return None
         ops.append(("resample", int(a), int(b)))
         L = resampled_len(N, L, O)
+    if wr is not None:
+        L = wpe_output_len(L, wr)
+        if L is None:
+            return None
     target = _samples(cut.duration, sr)
     diff = target - L
     if abs(diff) > int(math.ceil(get_audio_duration_mismatch_tolerance() * sr)) or diff > L - 1:
         return None
     return TransformRequest(source=make(path=h.path, first_sample=first, num_samples=n), ops=tuple(ops), num_samples=target,
-                            sampling_rate=int(sr), reverb=rv)
+                            sampling_rate=int(sr), reverb=rv, wpe=wr)
 
 
 def _has_transforms(cut) -> bool:
     return bool(getattr(getattr(cut, "recording", None), "transforms", None))
 
 
-def transform_requests_for_batch(cuts, reverb: bool = False, generated_rir: bool = False) -> Optional[List[TransformRequest]]:
+def transform_requests_for_batch(cuts, reverb: bool = False, generated_rir: bool = False,
+                                 wpe: bool = False) -> Optional[List[TransformRequest]]:
     """The "transform" route's requests for a batch: no MixedCut, every cut a plain 16-bit WAV / FLAC slice or an eligible
     transformed MonoCut, and at least one of the latter (batches of plain slices keep their routes).  None otherwise.
-    `reverb=True`: see `transform_request_for_cut`."""
+    `reverb=True`, `wpe=True`: see `transform_request_for_cut`."""
     if any(getattr(c, "tracks", None) is not None for c in cuts) or not any(_has_transforms(c) for c in cuts):
         return None
-    reqs = [_transform_or_plain_request(c, reverb, generated_rir) for c in cuts]
+    reqs = [_transform_or_plain_request(c, reverb, generated_rir, wpe) for c in cuts]
     return None if any(r is None for r in reqs) else reqs
 
 
-def _transform_or_plain_request(cut, reverb: bool = False, generated_rir: bool = False) -> Optional[TransformRequest]:
+def _transform_or_plain_request(cut, reverb: bool = False, generated_rir: bool = False,
+                                wpe: bool = False) -> Optional[TransformRequest]:
     """transform_request_for_cut, or a plain 16-bit WAV / FLAC slice as an empty chain (a copy of x = q / 32768)."""
     if _has_transforms(cut):
-        r = transform_request_for_cut(cut, reverb=reverb, generated_rir=generated_rir)
+        r = transform_request_for_cut(cut, reverb=reverb, generated_rir=generated_rir, wpe=wpe)
     else:
         src = slice_request_for_cut(cut)
         r = (TransformRequest(source=src, ops=(), num_samples=int(src.num_samples), sampling_rate=int(cut.sampling_rate))
@@ -1295,6 +1352,8 @@ class TransformBatch:
     reverb_rirs: Optional[np.ndarray] = None  # engine.REVERB_RIR_DTYPE: the batch's distinct RIRs in the two int16 sources
     reverb_cuts: Optional[np.ndarray] = None  # engine.REVERB_CUT_DTYPE: the reverberated cuts, reading `mid`
     generated: Optional["GeneratedRirs"] = None  # the generated RIRs, after the recorded ones in `reverb_rirs`
+    reverb_mid_cuts: Optional[np.ndarray] = None  # engine.REVERB_CUT_DTYPE: the reverberated cuts that WPE follows, `mid` to `mid`
+    wpe: List[Tuple[WpeRequest, np.ndarray]] = field(default_factory=list)  # engine.WPE_CUT_DTYPE per parameter set, `mid` to out
 
 
 def _stage_rirs(reqs) -> List[_SliceRequest]:
@@ -1391,15 +1450,16 @@ def _generate_rirs(gen: GeneratedRirs, device, handle=None) -> torch.Tensor:
     return out
 
 
-def _reverb_with(batch, src0, src1, x, out, handle, rir32) -> None:
-    """b200feat_reverb_ex over a staged batch's reverb tables, the generated RIRs' lengths filled in from their draws."""
+def _reverb_with(batch, src0, src1, x, out, handle, rir32, cuts: Optional[np.ndarray] = None) -> None:
+    """b200feat_reverb_ex over a staged batch's reverb tables (`cuts`, or its reverb_cuts), the generated RIRs' lengths
+    filled in from their draws."""
     from .engine import reverb
 
     rt = batch.reverb_rirs
     if batch.generated is not None:
         rt = rt.copy()
         rt["num_samples"][len(rt) - len(batch.generated.reqs):] = batch.generated.draws.lens
-    reverb(src0, src1, x, rt, batch.reverb_cuts, out, handle, rir32=rir32)
+    reverb(src0, src1, x, rt, batch.reverb_cuts if cuts is None else cuts, out, handle, rir32=rir32)
 
 
 def _reverb_tables(rirs, source, rir_elem, cuts, generated: Optional[GeneratedRirs] = None) -> Tuple[np.ndarray, np.ndarray]:
@@ -1427,6 +1487,17 @@ def _reverb_tables(rirs, source, rir_elem, cuts, generated: Optional[GeneratedRi
     for name, col in zip(("in_elem", "in_len", "out_elem", "target_len"), range(1, 5)):
         ct[name] = [c[col] for c in cuts]
     return rt, ct
+
+
+def _wpe_table(rows) -> np.ndarray:
+    """The b200feat_wpe cut table of rows = [(in_elem, in_len, out_elem, target_len)]."""
+    from .engine import WPE_CUT_DTYPE
+
+    ct = np.zeros(len(rows), dtype=WPE_CUT_DTYPE)
+    ct["struct_size"] = WPE_CUT_DTYPE.itemsize
+    for name, col in zip(("in_elem", "in_len", "out_elem", "target_len"), range(4)):
+        ct[name] = [r[col] for r in rows]
+    return ct
 
 
 class TransformStagingRing(_PinnedRing):
@@ -1465,6 +1536,8 @@ class TransformStagingRing(_PinnedRing):
         pairs, pair_ix = [], {}
         rows = []  # (depth, cut, table pair, source, in_elem, in_len, target, out_elem, out_len, target_len, scale_in, scale_out)
         rv_cuts = []  # (ReverbRequest, in_elem, in_len, out_elem, target_len)
+        rv_mid = []   # the same, for the reverbs that WPE follows: into `mid` at their natural length
+        wpe_cuts = {}  # WpeRequest -> [(in_elem, in_len, out_elem, target_len)]
         mid = 0
         for i, r in enumerate(requests):
             chain = _chain_stages(r.ops)
@@ -1479,14 +1552,21 @@ class TransformStagingRing(_PinnedRing):
                     N, O, _, _ = _resample_geometry(*pair)
                     n_out = resampled_len(N, L, O)
                 last = d == len(chain) - 1
-                to_out = last and r.reverb is None  # a reverberated cut's last stage writes the pre-reverb signal into `mid`
+                # a reverberated or dereverberated cut's last stage writes its signal into `mid` at its natural length
+                to_out = last and r.reverb is None and r.wpe is None
                 out_elem = offs[i] if to_out else mid
                 rows.append((d, i, pi, source, in_elem, L, RESAMPLE_TO_OUT if to_out else RESAMPLE_TO_MID, out_elem, n_out,
                              lens[i] if to_out else n_out, s_in, s_out))
                 if not to_out:
                     mid += n_out
-                if last and r.reverb is not None:
+                if last and r.reverb is not None and r.wpe is None:
                     rv_cuts.append((r.reverb, out_elem, n_out, offs[i], lens[i]))
+                elif last and r.reverb is not None:
+                    rv_mid.append((r.reverb, out_elem, n_out, mid, n_out))  # the reverb keeps the length: no length fix
+                    out_elem = mid
+                    mid += n_out
+                if last and r.wpe is not None:
+                    wpe_cuts.setdefault(r.wpe, []).append((out_elem, n_out, offs[i], lens[i]))
                 source, in_elem, L = RESAMPLE_MID, out_elem, n_out
         rows.sort(key=lambda row: (row[0], row[1]))
         nb = len(rows) * RESAMPLE_STAGE_DTYPE.itemsize
@@ -1501,9 +1581,13 @@ class TransformStagingRing(_PinnedRing):
         st["reserved"] = 0
         batch = TransformBatch(pcm=pcm_buf, flac=flac_batch, stages=st, pair=np.asarray(cols[2], dtype=np.int64), pairs=pairs,
                                mid_elems=mid, lens=lens, offsets=offs, out_elems=out_elems)
-        if rv_cuts:
+        if rv_cuts or rv_mid:
             batch.generated = generated if gen_reqs else None
-            batch.reverb_rirs, batch.reverb_cuts = _reverb_tables(rirs, kind[B:], src_elem[B:], rv_cuts, batch.generated)
+            batch.reverb_rirs, ct = _reverb_tables(rirs, kind[B:], src_elem[B:], rv_cuts + rv_mid, batch.generated)
+            batch.reverb_cuts = ct[: len(rv_cuts)] if rv_cuts else None
+            batch.reverb_mid_cuts = ct[len(rv_cuts):] if rv_mid else None
+        for w, rows_w in wpe_cuts.items():
+            batch.wpe.append((w, _wpe_table(rows_w)))
         if own:
             generated.draw()
         return batch, lens, offs, (srs.pop() if len(srs) == 1 else None)
@@ -1512,10 +1596,10 @@ class TransformStagingRing(_PinnedRing):
 def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] = None, handle=None,
                      rir32: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, List[int], List[int]]:
     """The device half of the "transform" route on the current stream: the rate pairs' tables (built and uploaded once per
-    device), H2D of the WAV slices, the FLAC decode (if any), the resampling stages, the reverb (if any); then `ring`'s copies
+    device), H2D of the WAV slices, the FLAC decode (if any), the resampling stages, the reverb and WPE (if any); then `ring`'s copies
     are marked in flight.  Returns (float32 samples on `device`, lengths, offsets).  The generated RIRs are built first
     unless `rir32` holds them (an enclosing mix batch built them)."""
-    from .engine import resample, resample_table
+    from .engine import resample, resample_table, wpe
 
     device = torch.device(device)
     with torch.cuda.device(device):
@@ -1526,25 +1610,33 @@ def transform_staged(batch: TransformBatch, device, ring: Optional[_PinnedRing] 
         mid = torch.empty(batch.mid_elems, dtype=torch.float32, device=device) if batch.mid_elems else None
         out = torch.zeros(max(batch.out_elems, 1), dtype=torch.float32, device=device)
         resample(src0, src1, mid, batch.stages, out, handle)
-        if batch.reverb_cuts is not None:
+        if batch.reverb_cuts is not None or batch.reverb_mid_cuts is not None:
             if batch.generated is not None and rir32 is None:
                 rir32 = _generate_rirs(batch.generated, device, handle)
-            _reverb_with(batch, src0, src1, mid, out, handle, rir32)
+            if batch.reverb_cuts is not None:
+                _reverb_with(batch, src0, src1, mid, out, handle, rir32)
+            if batch.reverb_mid_cuts is not None:
+                _reverb_with(batch, src0, src1, mid, mid, handle, rir32, batch.reverb_mid_cuts)
+        for w, table in batch.wpe:
+            wpe(mid, table, out, taps=w.taps, delay=w.delay, iterations=w.iterations, statistics_mode=w.statistics_mode,
+                handle=handle)
         if ring is not None:
             ring.mark_in_flight(device)
     return out, batch.lens, batch.offsets
 
 
 def transform_cuts(cuts, device="cuda", executor=None, ring: Optional[TransformStagingRing] = None,
-                   reverb: bool = False, generated_rir: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
+                   reverb: bool = False, generated_rir: bool = False,
+                   wpe: bool = False) -> Tuple[torch.Tensor, List[int], List[int]]:
     """Loads speed-perturbed, volume-perturbed and resampled cuts (and plain 16-bit WAV / FLAC slices) with the transforms run
     on the GPU: (float32 device tensor holding every cut's samples at its offset, on 4-sample boundaries, lengths, offsets),
     each cut bit-identical to float32(cut.load_audio()).  Raises ValueError naming the first cut the route cannot take.
     `reverb=True` also takes chains that end in a ReverbWithImpulseResponse with a recorded RIR, reverberated on the GPU
     within a float32 tolerance of a float64 convolution (see `transform_request_for_cut`; off by default).
     `generated_rir=True` takes such chains whose RIR lhotse generates, drawn here from the cuts' generators (rir_draws.py;
-    off by default)."""
-    reqs = _requests_or_raise(cuts, lambda c: _transform_or_plain_request(c, reverb, generated_rir),
+    off by default).  `wpe=True` takes chains that end in lhotse's DereverbWPE, dereverberated on the GPU within a float32
+    tolerance of a float64 restatement (see `transform_request_for_cut`; off by default)."""
+    reqs = _requests_or_raise(cuts, lambda c: _transform_or_plain_request(c, reverb, generated_rir, wpe),
                               "cannot be loaded on the GPU (see transform_request_for_cut)")
     ring = ring or TransformStagingRing()
     batch, _, _, _ = ring.stage(reqs, executor=executor)
@@ -1557,19 +1649,19 @@ STAGED_ROUTES = ("pcm16", "flac", "mix", "transform")
 
 
 def staged_route(cuts, perturbed_tracks: bool = False, reverb: bool = False,
-                 generated_rir: bool = False) -> Optional[Tuple[str, list]]:
+                 generated_rir: bool = False, wpe: bool = False) -> Optional[Tuple[str, list]]:
     """(route, requests) of the staged route that takes the batch, the route one of STAGED_ROUTES; None when the cuts have
     more than one sampling rate or no staged route takes them.  A batch with a MixedCut can only go to "mix", else one with
     recording transforms only to "transform"; a batch of plain slices goes to "pcm16" when they are all WAV, to "flac" when
     they are all FLAC.  `perturbed_tracks`, `reverb` and `generated_rir`: see `mix_request_for_cut` and
-    `transform_request_for_cut`."""
+    `transform_request_for_cut`; `wpe`: see `transform_request_for_cut` (the "transform" route only)."""
     if len({c.sampling_rate for c in cuts}) != 1:
         return None
     if any(getattr(c, "tracks", None) is not None for c in cuts):
         route, reqs = "mix", mix_requests_for_batch(cuts, perturbed_tracks=perturbed_tracks, reverb=reverb,
                                                     generated_rir=generated_rir)
     elif any(_has_transforms(c) for c in cuts):
-        route, reqs = "transform", transform_requests_for_batch(cuts, reverb=reverb, generated_rir=generated_rir)
+        route, reqs = "transform", transform_requests_for_batch(cuts, reverb=reverb, generated_rir=generated_rir, wpe=wpe)
     else:
         reqs = [slice_request_for_cut(c) for c in cuts]
         route = {PcmRequest: "pcm16", FlacRequest: "flac"}.get(type(reqs[0]))

@@ -228,6 +228,7 @@ def compute_and_store_features_fused(
     perturbed_tracks: bool = False,
     reverb: bool = False,
     generated_rir: bool = False,
+    wpe: bool = False,
 ):
     """`CutSet.compute_and_store_features_batch(extractor, storage_path, manifest_path, batch_duration, num_workers,
     overwrite=...)` (lhotse/cut/set.py:2197-2408) with the batch kept whole from the GPU to the disk: one packed
@@ -244,7 +245,9 @@ def compute_and_store_features_fused(
     with a recorded RIR (`pcm_staging.transform_request_for_cut`, `mix_request_for_cut`); off by default because those
     samples match the float route within a float32 tolerance, not bit for bit (the float route's own convolution is not
     bit-reproducible), until H100 measurements of it decide the default.  `generated_rir=True` does the same for cuts whose
-    RIR lhotse generates (`pcm_staging.reverb_request`, DESIGN.md §3.1l); off by default for the same reason."""
+    RIR lhotse generates (`pcm_staging.reverb_request`, DESIGN.md §3.1l); off by default for the same reason.  `wpe=True`
+    lets the "transform" stage also take cuts whose chain ends in lhotse's DereverbWPE (`pcm_staging.wpe_request`, DESIGN.md
+    §3.1q); off by default because those samples match the float route within a float32 tolerance, not bit for bit."""
     import json
     import queue
     import threading
@@ -328,7 +331,8 @@ def compute_and_store_features_fused(
             sr = batch_cuts[0].sampling_rate
             assert all(c.sampling_rate == sr for c in batch_cuts)
             item = None
-            chosen = (staged_route(batch_cuts, perturbed_tracks=perturbed_tracks, reverb=reverb, generated_rir=generated_rir)
+            chosen = (staged_route(batch_cuts, perturbed_tracks=perturbed_tracks, reverb=reverb, generated_rir=generated_rir,
+                                   wpe=wpe)
                       if use_ring else None)
             if chosen is not None:
                 kind, reqs = chosen
